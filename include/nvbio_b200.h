@@ -428,6 +428,42 @@ int nvb_seed_extend_traceback(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     const nvb_best_alignment_out* best_alignment,
                     void* d_temp, size_t* temp_bytes, void* stream);
 
+/* Second-best distinct alignment and mapping quality of every read (single end; what nvBowtie's score_reduce_kernel and BowtieMapq2
+ * produce, nvBowtie/bowtie2/cuda/reduce_inl.h:73-152, mapq.h:142-331).  The candidates of read r are the alignments the call scores:
+ * its distinct (strand, window) jobs, or every kept hit when per-hit outputs are requested; each has a score s, a strand t, an end p
+ * (window begin + sink.x, like d_best_pos) and a tie index (its first hit).  A candidate is distinct from the best alignment (strand bt,
+ * end bp) when t != bt or p lies outside [bp - min(bp, len/2), bp + len/2] (len = the read's length; io::distinct_alignments).
+ * The second best is the distinct candidate with s >= d_min_score[len] and the largest s, ties to the smallest tie index -- one answer
+ * whatever the job order, path or de-duplication (nvBowtie's order-dependent hit-by-hit reduction can differ, see DESIGN.md).
+ *   d_second_score[r]   INT_MIN when there is none;  d_second_pos[r]  its end, 0xFFFFFFFF when none;  d_second_strand[r]  0 when none
+ *   d_mapq[r]           BowtieMapq2 of an unpaired read with perfect_score(len) = len * match_bonus, min_score(len) = d_min_score[len]
+ *                       and the end-to-end (monotone) branch when match_bonus == 0; 0 for reads without an alignment
+ * d_min_score is the caller's --score-min evaluated on the host for every length 0 .. max_read_len (nvbio_b200.MapqParams does it
+ * for nvBowtie's SimpleFunc).  Call with the same arguments as nvb_seed_extend_traceback; best_alignment may be NULL.  The best
+ * alignment outputs are those of nvb_seed_extend.  Returns NVB_E_INVALID when mapq, mapq_out, d_min_score, d_second_score or d_mapq
+ * is NULL, or max_read_len < reads->length; the temp size grows by 8 bytes per read. */
+typedef struct nvb_mapq_params {
+    const int32_t* d_min_score;   /* device, [max_read_len + 1]: minimum valid score of a read of each length (host-evaluated --score-min) */
+    uint32_t       max_read_len;
+    int32_t        match_bonus;   /* perfect_score(len) = len * match_bonus; 0 = end-to-end scheme (BowtieMapq2's monotone branch) */
+} nvb_mapq_params;
+typedef struct nvb_mapq_out {
+    int32_t*  d_second_score;     /* [n_reads], required */
+    uint32_t* d_second_pos;       /* [n_reads], may be NULL */
+    uint8_t*  d_second_strand;    /* [n_reads], may be NULL */
+    uint8_t*  d_mapq;             /* [n_reads], required */
+} nvb_mapq_out;
+
+int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_reads,
+                    const nvb_seed_extend_params* params, uint32_t hit_capacity,
+                    int32_t* d_best_score, uint32_t* d_best_pos,
+                    uint32_t* d_n_hits, uint32_t* d_hit_read, nvb_uint2* d_hit_window,
+                    int32_t* d_hit_score, nvb_uint2* d_hit_sink,
+                    const nvb_best_alignment_out* best_alignment,
+                    const nvb_mapq_params* mapq, const nvb_mapq_out* mapq_out,
+                    void* d_temp, size_t* temp_bytes, void* stream);
+
 /* -------------------------------------------------------------------------------------------
  * Paired-end composition (BASELINE configs[4] shape; nvBowtie best_approx paired: anchor scoring + opposite-mate full DP,
  * nvBowtie/bowtie2/cuda/aligner_best_approx_paired.h, score_opposite_inl.h:90-266, alignment_utils.h:62-95 PE_POLICY_FR).
@@ -516,8 +552,8 @@ void nvb_pipeline_destroy(nvb_pipeline* p);
 
 /* Profiling aid (the reference wraps every stage in cuda::Timer, nvBowtie/bowtie2/cuda/aligner_best_approx.h:
  * 219-241): device time in ms of the seven stages of the most recent nvb_seed_extend call -- [fw,rc] strings,
- * seed match (FM-index), hit slots, locate + windows, job de-duplication, banded extension, best-per-read.
- * Synchronises on the call's last event. */
+ * seed match (FM-index), hit slots, locate + windows, job de-duplication, banded extension, best-per-read (which includes the
+ * traceback and, in nvb_seed_extend_mapq, the second-best pass and the MAPQ).  Synchronises on the call's last event. */
 int nvb_seed_extend_stage_ms(float ms[7]);
 
 #ifdef __cplusplus

@@ -3,6 +3,7 @@
  * compare them; none of them changes a result.  Process-wide, not thread-safe. */
 #ifndef NVBIO_B200_DEBUG_H
 #define NVBIO_B200_DEBUG_H
+#include <stdint.h>
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -36,6 +37,12 @@ void nvb_debug_seed_split(int on);
    diagonal gets score = match * len and its sink without running the DP (exact: nothing can score more), 0 = every job through the
    DP kernels.  Same results; for A/B timing and tests */
 void nvb_debug_perfect_shortcut(int on);
+
+/* the device build of the MAPQ function of nvb_seed_extend_mapq over n points (device arrays): d_mapq[i] = BowtieMapq2 of an unpaired
+   read with best score d_best[i], a second score d_second[i] when d_has_second[i] != 0, perfect_score = d_len[i] * d_match_bonus[i],
+   min_score = d_min_score[i] and the monotone branch when d_match_bonus[i] == 0.  For tests: it changes no state */
+int nvb_debug_mapq_eval(const int32_t* d_best, const uint8_t* d_has_second, const int32_t* d_second, const uint32_t* d_len,
+                        const int32_t* d_match_bonus, const int32_t* d_min_score, uint32_t n, uint8_t* d_mapq, void* stream);
 
 #ifdef __cplusplus
 }

@@ -8,4 +8,4 @@ from .fmindex import (FMIndexDevice, FMIndexFilterDevice, rank, rank4, match, ma
                       MAP_EXACT, MAP_APPROX, dict_rank, dict_build_occ,
                       MATCH_FORWARD_ORDER, MATCH_COMPLEMENT)
 from . import aln                                                                # noqa: F401
-from .pipeline import SeedExtendParams, seed_extend, StreamingSeedExtend, PairParams, seed_extend_paired     # noqa: F401
+from .pipeline import SeedExtendParams, seed_extend, StreamingSeedExtend, PairParams, seed_extend_paired, MapqParams     # noqa: F401

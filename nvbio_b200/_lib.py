@@ -10,7 +10,7 @@ EXPORTS = [
     "nvb_version", "nvb_error_string",
     "nvb_fm_rank", "nvb_fm_rank4", "nvb_fm_match", "nvb_fm_match_approx", "nvb_fm_locate", "nvb_fm_filter_rank", "nvb_fm_filter_locate",
     "nvb_banded_gotoh_score", "nvb_banded_gotoh_score_indirect", "nvb_banded_gotoh_traceback", "nvb_gotoh_score", "nvb_gotoh_score_indirect", "nvb_banded_gotoh_score_window", "nvb_banded_gotoh_score_best2", "nvb_gotoh_traceback", "nvb_seed_extend_paired",
-    "nvb_fm_build_occ", "nvb_fm_build_bwt", "nvb_fm_build_ktab", "nvb_fm_build_ktab_located", "nvb_fm_build_ktab_context", "nvb_seed_extend", "nvb_seed_extend_traceback", "nvb_seed_extend_stage_ms",
+    "nvb_fm_build_occ", "nvb_fm_build_bwt", "nvb_fm_build_ktab", "nvb_fm_build_ktab_located", "nvb_fm_build_ktab_context", "nvb_seed_extend", "nvb_seed_extend_traceback", "nvb_seed_extend_mapq", "nvb_seed_extend_stage_ms",
     "nvb_dict_rank", "nvb_dict_rank4", "nvb_dict_build_occ",
     "nvb_map_seeds", "nvb_fm_locate_init", "nvb_fm_locate_lookup", "nvb_fm_locate_sorted",
     "nvb_pipeline_create", "nvb_pipeline_submit", "nvb_pipeline_wait", "nvb_pipeline_traffic", "nvb_pipeline_destroy",
@@ -48,6 +48,14 @@ class SeedExtendParamsStruct(C.Structure):  # nvb_seed_extend_params
 class BestAlignmentOutStruct(C.Structure):   # nvb_best_alignment_out
     _fields_ = [("d_ops", C.c_void_p), ("max_ops", C.c_uint32), ("d_n_ops", C.c_void_p), ("d_begin", C.c_void_p),
                 ("d_strand", C.c_void_p)]
+
+
+class MapqParamsStruct(C.Structure):       # nvb_mapq_params
+    _fields_ = [("d_min_score", C.c_void_p), ("max_read_len", C.c_uint32), ("match_bonus", C.c_int32)]
+
+
+class MapqOutStruct(C.Structure):          # nvb_mapq_out
+    _fields_ = [("d_second_score", C.c_void_p), ("d_second_pos", C.c_void_p), ("d_second_strand", C.c_void_p), ("d_mapq", C.c_void_p)]
 
 
 class PairParamsStruct(C.Structure):        # nvb_pair_params

@@ -568,6 +568,84 @@ pipe_export_hits_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, c
 }
 
 // ---------------------------------------------------------------------------------------------
+// second-best distinct alignment and MAPQ (nvb_seed_extend_mapq).  The candidates are the scored alignments of a read: the per-read
+// path's distinct jobs (tie index: the job's first hit) or the per-hit path's kept hits (tie index: the hit).  Both paths see the
+// same (score, strand, end, smallest index) set, so the result does not depend on the path, the job order or the de-duplication.
+// ---------------------------------------------------------------------------------------------
+
+// a candidate competes for the second-best alignment when it reaches the read's min score and is distinct from the best alignment
+__device__ __forceinline__ bool second_candidate(int32_t score, uint32_t end, uint32_t strand, uint32_t len, uint32_t best_end,
+                                                 uint32_t best_strand, const int32_t* __restrict__ min_score)
+{
+    return score >= min_score[len] && distinct_alignment(end, strand, best_end, best_strand, len);
+}
+
+// best qualifying candidate per read (64-bit atomicMax of make_best_key); the count lives on the device: resident grid striding over it.
+// index == NULL: the candidate's own index is its tie index (per-hit path)
+__global__ void __launch_bounds__(256)
+pipe_second_reduce_kernel(const PipeGeom g, const uint32_t* __restrict__ count, const uint32_t* __restrict__ c_string,
+                          const uint32_t* __restrict__ index, const uint32_t* __restrict__ t_off, const int32_t* __restrict__ score,
+                          const uint2* __restrict__ sink, const uint32_t* __restrict__ str_len, const uint32_t* __restrict__ best_pos,
+                          const uint8_t* __restrict__ best_strand, const int32_t* __restrict__ min_score,
+                          unsigned long long* __restrict__ second_key)
+{
+    const uint32_t n = *count;
+    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
+        const uint32_t s = c_string[j], read = s / g.strands;
+        const int32_t sc = score[j];
+        if (second_candidate(sc, t_off[j] + sink[j].x, s % g.strands, str_len[s], best_pos[read], best_strand[read], min_score))
+            atomicMax(second_key + read, make_best_key(sc, index ? index[j] : j));
+    }
+}
+
+// the winning candidate of every read writes its end and strand (tie indices are unique, so exactly one candidate matches the key)
+__global__ void __launch_bounds__(256)
+pipe_second_finalize_kernel(const PipeGeom g, const uint32_t* __restrict__ count, const uint32_t* __restrict__ c_string,
+                            const uint32_t* __restrict__ index, const uint32_t* __restrict__ t_off, const int32_t* __restrict__ score,
+                            const uint2* __restrict__ sink, const unsigned long long* __restrict__ second_key,
+                            uint32_t* __restrict__ second_pos, uint8_t* __restrict__ second_strand)
+{
+    const uint32_t n = *count;
+    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
+        const uint32_t s = c_string[j], read = s / g.strands;
+        if (second_key[read] != make_best_key(score[j], index ? index[j] : j)) continue;
+        if (second_pos) second_pos[read] = t_off[j] + sink[j].x;
+        if (second_strand) second_strand[read] = (uint8_t)(s % g.strands);
+    }
+}
+
+// one thread per read: the second score (INT_MIN / 0xFFFFFFFF / strand 0 when there is none) and BowtieMapq2
+__global__ void __launch_bounds__(256)
+pipe_mapq_kernel(const PipeGeom g, const nvb_mapq_params mp, const uint32_t* __restrict__ str_len, const int32_t* __restrict__ best_score,
+                 const unsigned long long* __restrict__ second_key, int32_t* __restrict__ second_score, uint32_t* __restrict__ second_pos,
+                 uint8_t* __restrict__ second_strand, uint8_t* __restrict__ mapq)
+{
+    const uint32_t r = blockIdx.x * 256 + threadIdx.x;
+    if (r >= g.n_reads) return;
+    const unsigned long long key = second_key[r];
+    const bool has = key != 0ull;
+    const int32_t s2 = has ? best_key_score(key) : INT_MIN;
+    second_score[r] = s2;
+    if (!has) {
+        if (second_pos) second_pos[r] = 0xFFFFFFFFu;
+        if (second_strand) second_strand[r] = 0;
+    }
+    const uint32_t len = str_len[r * g.strands];
+    mapq[r] = (uint8_t)bowtie_mapq2(best_score[r], has, s2, (int32_t)len * mp.match_bonus, mp.d_min_score[len], mp.match_bonus == 0);
+}
+
+// nvb_debug_mapq_eval: bowtie_mapq2 over arrays
+__global__ void __launch_bounds__(256)
+debug_mapq_eval_kernel(const int32_t* __restrict__ best, const uint8_t* __restrict__ has_second, const int32_t* __restrict__ second,
+                       const uint32_t* __restrict__ len, const int32_t* __restrict__ match_bonus, const int32_t* __restrict__ min_score,
+                       uint32_t n, uint8_t* __restrict__ mapq)
+{
+    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    mapq[i] = (uint8_t)bowtie_mapq2(best[i], has_second[i] != 0, second[i], (int32_t)len[i] * match_bonus[i], min_score[i], match_bonus[i] == 0);
+}
+
+// ---------------------------------------------------------------------------------------------
 // paired-end stage (see nvb_seed_extend_paired in the header for the rules)
 // ---------------------------------------------------------------------------------------------
 struct MateBest { bool has; int32_t score; uint32_t strand, beg, end, len; };
@@ -734,6 +812,7 @@ struct PipeCall {
     bool dedup, per_read, eligible;                                         // eligible: the exact shortcut applies (pipe_perfect_jobs_kernel)
     int32_t* best_score; uint32_t* best_pos; int32_t* hit_score; nvb_uint2* hit_sink;   // the caller's outputs (per-hit ones may be NULL)
     const nvb_best_alignment_out* BA; const nvb_pair_params* PP; const nvb_pair_out* PO;
+    const nvb_mapq_params* MP; const nvb_mapq_out* MO;
     StageEvents* SE;
     uint32_t *str_words, *str_len; uint8_t* str_quals;                      // [fw, rc] strings
     uint2* ranges; uint32_t *sizes, *excl, *counts, *seed_todo_n;           // counts: [0] hits kept, [1] hits found, [2] alignment jobs
@@ -747,6 +826,7 @@ struct PipeCall {
     Jobs best; int32_t* b_score; uint2 *b_sink, *b_source; char* tb_tmp; size_t tb_bytes;      // best-alignment traceback
     uint32_t *pw_want, *pw_idx, *pw_pstr, *pw_toff, *pw_tlen, *pcounts;     // paired: two opposite-mate job slots per pair
     Jobs rescue; int32_t* rs_score; uint2* rs_sink; char *pscan_tmp, *full_tmp; size_t pscan_bytes, full_bytes;
+    unsigned long long* second_key;                                         // second-best alignment of every read (MO)
 
     int stage(int i) const { return (int)cudaEventRecord(SE->ev[i], s); }    // boundary i of nvb_seed_extend_stage_ms
 
@@ -819,6 +899,7 @@ struct PipeCall {
                                                        nullptr, &full_bytes, s)));
             full_tmp = tc.take<char>(full_bytes);
         }
+        if (MO) second_key = tc.take<unsigned long long>(n_reads);
         need = tc.total();
         return NVB_OK;
     }
@@ -952,6 +1033,32 @@ struct PipeCall {
         return launched();
     }
 
+    // second-best distinct alignment and MAPQ of every read: one more pass over the candidates the extension scored (the per-read path's
+    // jobs, tie index = their first hit; the per-hit path's kept hits), after the best alignment is known
+    int second_best() const
+    {
+        const uint32_t cap = hit_capacity, hgrid = (cap + 255) / 256;
+        NVB_CUDA_TRY(cudaMemsetAsync(second_key, 0, sizeof(unsigned long long) * g.n_reads, s));
+        if (cap) {
+            const uint32_t* n   = per_read ? counts + 2 : counts;
+            const uint32_t* cs  = per_read ? j_string : hit_string;
+            const uint32_t* idx = per_read ? j_first : nullptr;
+            const uint32_t* to  = per_read ? jobs.t_off : hits.t_off;
+            const int32_t* sc   = per_read ? job_score : h_score;
+            const uint2* sk     = per_read ? job_sink : h_sink;
+            const uint32_t grid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
+            pipe_second_reduce_kernel<<<grid, 256, 0, s>>>(g, n, cs, idx, to, sc, sk, str_len, best_pos, rb_strand, MP->d_min_score, second_key);
+            NVB_LAUNCH_CHECK();
+            if (MO->d_second_pos || MO->d_second_strand) {
+                pipe_second_finalize_kernel<<<grid, 256, 0, s>>>(g, n, cs, idx, to, sc, sk, second_key, MO->d_second_pos, MO->d_second_strand);
+                NVB_LAUNCH_CHECK();
+            }
+        }
+        pipe_mapq_kernel<<<(g.n_reads + 255) / 256, 256, 0, s>>>(g, *MP, str_len, best_score, second_key, MO->d_second_score, MO->d_second_pos,
+                                                                MO->d_second_strand, MO->d_mapq);
+        return launched();
+    }
+
     // paired-end rescue: non-concordant pairs get opposite-mate jobs (scan-compacted) for the full-matrix DP; the best rescue wins
     int paired_rescue() const
     {
@@ -988,6 +1095,7 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     int32_t* d_hit_score, nvb_uint2* d_hit_sink,
                     const nvb_best_alignment_out* BA,
                     const nvb_pair_params* PP, const nvb_pair_out* PO,
+                    const nvb_mapq_params* MP, const nvb_mapq_out* MO,
                     void* d_temp, size_t* temp_bytes, void* stream)
 {
     if (PP) {
@@ -1019,7 +1127,7 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
 
     const cudaStream_t s = c.s = as_stream(stream);
     c.P = P; c.f = make_fmindex(fmi); c.rd = make_strset(reads); c.genome = d_genome; c.nq = (uint32_t)nq64; c.hit_capacity = hit_capacity;
-    c.best_score = d_best_score; c.best_pos = d_best_pos; c.hit_score = d_hit_score; c.hit_sink = d_hit_sink; c.BA = BA; c.PP = PP; c.PO = PO;
+    c.best_score = d_best_score; c.best_pos = d_best_pos; c.hit_score = d_hit_score; c.hit_sink = d_hit_sink; c.BA = BA; c.PP = PP; c.PO = PO; c.MP = MP; c.MO = MO;
     c.dedup = P->dedup_jobs != 0;
     // per-read path: nobody asked for per-hit outputs, so no per-hit array needs to exist
     c.per_read = c.dedup && g_pipe_path != 1 && !d_hit_read && !d_hit_window && !d_hit_score && !d_hit_sink && !BA;
@@ -1047,6 +1155,7 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     }
     if (BA) NVB_TRY(c.best_traceback());
     if (PP) NVB_TRY(c.paired_rescue());
+    if (MO) NVB_TRY(c.second_best());
     if (!c.dedup) NVB_CUDA_TRY(cudaMemcpyAsync(c.counts + 2, c.counts, sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
     if (d_n_hits) NVB_CUDA_TRY(cudaMemcpyAsync(d_n_hits, c.counts, 3 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
     NVB_TRY(c.stage(7));
@@ -1067,7 +1176,7 @@ extern "C" int nvb_seed_extend(const nvb_fm_index* fmi, const uint32_t* d_genome
                     void* d_temp, size_t* temp_bytes, void* stream)
 {
     return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
-                            d_hit_score, d_hit_sink, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
+                            d_hit_score, d_hit_sink, nullptr, nullptr, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_traceback(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1081,7 +1190,7 @@ extern "C" int nvb_seed_extend_traceback(const nvb_fm_index* fmi, const uint32_t
 {
     if (!best_alignment) return NVB_E_INVALID;
     return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
-                            d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, d_temp, temp_bytes, stream);
+                            d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1093,5 +1202,30 @@ extern "C" int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d
     if (!pair_params || !out || n_pairs > 0x3FFFFFFFu || !temp_bytes) return NVB_E_INVALID;
     // the per-read best (score, end) of the single-end stage lands in the mate arrays first and is then refined per pair
     return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
-                            nullptr, nullptr, nullptr, pair_params, out, d_temp, temp_bytes, stream);
+                            nullptr, nullptr, nullptr, pair_params, out, nullptr, nullptr, d_temp, temp_bytes, stream);
+}
+
+extern "C" int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_reads,
+                    const nvb_seed_extend_params* P, uint32_t hit_capacity,
+                    int32_t* d_best_score, uint32_t* d_best_pos,
+                    uint32_t* d_n_hits, uint32_t* d_hit_read, nvb_uint2* d_hit_window,
+                    int32_t* d_hit_score, nvb_uint2* d_hit_sink,
+                    const nvb_best_alignment_out* best_alignment,
+                    const nvb_mapq_params* mapq, const nvb_mapq_out* mapq_out,
+                    void* d_temp, size_t* temp_bytes, void* stream)
+{
+    if (!mapq || !mapq_out || !mapq->d_min_score || !mapq_out->d_second_score || !mapq_out->d_mapq) return NVB_E_INVALID;
+    if (!reads || mapq->max_read_len < reads->length) return NVB_E_INVALID;           // the min-score table must cover every read length
+    return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
+                            d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, mapq, mapq_out, d_temp, temp_bytes, stream);
+}
+
+extern "C" int nvb_debug_mapq_eval(const int32_t* d_best, const uint8_t* d_has_second, const int32_t* d_second, const uint32_t* d_len,
+                                   const int32_t* d_match_bonus, const int32_t* d_min_score, uint32_t n, uint8_t* d_mapq, void* stream)
+{
+    if (!n) return NVB_OK;
+    if (!d_best || !d_has_second || !d_second || !d_len || !d_match_bonus || !d_min_score || !d_mapq) return NVB_E_INVALID;
+    debug_mapq_eval_kernel<<<(n + 255) / 256, 256, 0, as_stream(stream)>>>(d_best, d_has_second, d_second, d_len, d_match_bonus, d_min_score, n, d_mapq);
+    return launched();
 }

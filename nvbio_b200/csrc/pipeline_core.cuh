@@ -1,5 +1,5 @@
 // pipeline_core.cuh -- per-thread routines of the seed + extend composition that tests also run on the host
-// (tests/host/host_harness.cu), like fm_core.cuh / gotoh_core.cuh.
+// (tests/host/host_harness.cu, tests/host/mapq_harness.cu), like fm_core.cuh / gotoh_core.cuh.
 #pragma once
 #include "fm_core.cuh"
 
@@ -100,6 +100,73 @@ __host__ __device__ inline bool gapless_job_shortcut(const uint32_t* __restrict_
     if (perfect) { sink_x = M + jtop; sink_y = M; }
     else         { sink_x = end + j0; sink_y = end; }
     return true;
+}
+
+// Alignment ending at p on strand t is distinct from the best one (bp, bt) of a read of length len: another strand, or an end more than
+// len/2 away (nvbio io::distinct_alignments, alignments_inl.h:35-47, in the same unsigned arithmetic)
+__host__ __device__ __forceinline__ bool distinct_alignment(uint32_t p, uint32_t t, uint32_t bp, uint32_t bt, uint32_t len)
+{
+    const uint32_t d = len / 2u;
+    return t != bt || p < bp - (bp < d ? bp : d) || p > bp + d;
+}
+
+// Mapping quality of an unpaired read: nvBowtie's BowtieMapq2 (mapq.h:155-327) for a scheme with perfect_score(len) = perfect,
+// min_score(len) = min_score and m_monotone = monotone (match bonus 0, end-to-end).  The same float operations in the same order (only
+// multiplies, subtractions, fabsf and compares: nothing the compiler could contract into an FMA), so host and device agree bit for bit.
+// A read without an alignment (best = INT_MIN) is below any min_score > INT_MIN and gets 0.
+__host__ __device__ inline uint32_t bowtie_mapq2(int32_t best_score, bool has_second, int32_t second_score, int32_t perfect, int32_t min_score,
+                                                 bool monotone)
+{
+    const float max_s = (float)perfect, min_s = (float)min_score;
+    const float diff = max_s - min_s;
+    const float best = (float)best_score;
+    if (best < min_s) return 0;
+    const float best_over = best - min_s;
+    const bool top = best_over == diff;
+    if (monotone) {                                             // end-to-end
+        if (!has_second) {
+            if      (best_over >= diff * 0.8f) return 42;
+            else if (best_over >= diff * 0.7f) return 40;
+            else if (best_over >= diff * 0.6f) return 24;
+            else if (best_over >= diff * 0.5f) return 23;
+            else if (best_over >= diff * 0.4f) return 8;
+            else if (best_over >= diff * 0.3f) return 3;
+            return 0;
+        }
+        const float best_diff = fabsf(fabsf(best) - fabsf((float)second_score));
+        if      (best_diff >= diff * 0.9f) return top ? 39 : 33;
+        else if (best_diff >= diff * 0.8f) return top ? 38 : 27;
+        else if (best_diff >= diff * 0.7f) return top ? 37 : 26;
+        else if (best_diff >= diff * 0.6f) return top ? 36 : 22;
+        else if (best_diff >= diff * 0.5f) return top ? 35 : best_over >= diff * 0.84f ? 25 : best_over >= diff * 0.68f ? 16 : 5;
+        else if (best_diff >= diff * 0.4f) return top ? 34 : best_over >= diff * 0.84f ? 21 : best_over >= diff * 0.68f ? 14 : 4;
+        else if (best_diff >= diff * 0.3f) return top ? 32 : best_over >= diff * 0.88f ? 18 : best_over >= diff * 0.67f ? 15 : 3;
+        else if (best_diff >= diff * 0.2f) return top ? 31 : best_over >= diff * 0.88f ? 17 : best_over >= diff * 0.67f ? 11 : 0;
+        else if (best_diff >= diff * 0.1f) return top ? 30 : best_over >= diff * 0.88f ? 12 : best_over >= diff * 0.67f ? 7 : 0;
+        else if (best_diff > 0.0f)         return best_over >= diff * 0.67f ? 6 : 2;
+        return best_over >= diff * 0.67f ? 1 : 0;
+    }
+    if (!has_second) {                                          // local
+        if      (best_over >= diff * 0.8f) return 44;
+        else if (best_over >= diff * 0.7f) return 42;
+        else if (best_over >= diff * 0.6f) return 41;
+        else if (best_over >= diff * 0.5f) return 36;
+        else if (best_over >= diff * 0.4f) return 28;
+        else if (best_over >= diff * 0.3f) return 24;
+        return 22;
+    }
+    const float best_diff = fabsf(fabsf(best) - fabsf((float)second_score));
+    if      (best_diff >= diff * 0.9f) return 40;
+    else if (best_diff >= diff * 0.8f) return 39;
+    else if (best_diff >= diff * 0.7f) return 38;
+    else if (best_diff >= diff * 0.6f) return 37;
+    else if (best_diff >= diff * 0.5f) return top ? 35 : best_over >= diff * 0.5f ? 25 : 20;
+    else if (best_diff >= diff * 0.4f) return top ? 34 : best_over >= diff * 0.5f ? 21 : 19;
+    else if (best_diff >= diff * 0.3f) return top ? 33 : best_over >= diff * 0.5f ? 18 : 16;
+    else if (best_diff >= diff * 0.2f) return top ? 32 : best_over >= diff * 0.5f ? 17 : 12;
+    else if (best_diff >= diff * 0.1f) return top ? 31 : best_over >= diff * 0.5f ? 14 : 9;
+    else if (best_diff > 0.0f)         return best_over >= diff * 0.5f ? 11 : 2;
+    return best_over >= diff * 0.5f ? 1 : 0;
 }
 
 } // namespace nvb

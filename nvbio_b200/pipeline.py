@@ -1,9 +1,11 @@
 """Seed + extend composition (examples/fmmap/fmmap.cu:255-400 shaped) over the C ABI."""
 import ctypes as C
+import ctypes.util
 from dataclasses import dataclass, field
 from typing import Optional
 import torch
-from ._lib import lib, check, SeedExtendParamsStruct, BestAlignmentOutStruct, PairParamsStruct, PairOutStruct
+import numpy as np
+from ._lib import lib, check, SeedExtendParamsStruct, BestAlignmentOutStruct, PairParamsStruct, PairOutStruct, MapqParamsStruct, MapqOutStruct
 from .strings import PackedStringSet
 from .fmindex import FMIndexDevice
 from . import aln
@@ -32,11 +34,77 @@ class SeedExtendParams:
         return p
 
 
+_libm = None
+
+
+def simple_func(kind: str, const: float, coeff: float, x) -> np.ndarray:
+    """nvBowtie's SimpleFunc (nvBowtie/bowtie2/cuda/func.h:39-51), int32(const + coeff * f(float32(x))) with f = x ('L'), logf ('G') or
+    sqrtf ('S'), in float32 like the reference's host code.  logf / sqrtf are the C library's (numpy's float32 log is a vectorised
+    implementation picked by CPU features, so it is not guaranteed to round as the C library does).  Results outside the int32 range
+    (x = 0 under 'G' gives -inf) are clamped to +-(2**31 - 1): INT_MIN stays the score of a read without an alignment."""
+    global _libm
+    if kind not in ("L", "G", "S"):
+        raise ValueError("SimpleFunc type must be 'L', 'G' or 'S', not %r" % (kind,))
+    if kind != "L" and _libm is None:
+        _libm = C.CDLL(ctypes.util.find_library("m"))
+        for f in (_libm.logf, _libm.sqrtf):
+            f.restype, f.argtypes = C.c_float, [C.c_float]
+    k, m = np.float32(const), np.float32(coeff)
+    out = []
+    for v in np.asarray(x, dtype=np.int64).reshape(-1):
+        fx = np.float32(v)
+        if kind == "G":
+            fx = np.float32(_libm.logf(float(fx)))
+        elif kind == "S":
+            fx = np.float32(_libm.sqrtf(float(fx)))
+        with np.errstate(invalid="ignore", over="ignore"):
+            y = k + m * fx
+        if np.isnan(y):
+            raise ValueError("SimpleFunc %s,%g,%g is not a number at x = %d" % (kind, const, coeff, v))
+        out.append(int(max(min(float(y), 2.0 ** 31 - 1), -(2.0 ** 31 - 1))))       # C truncation toward zero
+    return np.array(out, dtype=np.int32)
+
+
+@dataclass
+class MapqParams:
+    """Inputs of the second-best / MAPQ stage (nvb_mapq_params).  min_score: int32 tensor [max_read_len + 1] on the device, the minimum
+    valid score of a read of each length (--score-min evaluated on the host); match_bonus: perfect_score(len) = len * match_bonus,
+    0 = an end-to-end scheme (BowtieMapq2's monotone branch)."""
+    min_score: torch.Tensor
+    match_bonus: int
+
+    @property
+    def max_read_len(self) -> int:
+        return self.min_score.numel() - 1
+
+    @classmethod
+    def from_score_min(cls, kind: str, const: float, coeff: float, max_read_len: int, match_bonus: int, device="cuda") -> "MapqParams":
+        """nvBowtie's --score-min kind,const,coeff (kind 'L' linear, 'G' natural log, 'S' square root) for lengths 0 .. max_read_len"""
+        tab = simple_func(kind, const, coeff, np.arange(max_read_len + 1))
+        return cls(torch.from_numpy(tab).to(device), int(match_bonus))
+
+    @classmethod
+    def local(cls, max_read_len: int, device="cuda") -> "MapqParams":
+        """nvBowtie's --local scheme: match bonus 2, --score-min G,0,10 (scoring_inl.h:81-99)"""
+        return cls.from_score_min("G", 0.0, 10.0, max_read_len, 2, device)
+
+    @classmethod
+    def end_to_end(cls, max_read_len: int, device="cuda") -> "MapqParams":
+        """nvBowtie's end-to-end scheme: no match bonus, --score-min L,-0.6,-0.6 (scoring_inl.h:107-122)"""
+        return cls.from_score_min("L", -0.6, -0.6, max_read_len, 0, device)
+
+    def struct(self) -> MapqParamsStruct:
+        assert self.min_score.dtype == torch.int32 and self.min_score.is_cuda and self.min_score.is_contiguous()
+        p = MapqParamsStruct()
+        p.d_min_score, p.max_read_len, p.match_bonus = self.min_score.data_ptr(), self.max_read_len, self.match_bonus
+        return p
+
+
 class SeedExtendWorkspace:
     """pre-allocated outputs + temp storage for repeated calls on equally-shaped batches"""
 
     def __init__(self, fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStringSet, params: SeedExtendParams,
-                 hit_capacity: int, keep_hits: bool = False, traceback: bool = False):
+                 hit_capacity: int, keep_hits: bool = False, traceback: bool = False, mapq: Optional[MapqParams] = None):
         dev = fmi.device
         n = reads.count
         self.best_score = torch.empty(n, dtype=torch.int32, device=dev)
@@ -57,6 +125,14 @@ class SeedExtendWorkspace:
             self.best_n_ops = torch.zeros(n, dtype=torch.int32, device=dev)
             self.best_begin = torch.empty((n, 2), dtype=torch.int32, device=dev)
             self.best_strand = torch.empty(n, dtype=torch.uint8, device=dev)
+        # optional second-best distinct alignment and MAPQ of every read
+        self.mapq_params = mapq
+        self.second_score = self.second_pos = self.second_strand = self.mapq = None
+        if mapq is not None:
+            self.second_score = torch.empty(n, dtype=torch.int32, device=dev)
+            self.second_pos = torch.empty(n, dtype=torch.int32, device=dev)
+            self.second_strand = torch.empty(n, dtype=torch.uint8, device=dev)
+            self.mapq = torch.empty(n, dtype=torch.uint8, device=dev)
         tb = C.c_size_t(0)
         r = _call(fmi, genome, reads, params, self, None, tb)
         if r != -2:
@@ -71,10 +147,22 @@ def _p(t):
 
 def _call(fmi, genome, reads, params, ws, temp, tb):
     s, rd, ps = fmi.struct(), reads.struct(), params.struct()
+    ba = None
     if ws.best_ops is not None:
         ba = BestAlignmentOutStruct()
         ba.d_ops, ba.max_ops, ba.d_n_ops = ws.best_ops.data_ptr(), ws.max_ops, ws.best_n_ops.data_ptr()
         ba.d_begin, ba.d_strand = ws.best_begin.data_ptr(), ws.best_strand.data_ptr()
+    if ws.mapq is not None:
+        mp = ws.mapq_params.struct()
+        mo = MapqOutStruct()
+        mo.d_second_score, mo.d_second_pos = ws.second_score.data_ptr(), ws.second_pos.data_ptr()
+        mo.d_second_strand, mo.d_mapq = ws.second_strand.data_ptr(), ws.mapq.data_ptr()
+        return lib().nvb_seed_extend_mapq(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(reads.count), C.byref(ps),
+                                          C.c_uint32(ws.hit_capacity), _p(ws.best_score), _p(ws.best_pos), _p(ws.n_hits),
+                                          _p(ws.hit_read), _p(ws.hit_window), _p(ws.hit_score), _p(ws.hit_sink),
+                                          C.byref(ba) if ba is not None else None, C.byref(mp), C.byref(mo),
+                                          _p(temp), C.byref(tb), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+    if ba is not None:
         return lib().nvb_seed_extend_traceback(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(reads.count), C.byref(ps),
                                                C.c_uint32(ws.hit_capacity), _p(ws.best_score), _p(ws.best_pos), _p(ws.n_hits),
                                                _p(ws.hit_read), _p(ws.hit_window), _p(ws.hit_score), _p(ws.hit_sink), C.byref(ba),
@@ -87,14 +175,20 @@ def _call(fmi, genome, reads, params, ws, temp, tb):
 
 def seed_extend(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStringSet, params: SeedExtendParams,
                 workspace: Optional[SeedExtendWorkspace] = None, hit_capacity: Optional[int] = None, keep_hits: bool = False,
-                traceback: bool = False):
+                traceback: bool = False, mapq: Optional[MapqParams] = None):
     """returns the workspace: .best_score[n], .best_pos[n], .n_hits[3] = (kept, total, distinct jobs), optional per-hit
-    arrays, and with traceback=True the alignment of every read's best hit (.best_ops END->START, .best_n_ops,
-    .best_begin = (genome start, read start), .best_strand)"""
+    arrays, with traceback=True the alignment of every read's best hit (.best_ops END->START, .best_n_ops,
+    .best_begin = (genome start, read start), .best_strand), and with mapq=MapqParams(...) the second-best distinct alignment and
+    the mapping quality of every read (.second_score, .second_pos, .second_strand, .mapq; nvb_seed_extend_mapq).  A workspace made
+    with mapq keeps computing them; a new mapq replaces its table for this and later calls"""
     if workspace is None:
         if hit_capacity is None:
             hit_capacity = 32 * reads.count + 1024
-        workspace = SeedExtendWorkspace(fmi, genome, reads, params, hit_capacity, keep_hits, traceback)
+        workspace = SeedExtendWorkspace(fmi, genome, reads, params, hit_capacity, keep_hits, traceback, mapq)
+    elif mapq is not None:
+        if workspace.mapq is None:
+            raise ValueError("seed_extend(mapq=...): the workspace was created without mapq outputs")
+        workspace.mapq_params = mapq
     tb = C.c_size_t(workspace.temp_bytes)
     check(_call(fmi, genome, reads, params, workspace, workspace.temp, tb), "nvb_seed_extend")
     return workspace
