@@ -69,8 +69,12 @@ typedef struct nvb_fm_index {
                                     entry (y == x) holds the 16 text symbols before SA[x] instead, so that such a seed (up to k + 16
                                     symbols long) is resolved by the look-up alone; and, when length < 0xC0000000, a TWO-row entry is
                                     stored as {x, 0xC0000000 | a | b << 14, SA[x], SA[x+1]} (y = x + 1 implied; a, b = the 7 symbols before
-                                    SA[x], SA[x+1]), which resolves seeds up to k + 7 symbols the same way.  Ranges are identical in
-                                    every case.  */
+                                    SA[x], SA[x+1]), which resolves seeds up to k + 7 symbols the same way;  3: as 2, and d_rows is set
+                                    (needs sa_interval == 1 and d_ssa).  Ranges are identical in every case.  */
+    const nvb_uint2* d_rows;     /* read only when ktab_located == 3: length + 1 entries {SA[r], the 16 text symbols before SA[r]}
+                                    built by nvb_fm_build_rows.  The per-read seed + extend path then resolves a seed whose k-mer
+                                    occurs 3 to 8 times (and that is up to k + 16 symbols long) with one gather of those rows instead
+                                    of walking the range on; results are identical with and without it */
 } nvb_fm_index;
 
 /* A set of strings stored in one packed symbol stream (nvbio PackedStream semantics,
@@ -369,6 +373,12 @@ int nvb_fm_build_ktab_located(const nvb_fm_index* fmi, uint32_t k, void* d_ktab1
  * d_text (2-bit big-endian, the text the index was built from) that precede SA[x], symbol SA[x]-1 in the two lowest bits; two-row
  * entries are packed as described at nvb_fm_index.ktab_located.  Use with nvb_fm_index.d_ktab = d_ktab16, ktab_located = 2. */
 int nvb_fm_build_ktab_context(const nvb_fm_index* fmi, uint32_t k, const uint32_t* d_text, void* d_ktab16, void* stream);
+
+/* Per-row array of an index with the full suffix array: d_rows[r] = {SA[r], the (up to) 16 symbols of d_text before SA[r], symbol SA[r]-1
+ * in the two lowest bits} for r in [0, length] ((length + 1) * 8 bytes: 15.2 GB at 1.9 Gbp).  Row 0 (SA = 0xFFFFFFFF) gets context 0,
+ * a row with SA[r] < 16 the SA[r] symbols there are.  Needs fmi->sa_interval == 1 and fmi->d_ssa, else NVB_E_UNSUPPORTED; fmi's table
+ * fields are ignored.  Use with a context table (nvb_fm_build_ktab_context) as nvb_fm_index.d_rows = d_rows, ktab_located = 3. */
+int nvb_fm_build_rows(const nvb_fm_index* fmi, const uint32_t* d_text, nvb_uint2* d_rows, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Seed + extend composition (the fmmap / nvBowtie hot loop: seeds -> match -> locate -> window ->

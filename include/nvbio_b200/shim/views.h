@@ -260,6 +260,7 @@ struct fm_index_view<
         v.d_ktab      = NULL;
         v.ktab_k      = 0u;
         v.ktab_located = 0u;
+        v.d_rows      = NULL;
         cudaPointerAttributes attr;
         const bool on_device = cudaPointerGetAttributes( &attr, f.m_L2 ) == cudaSuccess &&
                                (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);

@@ -29,6 +29,8 @@ struct FmIndex {
     uint32_t ktab_k;
     uint32_t ktab_located;         // 1: table entries are 16 bytes {x, y, SA[x], SA[y]} (SA values filled for ranges of one or two rows; nvb_fm_build_ktab_located)
                                    // 2: the same, and the last word of a ONE-row entry holds the 16 text symbols before SA[x] (nvb_fm_build_ktab_context)
+    const uint2*    rows;          // optional, with a context table: {SA[r], the 16 text symbols before SA[r]} for every row r (nvb_fm_build_rows;
+                                   // nvb_fm_index.ktab_located == 3, which is 2 here plus this array)
     // constant-index selects keep the struct in the kernel-parameter constant bank (a dynamic L2[c]
     // would force a local-memory copy of the whole struct)
     __host__ __device__ __forceinline__ uint32_t l2(uint32_t c) const {
@@ -43,7 +45,8 @@ static inline bool valid_fmindex(const nvb_fm_index* f) {
     if (!f || !f->d_bwt_occ) return false;
     const uint32_t I = f->sa_interval;
     if (I != 0 && (I & (I - 1)) != 0) return false;           // power of two
-    if (f->d_ktab && (f->ktab_k < 1 || f->ktab_k > 16 || f->ktab_located > 2u)) return false;
+    if (f->d_ktab && (f->ktab_k < 1 || f->ktab_k > 16 || f->ktab_located > 3u)) return false;
+    if (f->d_ktab && f->ktab_located == 3u && (f->sa_interval != 1u || !f->d_ssa || !f->d_rows)) return false;
     return true;
 }
 static inline FmIndex make_fmindex(const nvb_fm_index* f) {
@@ -54,7 +57,10 @@ static inline FmIndex make_fmindex(const nvb_fm_index* f) {
     r.sa_shift = 0; while ((1u << r.sa_shift) < I) ++r.sa_shift;
     r.sa_mask = (1u << r.sa_shift) - 1u;
     r.ktab = (const uint2*)f->d_ktab; r.ktab_k = f->d_ktab ? f->ktab_k : 0u;
-    r.ktab_located = f->d_ktab ? f->ktab_located : 0u;
+    // d_rows is read only at level 3: callers that fill the struct field by field and stop at ktab_located leave it undefined
+    const bool with_rows = f->d_ktab && f->ktab_located == 3u;
+    r.ktab_located = f->d_ktab ? (with_rows ? 2u : f->ktab_located) : 0u;
+    r.rows = with_rows ? (const uint2*)f->d_rows : nullptr;
     return r;
 }
 
@@ -331,6 +337,34 @@ __host__ __device__ __forceinline__ uint32_t be4_window(const uint32_t* __restri
     return (squeeze_nibbles(hi) << 16) | squeeze_nibbles(lo);
 }
 
+// Text context words (one-row table entries, two-row entries' 7-symbol halves, the per-row array): the symbols before a text position pos,
+// symbol pos-1 in the lowest two bits.  unread_context() puts the first `rem` (1..16) symbols of a query in the same order (its symbol
+// rem-1 lowest; n_left is set when one of them is an N), and context_matches() tells whether the `cnt` (0..16) of them closest to pos
+// -- the first ones a backward search would consume from the row of pos -- are the symbols before pos (context_equal: the same
+// without the test that there are cnt symbols before pos).
+template <int BITS, bool BE>
+__host__ __device__ __forceinline__ uint32_t unread_context(const uint32_t* __restrict__ words, uint32_t off, uint32_t rem, bool& n_left)
+{
+    if (BITS == 2 && BE) return be2_window(words, off, rem) >> (32u - 2u * rem);
+    if (BITS == 4 && BE) return be4_window(words, off, rem, n_left) >> (32u - 2u * rem);
+    SymReader<BITS, BE> rd(words);
+    uint32_t qw = 0u;
+    for (uint32_t i = 0; i < rem; ++i) { const uint32_t c = rd.get(off + i); n_left |= (c > 3u); qw = (qw << 2) | (c & 3u); }
+    return qw;
+}
+__host__ __device__ __forceinline__ bool context_equal(uint32_t qw, uint32_t ctx, uint32_t cnt)
+{
+    const uint32_t mask = cnt >= 16u ? 0xFFFFFFFFu : ((1u << (2u * cnt)) - 1u);
+    return ((qw ^ ctx) & mask) == 0u;
+}
+__host__ __device__ __forceinline__ bool context_matches(uint32_t qw, uint32_t ctx, uint32_t pos, uint32_t cnt)
+{
+    return pos != 0xFFFFFFFFu && pos >= cnt && context_equal(qw, ctx, cnt);
+}
+
+// the widest k-mer range that the per-row array resolves: its rows are read with one gather each, all issued together
+constexpr uint32_t FM_ROWS_MAX = 8;
+
 // match() + locate() of one query in one pass, for callers that only need the hit POSITIONS of narrow ranges (the per-read
 // seed + extend path): as soon as the range is a single row (x == y) and the index keeps the full suffix array, the remaining
 // LF steps are replaced by one SA gather and a comparison of the not-yet-consumed symbols with the text itself:
@@ -414,18 +448,51 @@ __host__ __device__ __forceinline__ uint32_t fm_match_locate_one(const FmIndex& 
         bool m0, m1;
         if (two_ctx && rem <= 7u) {
             // both candidates' preceding symbols came with the entry: no read of the text
-            uint32_t qw = 0u; bool n_left = false;
-            if (BITS == 2 && BE)      qw = be2_window(words, off, rem) >> (32u - 2u * rem);
-            else if (BITS == 4 && BE) qw = be4_window(words, off, rem, n_left) >> (32u - 2u * rem);
-            else for (uint32_t i = 0; i < rem; ++i) { const uint32_t c = rd.get(off + i); n_left |= (c > 3u); qw = (qw << 2) | (c & 3u); }
-            const uint32_t mask = (1u << (2u * rem)) - 1u;
-            m0 = !n_left && known_pos  != 0xFFFFFFFFu && known_pos  >= rem && ((qw ^ ctx2) & mask) == 0u;
-            m1 = !n_left && known_pos2 != 0xFFFFFFFFu && known_pos2 >= rem && ((qw ^ (ctx2 >> 14)) & mask) == 0u;
+            bool n_left = false;
+            const uint32_t qw = unread_context<BITS, BE>(words, off, rem, n_left);
+            m0 = !n_left && context_matches(qw, ctx2, known_pos, rem);
+            m1 = !n_left && context_matches(qw, ctx2 >> 14, known_pos2, rem);
         } else {
             m0 = prefix_matches(known_pos, rem); m1 = prefix_matches(known_pos2, rem);
         }
         if (!m0 && !m1) return FM_EMPTY;
         if (m0 != m1) { ox = (m0 ? known_pos : known_pos2) - rem; oy = 0xFFFFFFFFu; return FM_LOCATED; }
+    }
+    if (MODE != FM_DEFER && f.rows && full_sa && s == f.ktab_k && s < len && y - x >= 2u && y - x < FM_ROWS_MAX && len - s <= 16u) {
+        // a k-mer with 3..FM_ROWS_MAX occurrences, on an index with the per-row array: the rows' contexts are compared with the unread
+        // symbols instead of walking the range on.  Row r survives the rem remaining LF steps <=> the rem symbols before SA[r] are the
+        // unread ones, and it is still in the range after j steps <=> the j symbols before SA[r] match.  The walk stops at the first
+        // step where one row is left and locates it there; when that happens only after the last step it returns the one-row RANGE
+        // instead.  So: no survivor = empty; one survivor that is also the only row matching the rem - 1 symbols closest to it =
+        // located at SA[r] - rem; anything else (a repeat of the whole query, a range narrowed to one row by its last step, an N
+        // among the unread symbols) takes the walk below, which is unchanged.
+        // Only the context words are gathered first (one register per row in flight, not two), so the position test of
+        // context_matches is left out: that can only add rows (a row with SA[r] < 16 has fewer context symbols), never drop one.
+        // An empty set stays exact, two or more take the walk, and a single survivor's SA[r] -- in the sector just read -- is
+        // checked after.
+        const uint32_t rem = len - s;
+        bool n_left = false;
+        const uint32_t qw = unread_context<BITS, BE>(words, off, rem, n_left);
+        if (!n_left) {
+            const uint32_t* ctx = (const uint32_t*)(f.rows + x) + 1;
+            uint32_t c[FM_ROWS_MAX];
+#pragma unroll
+            for (uint32_t i = 0; i < FM_ROWS_MAX; ++i) c[i] = (i <= y - x) ? gather_u32(ctx + 2u * i) : 0u;
+            uint32_t full = 0u, near = 0u, hit = 0u;
+#pragma unroll
+            for (uint32_t i = 0; i < FM_ROWS_MAX; ++i) {
+                if (i > y - x) continue;
+                if (context_equal(qw, c[i], rem)) { ++full; hit = i; }
+                near += context_equal(qw, c[i], rem - 1u) ? 1u : 0u;
+            }
+            if (full == 0u) return FM_EMPTY;
+            if (full == 1u && near == 1u) {
+                const uint32_t pos = gather_u32((const uint32_t*)(f.rows + x + hit));
+                if (pos == 0xFFFFFFFFu || pos < rem) return FM_EMPTY;
+                ox = pos - rem; oy = 0xFFFFFFFFu;
+                return FM_LOCATED;
+            }
+        }
     }
     if (MODE == FM_DEFER && s < len && x < y) { ox = x; oy = y; return FM_DEFERRED; }
     for (; s < len && x <= y; ++s) {
@@ -436,13 +503,9 @@ __host__ __device__ __forceinline__ uint32_t fm_match_locate_one(const FmIndex& 
             if (have_pos && f.ktab_located == 2u && rem <= 16u) {
                 // the entry also carries the 16 text symbols before SA[x] (symbol SA[x]-1 in the lowest bits): the comparison needs
                 // no read of the text at all -- the look-up was this seed's only gather
-                if (pos == 0xFFFFFFFFu || pos < rem) return FM_EMPTY;
-                uint32_t qw = 0u; bool n_left = false;
-                if (BITS == 2 && BE)      qw = be2_window(words, off, rem) >> (32u - 2u * rem);
-                else if (BITS == 4 && BE) qw = be4_window(words, off, rem, n_left) >> (32u - 2u * rem);
-                else for (uint32_t i = 0; i < rem; ++i) { const uint32_t c = rd.get(off + i); n_left |= (c > 3u); qw = (qw << 2) | (c & 3u); }
-                const uint32_t mask = rem == 16u ? 0xFFFFFFFFu : ((1u << (2u * rem)) - 1u);
-                if (n_left || ((qw ^ known_pos2) & mask) != 0u) return FM_EMPTY;
+                bool n_left = false;
+                const uint32_t qw = unread_context<BITS, BE>(words, off, rem, n_left);
+                if (n_left || !context_matches(qw, known_pos2, pos, rem)) return FM_EMPTY;
                 ox = pos - rem; oy = 0xFFFFFFFFu;
                 return FM_LOCATED;
             }

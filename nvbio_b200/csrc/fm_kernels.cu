@@ -160,6 +160,16 @@ fm_ktab16_context_kernel(const uint32_t* __restrict__ text, uint4* __restrict__ 
         tab[v].y = KTAB_TWO_ROW_MARK | text_before(text, e.z, 7u) | (text_before(text, e.w, 7u) << 14);
 }
 
+// the per-row array: rows[r] = {SA[r], the 16 text symbols before SA[r]} -- the suffix array read in order, the text gathered
+__global__ void __launch_bounds__(FM_BLOCKDIM)
+fm_rows_kernel(const uint32_t* __restrict__ sa, const uint32_t* __restrict__ text, uint2* __restrict__ rows, uint64_t n_rows)
+{
+    const uint64_t r = (uint64_t)blockIdx.x * FM_BLOCKDIM + threadIdx.x;
+    if (r >= n_rows) return;
+    const uint32_t pos = sa[r];
+    rows[r] = make_uint2(pos, text_before(text, pos, 16u));
+}
+
 // range sizes as uint64 (filter_inl.h:36-42: 1 + y - x in uint32 arithmetic, widened)
 struct RangeSize {
     __host__ __device__ __forceinline__ uint64_t operator()(const uint2& r) const { return (uint64_t)(uint32_t)(1u + r.y - r.x); }
@@ -343,6 +353,16 @@ int nvb_fm_build_ktab_context(const nvb_fm_index* fmi, uint32_t k, const uint32_
     if (r != NVB_OK) return r;
     const uint64_t entries = 1ull << (2u * k);
     fm_ktab16_context_kernel<<<(uint32_t)((entries + FM_BLOCKDIM - 1) / FM_BLOCKDIM), FM_BLOCKDIM, 0, as_stream(stream)>>>(d_text, (uint4*)d_ktab16, entries, fmi->length);
+    NVB_LAUNCH_CHECK();
+    return NVB_OK;
+}
+
+int nvb_fm_build_rows(const nvb_fm_index* fmi, const uint32_t* d_text, nvb_uint2* d_rows, void* stream)
+{
+    if (!fmi || !fmi->d_bwt_occ || !d_text || !d_rows || ((uintptr_t)d_rows & 7u)) return NVB_E_INVALID;
+    if (fmi->sa_interval != 1u || !fmi->d_ssa) return NVB_E_UNSUPPORTED;
+    const uint64_t n_rows = (uint64_t)fmi->length + 1u;
+    fm_rows_kernel<<<(uint32_t)((n_rows + FM_BLOCKDIM - 1) / FM_BLOCKDIM), FM_BLOCKDIM, 0, as_stream(stream)>>>(fmi->d_ssa, d_text, (uint2*)d_rows, n_rows);
     NVB_LAUNCH_CHECK();
     return NVB_OK;
 }

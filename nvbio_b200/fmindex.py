@@ -11,6 +11,11 @@ MATCH_FORWARD_ORDER = 1
 MATCH_COMPLEMENT = 2
 
 
+# device memory that build_ktab leaves free after the per-row array (a seed + extend call's temp buffers); without that room the
+# array is left out
+ROWS_HEADROOM = 4 << 30
+
+
 def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
@@ -36,6 +41,7 @@ class FMIndexDevice:
         self.sa_interval = int(sa_interval)        # 16 = the reference's SA_INT; 1 = full suffix array
         self.ktab, self.ktab_k = ktab, int(ktab_k)  # optional k-mer range table (an extension)
         self.ktab_located = 0                       # 1: 16-byte entries {x, y, SA[x], SA[y]} (build_ktab(k, located=True)); 2: + text context (text=...)
+        self.rows = None                            # with a context table: {SA[r], 16 symbols before SA[r]} per row (nvb_fm_build_rows)
 
     # -- views ------------------------------------------------------------------------------
     def struct(self) -> FmIndexStruct:
@@ -49,6 +55,8 @@ class FMIndexDevice:
         s.d_ktab = self.ktab.data_ptr() if self.ktab is not None else None
         s.ktab_k = self.ktab_k if self.ktab is not None else 0
         s.ktab_located = int(self.ktab_located) if self.ktab is not None else 0
+        if s.ktab_located == 2 and self.rows is not None:
+            s.ktab_located, s.d_rows = 3, self.rows.data_ptr()
         return s
 
     @property
@@ -57,14 +65,17 @@ class FMIndexDevice:
 
     def nbytes(self):
         return (self.bwt_occ.numel() * 4 + (self.ssa.numel() * 4 if self.ssa is not None else 0) +
-                (self.ktab.numel() * 4 if self.ktab is not None else 0))
+                (self.ktab.numel() * 4 if self.ktab is not None else 0) + (self.rows.numel() * 4 if self.rows is not None else 0))
 
     def build_ktab(self, k: int = 12, located: bool = False, text: Optional[torch.Tensor] = None):
         """k-mer range table (4^k x uint2): replaces the first k LF steps of every match().  located=True builds 16-byte entries
         {x, y, SA[x], SA[y]} instead (needs the full suffix array): a seed whose k-mer occurs once or twice is located by the look-up
         itself.  With text (the 2-bit big-endian words the index was built from) one-row entries also carry the 16 symbols before
-        SA[x] (nvb_fm_build_ktab_context): such a seed needs no read of the text at all."""
-        self.ktab = None                                   # release a previous table before allocating the new one
+        SA[x] (nvb_fm_build_ktab_context): such a seed needs no read of the text at all.  With the full suffix array and text, the
+        per-row array `rows` (nvb_fm_build_rows, (n + 1) x 8 bytes) is built as well when it fits the device's free memory: seeds whose
+        k-mer occurs 3 to 8 times are then resolved by one gather of their rows.  Results are the same with and without it."""
+        self.ktab = None                                   # release a previous table (and rows) before allocating the new one
+        self.rows = None
         tab = torch.empty((4 ** k, 4 if located else 2), dtype=torch.int32, device=self.device)
         s = self.struct()
         if located and text is not None:
@@ -76,6 +87,14 @@ class FMIndexDevice:
         else:
             check(lib().nvb_fm_build_ktab(C.byref(s), C.c_uint32(k), C.c_void_p(tab.data_ptr()), _stream()), "nvb_fm_build_ktab")
         self.ktab, self.ktab_k, self.ktab_located = tab, k, (2 if (located and text is not None) else (1 if located else 0))
+        if self.ktab_located == 2 and self.sa_interval == 1 and self.ssa is not None:
+            need = (self.length + 1) * 8
+            free, _ = torch.cuda.mem_get_info(self.device)
+            if need + ROWS_HEADROOM <= free:
+                rows = torch.empty((self.length + 1, 2), dtype=torch.int32, device=self.device)
+                check(lib().nvb_fm_build_rows(C.byref(self.struct()), C.c_void_p(text.data_ptr()), C.c_void_p(rows.data_ptr()), _stream()),
+                      "nvb_fm_build_rows")
+                self.rows = rows
         return self
 
     # -- construction -----------------------------------------------------------------------
