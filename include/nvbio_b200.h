@@ -521,6 +521,42 @@ int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     const nvb_pair_params* pair_params, const nvb_pair_out* out,
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream);
 
+/* Second-best pair and mapping quality of every mate (paired end; nvBowtie's BowtieMapq2 on BestPairedAlignments as MapqFunctorPE runs it,
+ * aligner_best_approx_paired.h:50-96, mapq.h:155-170).  The pairing is that of nvb_seed_extend_paired, whose outputs this call returns
+ * unchanged for the same inputs; call the pair it reports P*.
+ *   Mate candidates: those of nvb_seed_extend_mapq for that read (score s, strand t, end e, tie index), begin b = e - len clamped at 0,
+ *   and only those with s >= d_min_score[len].  Candidates with equal (strand, end) are merged into the one with the highest (s, -tie).
+ *   Candidate pairs of a pair that is not UNPAIRED: (1) every FR-concordant combination of one candidate of each mate (the concordance
+ *   test above), score s1 + s2; (2) every opposite-mate job the call ran (j < rescue_capacity) whose score rs reaches min_mate_score and
+ *   d_min_score[len]: the anchor's single-end best plus the rescued alignment (end = window begin + sink.x, strand opposite to the
+ *   anchor), score = anchor score + rs, the rescued mate's tie index 0xFFFFFFFF.  Rescues exist only for pairs that were not concordant
+ *   as they stood.
+ *   A candidate pair is not distinct from P* when both of its mates fail the single-end test against P*'s matching mate (same strand,
+ *   end within len/2).  The second-best pair is the distinct candidate pair with the largest score, ties to the smaller mate-1 tie index,
+ *   then the smaller mate-2 tie index -- one answer whatever the job order, path, de-duplication, exact shortcut or seed split.
+ *   A distinct pair may score ABOVE P*: two non-best alignments can be concordant where the bests are not and the rescue missed them.
+ *   It is still reported as the second pair (a low MAPQ); how the best pair is chosen does not change.
+ *   d_mate_mapq of a CONCORDANT or RESCUED pair, both mates: BowtieMapq2 with best = pair score, the second pair's score when there is
+ *   one, perfect = (len1 + len2) * match_bonus, min = d_min_score[len1] + d_min_score[len2], monotone when match_bonus == 0.  Mates of an
+ *   UNPAIRED pair: their single-end MAPQ (nvb_seed_extend_mapq on the 2n reads); an unaligned mate: 0.
+ * Mate m of pair p at index m * n_pairs + p, as in nvb_pair_out.  Validation as nvb_seed_extend_paired and nvb_seed_extend_mapq:
+ * NVB_E_INVALID when mapq, mapq_out, d_min_score, d_second_pair_score or d_mate_mapq is NULL, or max_read_len < reads->length.
+ * The temp size grows by about 36 bytes per unit of hit_capacity plus 28 bytes per read; nvb_seed_extend_paired does not carve it. */
+typedef struct nvb_pair_mapq_out {
+    int32_t*  d_second_pair_score;   /* [n_pairs], required; INT_MIN when there is no second pair */
+    uint32_t* d_second_mate_pos;     /* [2*n_pairs], may be NULL; each mate's end in the second pair, 0xFFFFFFFF when none */
+    uint8_t*  d_second_mate_strand;  /* [2*n_pairs], may be NULL; 0 when none */
+    int32_t*  d_mate_second_score;   /* [2*n_pairs], may be NULL; every mate's single-end second score (INT_MIN when none) */
+    uint8_t*  d_mate_mapq;           /* [2*n_pairs], required */
+} nvb_pair_mapq_out;
+
+int nvb_seed_extend_paired_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_pairs,
+                    const nvb_seed_extend_params* params, uint32_t hit_capacity,
+                    const nvb_pair_params* pair_params, const nvb_pair_out* out,
+                    const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
+                    uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream);
+
 /* -------------------------------------------------------------------------------------------
  * Host-buffer entry point: batches of reads in HOST memory in, per-read results in HOST memory out.
  * Replaces nvBowtie's input thread -> compute thread hand-off and its per-stage cudaDeviceSynchronize
@@ -563,7 +599,8 @@ void nvb_pipeline_destroy(nvb_pipeline* p);
 /* Profiling aid (the reference wraps every stage in cuda::Timer, nvBowtie/bowtie2/cuda/aligner_best_approx.h:
  * 219-241): device time in ms of the seven stages of the most recent nvb_seed_extend call -- [fw,rc] strings,
  * seed match (FM-index), hit slots, locate + windows, job de-duplication, banded extension, best-per-read (which includes the
- * traceback and, in nvb_seed_extend_mapq, the second-best pass and the MAPQ).  Synchronises on the call's last event. */
+ * traceback and, in nvb_seed_extend_mapq / nvb_seed_extend_paired_mapq, the second-best passes and the MAPQ).  Synchronises on the
+ * call's last event. */
 int nvb_seed_extend_stage_ms(float ms[7]);
 
 #ifdef __cplusplus

@@ -13,6 +13,7 @@
 #include "gotoh_core.cuh"
 #include "pipeline_core.cuh"
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_segmented_sort.cuh>
 #include <mutex>
 
 namespace nvb {
@@ -663,7 +664,7 @@ __device__ __forceinline__ MateBest mate_best(const PipeGeom& g, uint32_t r, con
     m.strand = best_strand[r];
     m.len = str_len[r * g.strands];                 // both strands of a read have its length
     m.end = end;
-    m.beg = m.end > m.len ? m.end - m.len : 0u;
+    m.beg = aln_begin(m.end, m.len);
     return m;
 }
 
@@ -691,7 +692,7 @@ pair_classify_kernel(const PipeGeom g, const uint32_t n_pairs, const nvb_pair_pa
     if (conc) {
         const MateBest& f = m[0].strand == 0 ? m[0] : m[1];
         const MateBest& r = m[0].strand == 0 ? m[1] : m[0];
-        conc = f.beg <= r.beg && f.end <= r.end && r.end > f.beg && (r.end - f.beg) >= pp.min_frag && (r.end - f.beg) <= pp.max_frag;
+        conc = fr_concordant(f.beg, f.end, r.beg, r.end, pp.min_frag, pp.max_frag);
     }
     if (conc) {
         pair_score[p] = m[0].score + m[1].score; pair_flags[p] = NVB_PAIR_CONCORDANT;
@@ -754,6 +755,111 @@ pair_finalize_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const uin
     mate_strand[o * n_pairs + p] = (uint8_t)(1u - mate_strand[best_a * n_pairs + p]);
 }
 
+// ---------------------------------------------------------------------------------------------
+// second-best pair and paired MAPQ (nvb_seed_extend_paired_mapq).  The candidates of a mate are those of the single-end stage (see
+// pipe_second_reduce_kernel) that reach the read's min score, gathered into one segment per read, sorted by (strand, end) and merged per
+// (strand, end); pair_second_kernel pairs them up (pair_combinations, pipeline_core.cuh) and adds the pair's rescues.
+// ---------------------------------------------------------------------------------------------
+
+// candidates per read (counts) or their place in the read's segment (seg != NULL: cursor = counts zeroed, key = (strand << 32) | end)
+__global__ void __launch_bounds__(256)
+pair_cand_scatter_kernel(const PipeGeom g, const uint32_t* __restrict__ count, const uint32_t* __restrict__ c_string,
+                         const uint32_t* __restrict__ t_off, const int32_t* __restrict__ score, const uint2* __restrict__ sink,
+                         const uint32_t* __restrict__ str_len, const int32_t* __restrict__ min_score, const uint32_t* __restrict__ seg,
+                         uint32_t* __restrict__ cursor, unsigned long long* __restrict__ key, uint32_t* __restrict__ val)
+{
+    const uint32_t n = *count;
+    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
+        const uint32_t s = c_string[j], read = s / g.strands;
+        if (score[j] < min_score[str_len[s]]) continue;
+        const uint32_t slot = atomicAdd(cursor + read, 1u);
+        if (!seg) continue;
+        key[seg[read] + slot] = ((unsigned long long)(s % g.strands) << 32) | (t_off[j] + sink[j].x);
+        val[seg[read] + slot] = j;
+    }
+}
+
+// one thread per read: its sorted segment merged per (strand, end) into the one with the highest (score, -tie), written to m_end / m_score
+// / m_tie from the segment's start; n_fw / n_merged = forward / all merged candidates
+__global__ void __launch_bounds__(256)
+pair_cand_merge_kernel(const uint32_t n_reads, const uint32_t* __restrict__ seg, const uint32_t* __restrict__ cnt,
+                       const unsigned long long* __restrict__ key, const uint32_t* __restrict__ val, const uint32_t* __restrict__ index,
+                       const int32_t* __restrict__ score, uint32_t* __restrict__ m_end, int32_t* __restrict__ m_score, uint32_t* __restrict__ m_tie,
+                       uint32_t* __restrict__ n_fw, uint32_t* __restrict__ n_merged)
+{
+    const uint32_t r = blockIdx.x * 256 + threadIdx.x;
+    if (r >= n_reads) return;
+    const uint32_t b = seg[r], n = cnt[r];
+    uint32_t m = 0, fw = 0; unsigned long long prev = ~0ull;
+    for (uint32_t k = b; k < b + n; ++k) {
+        const unsigned long long kk = key[k];
+        const uint32_t j = val[k], tie = index ? index[j] : j;
+        const int32_t sc = score[j];
+        if (kk == prev) {
+            const uint32_t o = b + m - 1u;
+            if (sc > m_score[o] || (sc == m_score[o] && tie < m_tie[o])) { m_score[o] = sc; m_tie[o] = tie; }
+            continue;
+        }
+        prev = kk;
+        m_end[b + m] = (uint32_t)kk; m_score[b + m] = sc; m_tie[b + m] = tie;
+        ++m; if ((kk >> 32) == 0ull) ++fw;
+    }
+    n_fw[r] = fw; n_merged[r] = m;
+}
+
+// one thread per pair: the second-best pair (combinations of the mates' candidates plus the pair's rescues) and the MAPQ of both mates.
+// UNPAIRED pairs keep the single-end MAPQ pipe_mapq_kernel wrote into mate_mapq.  se_pos: the mates' single-end best ends (a rescue's
+// anchor), best_key: their tie indices
+__global__ void __launch_bounds__(256)
+pair_second_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const nvb_mapq_params mp, const uint32_t* __restrict__ str_len,
+                   const uint32_t* __restrict__ seg, const uint32_t* __restrict__ n_fw, const uint32_t* __restrict__ n_merged,
+                   const uint32_t* __restrict__ m_end, const int32_t* __restrict__ m_score, const uint32_t* __restrict__ m_tie,
+                   const uint32_t* __restrict__ se_pos, const uint8_t* __restrict__ se_strand, const unsigned long long* __restrict__ best_key,
+                   const uint32_t* __restrict__ want, const uint32_t* __restrict__ job_idx, const uint32_t* __restrict__ w_toff,
+                   const int32_t* __restrict__ rs_score, const uint2* __restrict__ rs_sink,
+                   const int32_t* __restrict__ pair_score, const uint32_t* __restrict__ pair_flags,
+                   const uint32_t* __restrict__ mate_pos, const uint8_t* __restrict__ mate_strand,
+                   int32_t* __restrict__ second_pair_score, uint32_t* __restrict__ second_mate_pos, uint8_t* __restrict__ second_mate_strand,
+                   uint8_t* __restrict__ mate_mapq)
+{
+    const uint32_t p = blockIdx.x * 256 + threadIdx.x;
+    if (p >= n_pairs) return;
+    const uint32_t r0 = p, r1 = n_pairs + p;
+    const uint32_t len[2] = {str_len[2u * r0], str_len[2u * r1]};         // (both strands of a read have its length)
+    PairSecond ps;
+    ps.init(mate_pos[r0], mate_strand[r0], len[0], mate_pos[r1], mate_strand[r1], len[1]);
+    const uint32_t flags = pair_flags[p];
+    if (flags != NVB_PAIR_UNPAIRED) {
+        MateCands m[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const uint32_t r = k ? r1 : r0, b = seg[r];
+            m[k].end = m_end + b; m[k].score = m_score + b; m[k].tie = m_tie + b; m[k].n_fw = n_fw[r]; m[k].n = n_merged[r]; m[k].len = len[k];
+        }
+        pair_combinations(m, pp.min_frag, pp.max_frag, ps);
+        // rescues: the anchor's single-end best with the rescued alignment of the other mate (tie index 0xFFFFFFFF)
+        for (int a = 0; a < 2; ++a) {
+            const uint32_t i = 2u * p + a, ra = a ? r1 : r0;
+            if (!want[i]) continue;
+            const uint32_t j = job_idx[i];
+            if (j >= pp.rescue_capacity) continue;
+            const int32_t rs = rs_score[j];
+            if (rs < pp.min_mate_score || rs < mp.d_min_score[len[1 - a]]) continue;
+            const unsigned long long key = best_key[ra];
+            ps.offer_rescue(a, best_key_score(key) + rs, se_pos[ra], se_strand[ra], best_key_index(key), w_toff[i] + rs_sink[j].x);
+        }
+        const uint8_t q = (uint8_t)bowtie_mapq2(pair_score[p], ps.has, ps.score, (int32_t)(len[0] + len[1]) * mp.match_bonus,
+                                                mp.d_min_score[len[0]] + mp.d_min_score[len[1]], mp.match_bonus == 0);
+        mate_mapq[r0] = q; mate_mapq[r1] = q;
+    }
+    second_pair_score[p] = ps.score;
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        if (second_mate_pos) second_mate_pos[k * n_pairs + p] = ps.end[k];
+        if (second_mate_strand) second_mate_strand[k * n_pairs + p] = (uint8_t)ps.strand[k];
+    }
+}
+
 } // namespace nvb
 
 using namespace nvb;
@@ -812,7 +918,8 @@ struct PipeCall {
     bool dedup, per_read, eligible;                                         // eligible: the exact shortcut applies (pipe_perfect_jobs_kernel)
     int32_t* best_score; uint32_t* best_pos; int32_t* hit_score; nvb_uint2* hit_sink;   // the caller's outputs (per-hit ones may be NULL)
     const nvb_best_alignment_out* BA; const nvb_pair_params* PP; const nvb_pair_out* PO;
-    const nvb_mapq_params* MP; const nvb_mapq_out* MO;
+    const nvb_mapq_params* MP; const nvb_mapq_out* MO; const nvb_pair_mapq_out* PMO;
+    nvb_mapq_out se_mo;                                                     // paired MAPQ: the single-end stage's outputs (MO = &se_mo)
     StageEvents* SE;
     uint32_t *str_words, *str_len; uint8_t* str_quals;                      // [fw, rc] strings
     uint2* ranges; uint32_t *sizes, *excl, *counts, *seed_todo_n;           // counts: [0] hits kept, [1] hits found, [2] alignment jobs
@@ -827,6 +934,8 @@ struct PipeCall {
     uint32_t *pw_want, *pw_idx, *pw_pstr, *pw_toff, *pw_tlen, *pcounts;     // paired: two opposite-mate job slots per pair
     Jobs rescue; int32_t* rs_score; uint2* rs_sink; char *pscan_tmp, *full_tmp; size_t pscan_bytes, full_bytes;
     unsigned long long* second_key;                                         // second-best alignment of every read (MO)
+    uint32_t *pc_cnt, *pc_seg, *pc_fw, *pc_n, *pc_val[2], *pc_end, *pc_tie, *se_pos;     // paired MAPQ (PMO): candidate segments per read
+    unsigned long long* pc_key[2]; int32_t* pc_score; char *pc_scan_tmp, *pc_sort_tmp; size_t pc_scan_bytes, pc_sort_bytes;
 
     int stage(int i) const { return (int)cudaEventRecord(SE->ev[i], s); }    // boundary i of nvb_seed_extend_stage_ms
 
@@ -900,6 +1009,19 @@ struct PipeCall {
             full_tmp = tc.take<char>(full_bytes);
         }
         if (MO) second_key = tc.take<unsigned long long>(n_reads);
+        if (PMO) {
+            if (!PMO->d_mate_second_score) se_mo.d_second_score = tc.take<int32_t>(n_reads);
+            pc_cnt = tc.take<uint32_t>((size_t)n_reads + 1); pc_seg = tc.take<uint32_t>((size_t)n_reads + 1);
+            pc_fw = tc.take<uint32_t>(n_reads); pc_n = tc.take<uint32_t>(n_reads); se_pos = tc.take<uint32_t>(n_reads);
+            for (int k = 0; k < 2; ++k) { pc_key[k] = tc.take<unsigned long long>(cap); pc_val[k] = tc.take<uint32_t>(cap); }
+            pc_end = tc.take<uint32_t>(cap); pc_score = tc.take<int32_t>(cap); pc_tie = tc.take<uint32_t>(cap);
+            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, pc_scan_bytes, pc_cnt, pc_seg, (int)n_reads + 1, s));
+            pc_scan_tmp = tc.take<char>(pc_scan_bytes);
+            pc_sort_bytes = 0;
+            if (cap) NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairs(nullptr, pc_sort_bytes, pc_key[0], pc_key[1], pc_val[0], pc_val[1], (int)cap,
+                                                                     (int)n_reads, pc_seg, pc_seg + 1, s));
+            pc_sort_tmp = tc.take<char>(pc_sort_bytes);
+        }
         need = tc.total();
         return NVB_OK;
     }
@@ -1059,6 +1181,49 @@ struct PipeCall {
         return launched();
     }
 
+    // paired MAPQ, before the rescue overwrites the mate arrays: every read's candidates (those second_best() sees that reach its min
+    // score) in a segment of their own, sorted by (strand, end) and merged per (strand, end); the single-end best ends (rescue anchors)
+    int pair_candidates() const
+    {
+        const uint32_t cap = hit_capacity, n_reads = g.n_reads;
+        NVB_CUDA_TRY(cudaMemcpyAsync(se_pos, best_pos, sizeof(uint32_t) * n_reads, cudaMemcpyDeviceToDevice, s));
+        NVB_CUDA_TRY(cudaMemsetAsync(pc_cnt, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
+        if (cap) {
+            const uint32_t* n  = per_read ? counts + 2 : counts;
+            const uint32_t* cs = per_read ? j_string : hit_string;
+            const uint32_t* to = per_read ? jobs.t_off : hits.t_off;
+            const int32_t* sc  = per_read ? job_score : h_score;
+            const uint2* sk    = per_read ? job_sink : h_sink;
+            const uint32_t hgrid = (cap + 255) / 256, grid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
+            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, n, cs, to, sc, sk, str_len, MP->d_min_score, nullptr, pc_cnt, nullptr, nullptr);
+            NVB_LAUNCH_CHECK();
+            size_t bytes = pc_scan_bytes;
+            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(pc_scan_tmp, bytes, pc_cnt, pc_seg, (int)n_reads + 1, s));
+            NVB_CUDA_TRY(cudaMemsetAsync(pc_cnt, 0, sizeof(uint32_t) * n_reads, s));
+            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, n, cs, to, sc, sk, str_len, MP->d_min_score, pc_seg, pc_cnt, pc_key[0], pc_val[0]);
+            NVB_LAUNCH_CHECK();
+            bytes = pc_sort_bytes;
+            NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairs(pc_sort_tmp, bytes, pc_key[0], pc_key[1], pc_val[0], pc_val[1], (int)cap, (int)n_reads,
+                                                             pc_seg, pc_seg + 1, s));
+        } else
+            NVB_CUDA_TRY(cudaMemsetAsync(pc_seg, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
+        pair_cand_merge_kernel<<<(n_reads + 255) / 256, 256, 0, s>>>(n_reads, pc_seg, pc_cnt, pc_key[1], pc_val[1], per_read ? j_first : nullptr,
+                                                                      per_read ? job_score : h_score, pc_end, pc_score, pc_tie, pc_fw, pc_n);
+        return launched();
+    }
+
+    // second-best pair and MAPQ of every pair, after the rescue: the pairs' final flags and mates are P*
+    int pair_second() const
+    {
+        const uint32_t n_pairs = g.n_reads / 2u;
+        pair_second_kernel<<<(n_pairs + 255) / 256, 256, 0, s>>>(n_pairs, *PP, *MP, str_len, pc_seg, pc_fw, pc_n, pc_end, pc_score, pc_tie,
+                                                                  se_pos, rb_strand, best_key, pw_want, pw_idx, pw_toff, rs_score, rs_sink,
+                                                                  PO->d_pair_score, PO->d_pair_flags, PO->d_mate_pos, PO->d_mate_strand,
+                                                                  PMO->d_second_pair_score, PMO->d_second_mate_pos, PMO->d_second_mate_strand,
+                                                                  PMO->d_mate_mapq);
+        return launched();
+    }
+
     // paired-end rescue: non-concordant pairs get opposite-mate jobs (scan-compacted) for the full-matrix DP; the best rescue wins
     int paired_rescue() const
     {
@@ -1095,7 +1260,7 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     int32_t* d_hit_score, nvb_uint2* d_hit_sink,
                     const nvb_best_alignment_out* BA,
                     const nvb_pair_params* PP, const nvb_pair_out* PO,
-                    const nvb_mapq_params* MP, const nvb_mapq_out* MO,
+                    const nvb_mapq_params* MP, const nvb_mapq_out* MO, const nvb_pair_mapq_out* PMO,
                     void* d_temp, size_t* temp_bytes, void* stream)
 {
     if (PP) {
@@ -1128,6 +1293,11 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     const cudaStream_t s = c.s = as_stream(stream);
     c.P = P; c.f = make_fmindex(fmi); c.rd = make_strset(reads); c.genome = d_genome; c.nq = (uint32_t)nq64; c.hit_capacity = hit_capacity;
     c.best_score = d_best_score; c.best_pos = d_best_pos; c.hit_score = d_hit_score; c.hit_sink = d_hit_sink; c.BA = BA; c.PP = PP; c.PO = PO; c.MP = MP; c.MO = MO;
+    if (PMO) {                                 // the single-end second best and MAPQ of every mate (mate_mapq: overwritten for paired pairs)
+        c.PMO = PMO;
+        c.se_mo.d_second_score = PMO->d_mate_second_score; c.se_mo.d_mapq = PMO->d_mate_mapq;
+        c.MO = &c.se_mo;
+    }
     c.dedup = P->dedup_jobs != 0;
     // per-read path: nobody asked for per-hit outputs, so no per-hit array needs to exist
     c.per_read = c.dedup && g_pipe_path != 1 && !d_hit_read && !d_hit_window && !d_hit_score && !d_hit_sink && !BA;
@@ -1154,8 +1324,10 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
         NVB_LAUNCH_CHECK();
     }
     if (BA) NVB_TRY(c.best_traceback());
+    if (c.MO) NVB_TRY(c.second_best());
+    if (PMO) NVB_TRY(c.pair_candidates());
     if (PP) NVB_TRY(c.paired_rescue());
-    if (MO) NVB_TRY(c.second_best());
+    if (PMO) NVB_TRY(c.pair_second());
     if (!c.dedup) NVB_CUDA_TRY(cudaMemcpyAsync(c.counts + 2, c.counts, sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
     if (d_n_hits) NVB_CUDA_TRY(cudaMemcpyAsync(d_n_hits, c.counts, 3 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
     NVB_TRY(c.stage(7));
@@ -1176,7 +1348,7 @@ extern "C" int nvb_seed_extend(const nvb_fm_index* fmi, const uint32_t* d_genome
                     void* d_temp, size_t* temp_bytes, void* stream)
 {
     return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
-                            d_hit_score, d_hit_sink, nullptr, nullptr, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
+                            d_hit_score, d_hit_sink, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_traceback(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1190,7 +1362,7 @@ extern "C" int nvb_seed_extend_traceback(const nvb_fm_index* fmi, const uint32_t
 {
     if (!best_alignment) return NVB_E_INVALID;
     return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
-                            d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
+                            d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1202,7 +1374,7 @@ extern "C" int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d
     if (!pair_params || !out || n_pairs > 0x3FFFFFFFu || !temp_bytes) return NVB_E_INVALID;
     // the per-read best (score, end) of the single-end stage lands in the mate arrays first and is then refined per pair
     return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
-                            nullptr, nullptr, nullptr, pair_params, out, nullptr, nullptr, d_temp, temp_bytes, stream);
+                            nullptr, nullptr, nullptr, pair_params, out, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1218,7 +1390,21 @@ extern "C" int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_g
     if (!mapq || !mapq_out || !mapq->d_min_score || !mapq_out->d_second_score || !mapq_out->d_mapq) return NVB_E_INVALID;
     if (!reads || mapq->max_read_len < reads->length) return NVB_E_INVALID;           // the min-score table must cover every read length
     return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
-                            d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, mapq, mapq_out, d_temp, temp_bytes, stream);
+                            d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, mapq, mapq_out, nullptr, d_temp, temp_bytes, stream);
+}
+
+extern "C" int nvb_seed_extend_paired_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_pairs,
+                    const nvb_seed_extend_params* P, uint32_t hit_capacity,
+                    const nvb_pair_params* pair_params, const nvb_pair_out* out,
+                    const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
+                    uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream)
+{
+    if (!pair_params || !out || n_pairs > 0x3FFFFFFFu || !temp_bytes) return NVB_E_INVALID;
+    if (!mapq || !mapq_out || !mapq->d_min_score || !mapq_out->d_second_pair_score || !mapq_out->d_mate_mapq) return NVB_E_INVALID;
+    if (!reads || mapq->max_read_len < reads->length) return NVB_E_INVALID;           // the min-score table must cover every read length
+    return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
+                            nullptr, nullptr, nullptr, pair_params, out, mapq, nullptr, mapq_out, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_debug_mapq_eval(const int32_t* d_best, const uint8_t* d_has_second, const int32_t* d_second, const uint32_t* d_len,

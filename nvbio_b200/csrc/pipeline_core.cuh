@@ -110,6 +110,78 @@ __host__ __device__ __forceinline__ bool distinct_alignment(uint32_t p, uint32_t
     return t != bt || p < bp - (bp < d ? bp : d) || p > bp + d;
 }
 
+// begin of an alignment ending at `end` of a read of length len: end - len, clamped at 0 (no traceback: soft clips and indels ignored)
+__host__ __device__ __forceinline__ uint32_t aln_begin(uint32_t end, uint32_t len) { return end > len ? end - len : 0u; }
+
+// FR concordance of a forward mate [fb, fe) and a reverse mate [rb, re): the forward one starts and ends no later than the reverse one and
+// the fragment [fb, re) is non-empty with a length in [min_frag, max_frag] (nvb_seed_extend_paired, PE_POLICY_FR)
+__host__ __device__ __forceinline__ bool fr_concordant(uint32_t fb, uint32_t fe, uint32_t rb, uint32_t re, uint32_t min_frag, uint32_t max_frag)
+{
+    return fb <= rb && fe <= re && re > fb && (re - fb) >= min_frag && (re - fb) <= max_frag;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Second-best pair of nvb_seed_extend_paired_mapq.  A candidate pair is one alignment of each mate (end, strand, tie index); it is not
+// distinct from the reported pair P* when BOTH its mates fail distinct_alignment against P*'s matching mate.  The second-best pair is
+// the distinct candidate pair with the largest score, ties to the smaller mate-1 tie index, then the smaller mate-2 tie index -- a total
+// order, so the answer does not depend on the order the candidates are offered in.
+// ---------------------------------------------------------------------------------------------
+struct PairSecond {
+    uint32_t star_end[2], star_strand[2], len[2];              // P* and the mates' read lengths
+    bool has; int32_t score; uint32_t end[2], strand[2], tie[2];
+
+    __host__ __device__ __forceinline__ void init(uint32_t e1, uint32_t t1, uint32_t l1, uint32_t e2, uint32_t t2, uint32_t l2)
+    {
+        star_end[0] = e1; star_strand[0] = t1; len[0] = l1; star_end[1] = e2; star_strand[1] = t2; len[1] = l2;
+        has = false; score = INT_MIN; end[0] = end[1] = 0xFFFFFFFFu; strand[0] = strand[1] = 0u; tie[0] = tie[1] = 0xFFFFFFFFu;
+    }
+    __host__ __device__ __forceinline__ void offer(int32_t s, uint32_t e1, uint32_t t1, uint32_t i1, uint32_t e2, uint32_t t2, uint32_t i2)
+    {
+        if (!distinct_alignment(e1, t1, star_end[0], star_strand[0], len[0]) && !distinct_alignment(e2, t2, star_end[1], star_strand[1], len[1]))
+            return;
+        if (has && (s < score || (s == score && (i1 > tie[0] || (i1 == tie[0] && i2 >= tie[1]))))) return;
+        has = true; score = s; end[0] = e1; strand[0] = t1; tie[0] = i1; end[1] = e2; strand[1] = t2; tie[1] = i2;
+    }
+    // a rescue: anchor mate a's single-end best (end ae, strand at, tie index ai) with the other mate placed at end oe on the opposite
+    // strand (tie index 0xFFFFFFFF); s = the anchor's score + the rescue's
+    __host__ __device__ __forceinline__ void offer_rescue(int a, int32_t s, uint32_t ae, uint32_t at, uint32_t ai, uint32_t oe)
+    {
+        if (a == 0) offer(s, ae, at, ai, oe, 1u - at, 0xFFFFFFFFu);
+        else        offer(s, oe, 1u - at, 0xFFFFFFFFu, ae, at, ai);
+    }
+};
+
+// a mate's candidates, merged per (strand, end) and sorted: the forward ones [0, n_fw), then the reverse ones [n_fw, n), each by end
+struct MateCands { const uint32_t* end; const int32_t* score; const uint32_t* tie; uint32_t n_fw, n, len; };
+
+// first index in [lo, hi) whose end is >= v
+__host__ __device__ __forceinline__ uint32_t lower_bound_end(const uint32_t* end, uint32_t lo, uint32_t hi, uint64_t v)
+{
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if ((uint64_t)end[mid] < v) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+
+// offer every FR-concordant combination of one candidate of each mate: for each forward candidate of either mate, only the other mate's
+// reverse candidates ending in [begin + min_frag, begin + max_frag] are visited (binary search), so the work is bounded by the
+// concordant combinations and not by the product of the two lists
+__host__ __device__ inline void pair_combinations(const MateCands m[2], uint32_t min_frag, uint32_t max_frag, PairSecond& ps)
+{
+    for (int a = 0; a < 2; ++a) {
+        const MateCands& F = m[a]; const MateCands& R = m[1 - a];
+        for (uint32_t i = 0; i < F.n_fw; ++i) {
+            const uint32_t fe = F.end[i], fb = aln_begin(fe, F.len);
+            uint32_t k = lower_bound_end(R.end, R.n_fw, R.n, (uint64_t)fb + min_frag);
+            for (; k < R.n && (uint64_t)R.end[k] <= (uint64_t)fb + max_frag; ++k) {
+                const uint32_t re = R.end[k];
+                if (!fr_concordant(fb, fe, aln_begin(re, R.len), re, min_frag, max_frag)) continue;
+                const int32_t s = F.score[i] + R.score[k];
+                if (a == 0) ps.offer(s, fe, 0u, F.tie[i], re, 1u, R.tie[k]);
+                else        ps.offer(s, re, 1u, R.tie[k], fe, 0u, F.tie[i]);
+            }
+        }
+    }
+}
+
 // Mapping quality of an unpaired read: nvBowtie's BowtieMapq2 (mapq.h:155-327) for a scheme with perfect_score(len) = perfect,
 // min_score(len) = min_score and m_monotone = monotone (match bonus 0, end-to-end).  The same float operations in the same order (only
 // multiplies, subtractions, fabsf and compares: nothing the compiler could contract into an FMA), so host and device agree bit for bit.

@@ -5,7 +5,8 @@ from dataclasses import dataclass, field
 from typing import Optional
 import torch
 import numpy as np
-from ._lib import lib, check, SeedExtendParamsStruct, BestAlignmentOutStruct, PairParamsStruct, PairOutStruct, MapqParamsStruct, MapqOutStruct
+from ._lib import (lib, check, SeedExtendParamsStruct, BestAlignmentOutStruct, PairParamsStruct, PairOutStruct, MapqParamsStruct, MapqOutStruct,
+                   PairMapqOutStruct)
 from .strings import PackedStringSet
 from .fmindex import FMIndexDevice
 from . import aln
@@ -215,7 +216,8 @@ class PairParams:
 class PairedWorkspace:
     """outputs + temp storage of seed_extend_paired for repeated calls on equally-shaped batches"""
 
-    def __init__(self, fmi, genome, reads: PackedStringSet, params: SeedExtendParams, pair: PairParams, hit_capacity: int):
+    def __init__(self, fmi, genome, reads: PackedStringSet, params: SeedExtendParams, pair: PairParams, hit_capacity: int,
+                 mapq: Optional[MapqParams] = None):
         dev = fmi.device
         assert reads.count % 2 == 0
         self.n_pairs = n = reads.count // 2
@@ -227,6 +229,15 @@ class PairedWorkspace:
         self.mate_strand = torch.empty((2, n), dtype=torch.uint8, device=dev)
         self.n_rescue = torch.zeros(2, dtype=torch.int32, device=dev)
         self.n_hits = torch.zeros(3, dtype=torch.int32, device=dev)
+        # optional second-best pair and MAPQ of every mate
+        self.mapq_params = mapq
+        self.second_pair_score = self.second_mate_pos = self.second_mate_strand = self.mate_second_score = self.mate_mapq = None
+        if mapq is not None:
+            self.second_pair_score = torch.empty(n, dtype=torch.int32, device=dev)
+            self.second_mate_pos = torch.empty((2, n), dtype=torch.int32, device=dev)
+            self.second_mate_strand = torch.empty((2, n), dtype=torch.uint8, device=dev)
+            self.mate_second_score = torch.empty((2, n), dtype=torch.int32, device=dev)
+            self.mate_mapq = torch.empty((2, n), dtype=torch.uint8, device=dev)
         tb = C.c_size_t(0)
         r = _call_paired(fmi, genome, reads, params, pair, self, None, tb)
         if r != -2:
@@ -241,21 +252,36 @@ def _call_paired(fmi, genome, reads, params, pair, ws, temp, tb):
     po.d_pair_score, po.d_pair_flags = ws.pair_score.data_ptr(), ws.pair_flags.data_ptr()
     po.d_mate_score, po.d_mate_pos, po.d_mate_strand = ws.mate_score.data_ptr(), ws.mate_pos.data_ptr(), ws.mate_strand.data_ptr()
     po.d_n_rescue = ws.n_rescue.data_ptr()
+    if ws.mate_mapq is not None:
+        mp = ws.mapq_params.struct()
+        mo = PairMapqOutStruct()
+        mo.d_second_pair_score, mo.d_second_mate_pos = ws.second_pair_score.data_ptr(), ws.second_mate_pos.data_ptr()
+        mo.d_second_mate_strand, mo.d_mate_second_score = ws.second_mate_strand.data_ptr(), ws.mate_second_score.data_ptr()
+        mo.d_mate_mapq = ws.mate_mapq.data_ptr()
+        return lib().nvb_seed_extend_paired_mapq(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(ws.n_pairs), C.byref(ps),
+                                                 C.c_uint32(ws.hit_capacity), C.byref(pp), C.byref(po), C.byref(mp), C.byref(mo),
+                                                 _p(ws.n_hits), _p(temp), C.byref(tb), C.c_void_p(torch.cuda.current_stream().cuda_stream))
     return lib().nvb_seed_extend_paired(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(ws.n_pairs), C.byref(ps), C.c_uint32(ws.hit_capacity),
                                         C.byref(pp), C.byref(po), _p(ws.n_hits), _p(temp), C.byref(tb),
                                         C.c_void_p(torch.cuda.current_stream().cuda_stream))
 
 
 def seed_extend_paired(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStringSet, params: SeedExtendParams, pair: PairParams,
-                       workspace: Optional[PairedWorkspace] = None, hit_capacity: Optional[int] = None):
+                       workspace: Optional[PairedWorkspace] = None, hit_capacity: Optional[int] = None, mapq: Optional[MapqParams] = None):
     """paired-end seed + extend (reads = mate 1 of every pair, then mate 2 of every pair): concordant pairs straight from the two
     independent alignments, opposite-mate full-DP rescue for the rest (nvBowtie's best-approx paired flow,
     score_opposite_inl.h:90-266).  Returns the workspace: .pair_score[n], .pair_flags[n], .mate_score/.mate_pos/.mate_strand[2,n],
-    .n_rescue[2] = (full-DP jobs run, wanted)"""
+    .n_rescue[2] = (full-DP jobs run, wanted).  With mapq=MapqParams(...) also the second-best pair and the MAPQ of every mate
+    (nvb_seed_extend_paired_mapq): .second_pair_score[n], .second_mate_pos/.second_mate_strand[2,n], .mate_second_score[2,n] (each mate's
+    single-end second score) and .mate_mapq[2,n].  A workspace made with mapq keeps computing them; a new mapq replaces its table"""
     if workspace is None:
         if hit_capacity is None:
             hit_capacity = 32 * reads.count + 1024
-        workspace = PairedWorkspace(fmi, genome, reads, params, pair, hit_capacity)
+        workspace = PairedWorkspace(fmi, genome, reads, params, pair, hit_capacity, mapq)
+    elif mapq is not None:
+        if workspace.mate_mapq is None:
+            raise ValueError("seed_extend_paired(mapq=...): the workspace was created without mapq outputs")
+        workspace.mapq_params = mapq
     tb = C.c_size_t(workspace.temp_bytes)
     check(_call_paired(fmi, genome, reads, params, pair, workspace, workspace.temp, tb), "nvb_seed_extend_paired")
     return workspace
