@@ -70,8 +70,12 @@ typedef struct nvb_fm_index {
                                     symbols long) is resolved by the look-up alone; and, when length < 0xC0000000, a TWO-row entry is
                                     stored as {x, 0xC0000000 | a | b << 14, SA[x], SA[x+1]} (y = x + 1 implied; a, b = the 7 symbols before
                                     SA[x], SA[x+1]), which resolves seeds up to k + 7 symbols the same way;  3: as 2, and d_rows is set
-                                    (needs sa_interval == 1 and d_ssa).  Ranges are identical in every case.  */
-    const nvb_uint2* d_rows;     /* read only when ktab_located == 3: length + 1 entries {SA[r], the 16 text symbols before SA[r]}
+                                    (needs sa_interval == 1 and d_ssa);  4: d_ktab holds 32-byte entries (32-byte aligned) built by
+                                    nvb_fm_build_ktab_wide: the first 16 bytes of each as at level 2, and a k-mer with 3 to 8
+                                    occurrences also carries its rows' text contexts (and, for 3 or 4 rows, their SA values), so that
+                                    the seed + extend path resolves most such seeds with the look-up alone (needs sa_interval == 1 and
+                                    d_ssa);  5: as 4, and d_rows is set.  Ranges are identical in every case.  */
+    const nvb_uint2* d_rows;     /* read only when ktab_located is 3 or 5: length + 1 entries {SA[r], the 16 text symbols before SA[r]}
                                     built by nvb_fm_build_rows.  The per-read seed + extend path then resolves a seed whose k-mer
                                     occurs 3 to 8 times (and that is up to k + 16 symbols long) with one gather of those rows instead
                                     of walking the range on; results are identical with and without it */
@@ -373,6 +377,17 @@ int nvb_fm_build_ktab_located(const nvb_fm_index* fmi, uint32_t k, void* d_ktab1
  * d_text (2-bit big-endian, the text the index was built from) that precede SA[x], symbol SA[x]-1 in the two lowest bits; two-row
  * entries are packed as described at nvb_fm_index.ktab_located.  Use with nvb_fm_index.d_ktab = d_ktab16, ktab_located = 2. */
 int nvb_fm_build_ktab_context(const nvb_fm_index* fmi, uint32_t k, const uint32_t* d_text, void* d_ktab16, void* stream);
+
+/* The context table with 32-byte entries, one DRAM sector each (d_ktab32: 4^k * 32 bytes, 32-byte aligned; 34.4 GB at k = 15).  Words
+ * 0-3 of an entry are what nvb_fm_build_ktab_context writes, except for k-mers with 3 to 8 occurrences (rows x..y), which use the
+ * words that format leaves zero.  With ctxN(r) = the (up to) N symbols of d_text before SA[r], symbol SA[r]-1 in the two lowest bits:
+ *     3 rows:    {x, y, SA[x], SA[x+1], SA[x+2], ctx16(x), ctx16(x+1), ctx16(x+2)}
+ *     4 rows:    {x, y, ctx8(x) | ctx8(x+1) << 16, ctx8(x+2) | ctx8(x+3) << 16, SA[x], SA[x+1], SA[x+2], SA[x+3]}
+ *     5-8 rows:  {x, y, ctx8 of the rows two per word (row x in the low half of word 2, x+1 in its high half, ...), 0, ...}
+ * Other entries have zero in words 4-7.  Needs the full suffix array (fmi->sa_interval == 1, fmi->d_ssa), else NVB_E_UNSUPPORTED;
+ * fmi->d_ktab / ktab_k / ktab_located are ignored.  Uses no memory beyond the table.  Use with nvb_fm_index.d_ktab = d_ktab32,
+ * ktab_located = 4 (5 with d_rows). */
+int nvb_fm_build_ktab_wide(const nvb_fm_index* fmi, uint32_t k, const uint32_t* d_text, void* d_ktab32, void* stream);
 
 /* Per-row array of an index with the full suffix array: d_rows[r] = {SA[r], the (up to) 16 symbols of d_text before SA[r], symbol SA[r]-1
  * in the two lowest bits} for r in [0, length] ((length + 1) * 8 bytes: 15.2 GB at 1.9 Gbp).  Row 0 (SA = 0xFFFFFFFF) gets context 0,

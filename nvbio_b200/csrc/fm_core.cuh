@@ -30,7 +30,9 @@ struct FmIndex {
     uint32_t ktab_located;         // 1: table entries are 16 bytes {x, y, SA[x], SA[y]} (SA values filled for ranges of one or two rows; nvb_fm_build_ktab_located)
                                    // 2: the same, and the last word of a ONE-row entry holds the 16 text symbols before SA[x] (nvb_fm_build_ktab_context)
     const uint2*    rows;          // optional, with a context table: {SA[r], the 16 text symbols before SA[r]} for every row r (nvb_fm_build_rows;
-                                   // nvb_fm_index.ktab_located == 3, which is 2 here plus this array)
+                                   // nvb_fm_index.ktab_located == 3 or 5, which is 2 here plus this array)
+    uint32_t ktab_wide;            // 1: 32-byte entries (nvb_fm_build_ktab_wide; nvb_fm_index.ktab_located 4 / 5, ktab_located 2 here): the first
+                                   // 16 bytes as at level 2, k-mers with 3 to 8 occurrences also carry their rows' contexts (see ktab_wide_fill)
     // constant-index selects keep the struct in the kernel-parameter constant bank (a dynamic L2[c]
     // would force a local-memory copy of the whole struct)
     __host__ __device__ __forceinline__ uint32_t l2(uint32_t c) const {
@@ -45,8 +47,10 @@ static inline bool valid_fmindex(const nvb_fm_index* f) {
     if (!f || !f->d_bwt_occ) return false;
     const uint32_t I = f->sa_interval;
     if (I != 0 && (I & (I - 1)) != 0) return false;           // power of two
-    if (f->d_ktab && (f->ktab_k < 1 || f->ktab_k > 16 || f->ktab_located > 3u)) return false;
-    if (f->d_ktab && f->ktab_located == 3u && (f->sa_interval != 1u || !f->d_ssa || !f->d_rows)) return false;
+    if (f->d_ktab && (f->ktab_k < 1 || f->ktab_k > 16 || f->ktab_located > 5u)) return false;
+    if (f->d_ktab && f->ktab_located >= 3u && (f->sa_interval != 1u || !f->d_ssa)) return false;
+    if (f->d_ktab && f->ktab_located >= 4u && ((uintptr_t)f->d_ktab & 31u)) return false;
+    if (f->d_ktab && (f->ktab_located == 3u || f->ktab_located == 5u) && !f->d_rows) return false;
     return true;
 }
 static inline FmIndex make_fmindex(const nvb_fm_index* f) {
@@ -57,9 +61,10 @@ static inline FmIndex make_fmindex(const nvb_fm_index* f) {
     r.sa_shift = 0; while ((1u << r.sa_shift) < I) ++r.sa_shift;
     r.sa_mask = (1u << r.sa_shift) - 1u;
     r.ktab = (const uint2*)f->d_ktab; r.ktab_k = f->d_ktab ? f->ktab_k : 0u;
-    // d_rows is read only at level 3: callers that fill the struct field by field and stop at ktab_located leave it undefined
-    const bool with_rows = f->d_ktab && f->ktab_located == 3u;
-    r.ktab_located = f->d_ktab ? (with_rows ? 2u : f->ktab_located) : 0u;
+    // d_rows is read only at levels 3 and 5: callers that fill the struct field by field and stop at ktab_located leave it undefined
+    const bool with_rows = f->d_ktab && (f->ktab_located == 3u || f->ktab_located == 5u);
+    r.ktab_wide = (f->d_ktab && f->ktab_located >= 4u) ? 1u : 0u;
+    r.ktab_located = f->d_ktab ? (f->ktab_located >= 2u ? 2u : f->ktab_located) : 0u;
     r.rows = with_rows ? (const uint2*)f->d_rows : nullptr;
     return r;
 }
@@ -269,6 +274,79 @@ __host__ __device__ __forceinline__ bool ktab_two_row_marker(const FmIndex& f, c
     return f.ktab_located == 2u && f.n < KTAB_TWO_ROW_MARK && y >= KTAB_TWO_ROW_MARK;
 }
 
+// the (up to) `want` text symbols before pos, symbol pos-1 in the lowest two bits (none for the `$` row, pos symbols when pos < want)
+__host__ __device__ __forceinline__ uint32_t text_before(const uint32_t* __restrict__ text, const uint32_t pos, const uint32_t want)
+{
+    const uint32_t cnt = (pos == 0xFFFFFFFFu) ? 0u : (pos < want ? pos : want);
+    return cnt ? (be2_window(text, pos - cnt, cnt) >> (32u - 2u * cnt)) : 0u;
+}
+
+// Wide context tables (nvb_fm_build_ktab_wide): 32-byte entries w[0..7], one DRAM sector, whose first 16 bytes are the level-2 entry for
+// k-mers with at most two occurrences and the empty range.  A k-mer with 3 to KTAB_WIDE_ROWS occurrences (rows x..y) also carries, in
+// the words that level 2 leaves zero:
+//     3 rows:     {x, y, SA[x], SA[x+1], SA[x+2], ctx16(x), ctx16(x+1), ctx16(x+2)}
+//     4 rows:     {x, y, ctx8(x) | ctx8(x+1) << 16, ctx8(x+2) | ctx8(x+3) << 16, SA[x], SA[x+1], SA[x+2], SA[x+3]}
+//     5-8 rows:   {x, y, ctx8 of rows x, x+1 | x+2, x+3 | ... (two per word, words 2..5), 0, ...}
+// ctxN(r) = the N text symbols before SA[r] (text_before).  Wider ranges are {x, y, 0, ...}.
+constexpr uint32_t KTAB_WIDE_ROWS = 8;
+__host__ __device__ __forceinline__ void ktab_wide_fill(const uint32_t* __restrict__ sa, const uint32_t* __restrict__ text, uint32_t n,
+                                                        uint32_t x, uint32_t y, uint32_t (&w)[8])
+{
+#pragma unroll
+    for (int i = 0; i < 8; ++i) w[i] = 0u;
+    w[0] = x; w[1] = y;
+    if (x > y) return;
+    const uint32_t d = y - x;
+    if (d == 0u) { w[2] = sa[x]; w[3] = text_before(text, w[2], 16u); return; }
+    if (d == 1u) {
+        w[2] = sa[x]; w[3] = sa[y];
+        if (n < KTAB_TWO_ROW_MARK) w[1] = KTAB_TWO_ROW_MARK | text_before(text, w[2], 7u) | (text_before(text, w[3], 7u) << 14);
+        return;
+    }
+    if (d == 2u) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) { w[2 + i] = sa[x + i]; w[5 + i] = text_before(text, w[2 + i], 16u); }
+        return;
+    }
+    if (d >= KTAB_WIDE_ROWS) return;
+#pragma unroll
+    for (uint32_t i = 0; i < KTAB_WIDE_ROWS; ++i) {
+        if (i > d) continue;
+        const uint32_t pos = sa[x + i];
+        w[2 + i / 2u] |= text_before(text, pos, 8u) << (16u * (i & 1u));
+        if (d == 3u) w[4 + i] = pos;
+    }
+}
+// row x + i of a wide entry {lo, hi} with 3 (`three`) or 4..8 rows: its context (16 or 8 symbols) and, for 3 or 4 rows, its SA value
+__host__ __device__ __forceinline__ uint32_t ktab_wide_context(const uint4& lo, const uint4& hi, bool three, uint32_t i)
+{
+    if (three) return i == 0u ? hi.y : (i == 1u ? hi.z : hi.w);
+    const uint32_t w = i < 2u ? lo.z : (i < 4u ? lo.w : (i < 6u ? hi.x : hi.y));
+    return (i & 1u) ? (w >> 16) : (w & 0xFFFFu);
+}
+__host__ __device__ __forceinline__ uint32_t ktab_wide_sa(const uint4& lo, const uint4& hi, bool three, uint32_t i)
+{
+    if (three) return i == 0u ? lo.z : (i == 1u ? lo.w : hi.x);
+    return i == 0u ? hi.x : (i == 1u ? hi.y : (i == 2u ? hi.z : hi.w));
+}
+
+// the k-mer table entry u: 16 bytes into lo, and with a wide table the other 16 bytes of its sector into hi (else hi is left untouched),
+// both loads issued together
+__host__ __device__ __forceinline__ void gather_ktab_entry(const FmIndex& f, uint32_t u, uint4& lo, uint4& hi)
+{
+    const uint4* p = (const uint4*)f.ktab + ((uint64_t)u << f.ktab_wide);        // 4^16 x 32 B does not fit 32 bits
+#ifdef __CUDA_ARCH__
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %9, 0;\n\t"
+                 "ld.global.nc" NVB_FM_LD_QUAL ".v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "@p ld.global.nc" NVB_FM_LD_QUAL ".v4.u32 {%4,%5,%6,%7}, [%8+16];\n\t}"
+                 : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w), "+r"(hi.x), "+r"(hi.y), "+r"(hi.z), "+r"(hi.w)
+                 : "l"(p), "r"(f.ktab_wide));
+#else
+    lo = p[0];
+    if (f.ktab_wide) hi = p[1];
+#endif
+}
+
 // match() of one query read through a SymReader; FORWARD consumes left-to-right, COMPLEMENT maps
 // c<4 -> 3-c (nvBowtie's reverse-complement seed search over the forward index).
 template <int BITS, bool BE>
@@ -298,7 +376,8 @@ __host__ __device__ __forceinline__ void fm_match_one(const FmIndex& f, const ui
             }
         }
         if (!has_n) {                                   // an N among them: take the step-by-step path below
-            const uint2 r = gather_u2(f.ktab_located ? (const uint2*)((const uint4*)f.ktab + u) : f.ktab + u);
+            // (ranges only: the first 8 bytes of a 16- or 32-byte entry)
+            const uint2 r = gather_u2(f.ktab_located ? (const uint2*)((const uint4*)f.ktab + ((uint64_t)u << f.ktab_wide)) : f.ktab + u);
             x = r.x; y = ktab_two_row_marker(f, r.y) ? r.x + 1u : r.y; s = f.ktab_k;
         }
     }
@@ -375,7 +454,8 @@ constexpr uint32_t FM_ROWS_MAX = 8;
 // position x).  Backward order only (flags == 0); symbols > 3 never match.
 // MODE (the seed-match stage splits its seeds by how many dependent gathers they need, so that a warp does not wait on its slowest
 // lane): FM_WHOLE = everything in one call;  FM_DEFER = stop after the table look-up when the k-mer occurs three or more times (or
-// twice, with both occurrences spelling the whole query) and return FM_DEFERRED with the range reached so far in (ox, oy);
+// twice, with both occurrences spelling the whole query; with a wide table, only when the entry's contexts do not decide the seed) and
+// return FM_DEFERRED with the range reached so far in (ox, oy);
 // FM_RESUME = continue such a query: (ox, oy) hold that range on entry, the first ktab_k steps are taken as done ((0, n) = none).
 enum { FM_EMPTY = 0, FM_RANGE = 1, FM_LOCATED = 2, FM_DEFERRED = 3 };
 enum { FM_WHOLE = 0, FM_DEFER = 1, FM_RESUME = 2 };
@@ -387,6 +467,7 @@ __host__ __device__ __forceinline__ uint32_t fm_match_locate_one(const FmIndex& 
     SymReader<BITS, BE> rd(words);
     uint32_t x = 0, y = f.n, s = 0;
     uint32_t known_pos = 0u, known_pos2 = 0u, ctx2 = 0u; bool have_pos = false, have_two = false, two_ctx = false;
+    uint4 e = make_uint4(0u, 0u, 0u, 0u), e_hi = make_uint4(0u, 0u, 0u, 0u);     // the table entry (e_hi: second half of a wide one)
     if (MODE == FM_RESUME) { x = ox; y = oy; s = (x == 0u && y == f.n) ? 0u : f.ktab_k; }   // (0, n): deferred before any step (no look-up: an N, a short query)
     if (MODE != FM_RESUME && f.ktab_k && len >= f.ktab_k) {
         uint32_t u = 0; bool has_n = false;
@@ -404,7 +485,7 @@ __host__ __device__ __forceinline__ uint32_t fm_match_locate_one(const FmIndex& 
         }
         if (!has_n) {
             if (f.ktab_located) {                       // the entry of a single-row k-mer carries SA[x]: no SA gather below
-                const uint4 e = gather_u4((const uint4*)f.ktab + u);
+                gather_ktab_entry(f, u, e, e_hi);
                 x = e.x; y = e.y; known_pos = e.z; known_pos2 = e.w;
                 if (ktab_two_row_marker(f, y)) { ctx2 = y; y = x + 1u; two_ctx = true; }
                 have_pos = (x == y); have_two = (y == x + 1u);
@@ -457,6 +538,35 @@ __host__ __device__ __forceinline__ uint32_t fm_match_locate_one(const FmIndex& 
         }
         if (!m0 && !m1) return FM_EMPTY;
         if (m0 != m1) { ox = (m0 ? known_pos : known_pos2) - rem; oy = 0xFFFFFFFFu; return FM_LOCATED; }
+    }
+    if (MODE != FM_RESUME && f.ktab_wide && full_sa && s == f.ktab_k && s < len && y - x >= 2u && y - x < KTAB_WIDE_ROWS) {
+        // a k-mer with 3..8 occurrences on a wide table: the rule of the per-row array below, decided on the contexts that came with the
+        // look-up.  They are 16 symbols long for 3 rows and 8 for 4..8, so the unread symbols are compared over min(rem, width) of them:
+        // no survivor = empty (exact: a longer remainder or a short context near the text start can only add survivors); with 3 or 4 rows
+        // (whose SA values are in the entry too) and rem <= width, one survivor that is also the only row matching the rem - 1 closest
+        // symbols = located.  Anything else is deferred or walked as without the wide half.
+        const uint32_t rem = len - s, cnt = rem < 16u ? rem : 16u;
+        const bool three = (y - x == 2u);
+        const uint32_t width = three ? 16u : 8u, wc = cnt < width ? cnt : width;
+        bool n_left = false;
+        const uint32_t qw = unread_context<BITS, BE>(words, off + rem - cnt, cnt, n_left);     // the cnt unread symbols closest to the k-mer
+        if (!n_left) {
+            uint32_t full = 0u, near = 0u, hit = 0u;
+#pragma unroll
+            for (uint32_t i = 0; i < KTAB_WIDE_ROWS; ++i) {
+                if (i > y - x) continue;
+                const uint32_t c = ktab_wide_context(e, e_hi, three, i);
+                if (context_equal(qw, c, wc)) { ++full; hit = i; }
+                near += context_equal(qw, c, wc - 1u) ? 1u : 0u;
+            }
+            if (full == 0u) return FM_EMPTY;
+            if (full == 1u && near == 1u && y - x <= 3u && rem <= width) {
+                const uint32_t pos = ktab_wide_sa(e, e_hi, three, hit);
+                if (pos == 0xFFFFFFFFu || pos < rem) return FM_EMPTY;
+                ox = pos - rem; oy = 0xFFFFFFFFu;
+                return FM_LOCATED;
+            }
+        }
     }
     if (MODE != FM_DEFER && f.rows && full_sa && s == f.ktab_k && s < len && y - x >= 2u && y - x < FM_ROWS_MAX && len - s <= 16u) {
         // a k-mer with 3..FM_ROWS_MAX occurrences, on an index with the per-row array: the rows' contexts are compared with the unread

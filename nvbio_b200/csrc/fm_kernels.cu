@@ -117,18 +117,20 @@ fm_ktab_level_kernel(const FmIndex f, uint2* __restrict__ tab, uint32_t prev_ent
     }
 }
 
-// the same with 16-byte entries {x, y, -, -}, and the pass that fills the SA values into the one- and two-row ones
+// the same with 16-byte entries {x, y, -, -} (STRIDE 1) or the first half of 32-byte ones (STRIDE 2: the other half is filled by
+// fm_ktab32_fill_kernel), and the pass that fills the SA values into the one- and two-row 16-byte ones
+template <uint32_t STRIDE>
 __global__ void __launch_bounds__(FM_BLOCKDIM)
 fm_ktab16_level_kernel(const FmIndex f, uint4* __restrict__ tab, uint32_t prev_entries)
 {
     const uint32_t v = blockIdx.x * FM_BLOCKDIM + threadIdx.x;
     if (v >= prev_entries) return;
-    const uint4 r = tab[v];
+    const uint4 r = tab[(size_t)v * STRIDE];
 #pragma unroll
     for (int c = 3; c >= 0; --c) {
         uint32_t x = r.x, y = r.y;
         if (x <= y) fm_step(f, (uint32_t)c, x, y);
-        tab[(size_t)c * prev_entries + v] = make_uint4(x, y, 0u, 0u);
+        tab[((size_t)c * prev_entries + v) * STRIDE] = make_uint4(x, y, 0u, 0u);
     }
 }
 __global__ void __launch_bounds__(FM_BLOCKDIM)
@@ -144,11 +146,6 @@ fm_ktab16_locate_kernel(const FmIndex f, uint4* __restrict__ tab, uint64_t entri
 
 // one-row entries of a located table: .w = the (up to) 16 text symbols before SA[x], symbol SA[x]-1 in the lowest two bits;
 // two-row entries (index with fewer than 0xC0000000 rows): .y = marker | the 7 symbols before SA[x] | those before SA[x+1] << 14
-__device__ __forceinline__ uint32_t text_before(const uint32_t* __restrict__ text, const uint32_t pos, const uint32_t want)
-{
-    const uint32_t cnt = (pos == 0xFFFFFFFFu) ? 0u : (pos < want ? pos : want);
-    return cnt ? (be2_window(text, pos - cnt, cnt) >> (32u - 2u * cnt)) : 0u;
-}
 __global__ void __launch_bounds__(FM_BLOCKDIM)
 fm_ktab16_context_kernel(const uint32_t* __restrict__ text, uint4* __restrict__ tab, uint64_t entries, uint32_t n_rows)
 {
@@ -168,6 +165,19 @@ fm_rows_kernel(const uint32_t* __restrict__ sa, const uint32_t* __restrict__ tex
     if (r >= n_rows) return;
     const uint32_t pos = sa[r];
     rows[r] = make_uint2(pos, text_before(text, pos, 16u));
+}
+
+// every 32-byte entry of a wide table from its range {x, y} (left in its first half by the level kernels): ktab_wide_fill
+__global__ void __launch_bounds__(FM_BLOCKDIM)
+fm_ktab32_fill_kernel(const uint32_t* __restrict__ sa, const uint32_t* __restrict__ text, uint4* __restrict__ tab, uint64_t entries, uint32_t n)
+{
+    const uint64_t v = (uint64_t)blockIdx.x * FM_BLOCKDIM + threadIdx.x;
+    if (v >= entries) return;
+    const uint4 e = tab[2u * v];
+    uint32_t w[8];
+    ktab_wide_fill(sa, text, n, e.x, e.y, w);
+    tab[2u * v] = make_uint4(w[0], w[1], w[2], w[3]);
+    tab[2u * v + 1u] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 
 // range sizes as uint64 (filter_inl.h:36-42: 1 + y - x in uint32 arithmetic, widened)
@@ -337,7 +347,7 @@ int nvb_fm_build_ktab_located(const nvb_fm_index* fmi, uint32_t k, void* d_ktab1
     NVB_CUDA_TRY(cudaStreamSynchronize(s));              // `root` lives on this stack frame
     uint32_t prev = 1;
     for (uint32_t t = 1; t <= k; ++t, prev *= 4u) {
-        fm_ktab16_level_kernel<<<(prev + FM_BLOCKDIM - 1) / FM_BLOCKDIM, FM_BLOCKDIM, 0, s>>>(f, (uint4*)d_ktab16, prev);
+        fm_ktab16_level_kernel<1><<<(prev + FM_BLOCKDIM - 1) / FM_BLOCKDIM, FM_BLOCKDIM, 0, s>>>(f, (uint4*)d_ktab16, prev);
         NVB_LAUNCH_CHECK();
     }
     const uint64_t entries = 1ull << (2u * k);
@@ -353,6 +363,27 @@ int nvb_fm_build_ktab_context(const nvb_fm_index* fmi, uint32_t k, const uint32_
     if (r != NVB_OK) return r;
     const uint64_t entries = 1ull << (2u * k);
     fm_ktab16_context_kernel<<<(uint32_t)((entries + FM_BLOCKDIM - 1) / FM_BLOCKDIM), FM_BLOCKDIM, 0, as_stream(stream)>>>(d_text, (uint4*)d_ktab16, entries, fmi->length);
+    NVB_LAUNCH_CHECK();
+    return NVB_OK;
+}
+
+int nvb_fm_build_ktab_wide(const nvb_fm_index* fmi, uint32_t k, const uint32_t* d_text, void* d_ktab32, void* stream)
+{
+    if (!valid_fmindex(fmi) || k < 1 || k > 16 || !d_text || !d_ktab32 || ((uintptr_t)d_ktab32 & 31u)) return NVB_E_INVALID;
+    if (fmi->sa_interval != 1u || !fmi->d_ssa) return NVB_E_UNSUPPORTED;
+    nvb_fm_index plain = *fmi; plain.d_ktab = nullptr; plain.ktab_k = 0; plain.ktab_located = 0;
+    const FmIndex f = make_fmindex(&plain);
+    cudaStream_t s = as_stream(stream);
+    const uint4 root = make_uint4(0u, fmi->length, 0u, 0u);
+    NVB_CUDA_TRY(cudaMemcpyAsync(d_ktab32, &root, sizeof(uint4), cudaMemcpyHostToDevice, s));
+    NVB_CUDA_TRY(cudaStreamSynchronize(s));              // `root` lives on this stack frame
+    uint32_t prev = 1;
+    for (uint32_t t = 1; t <= k; ++t, prev *= 4u) {
+        fm_ktab16_level_kernel<2><<<(prev + FM_BLOCKDIM - 1) / FM_BLOCKDIM, FM_BLOCKDIM, 0, s>>>(f, (uint4*)d_ktab32, prev);
+        NVB_LAUNCH_CHECK();
+    }
+    const uint64_t entries = 1ull << (2u * k);
+    fm_ktab32_fill_kernel<<<(uint32_t)((entries + FM_BLOCKDIM - 1) / FM_BLOCKDIM), FM_BLOCKDIM, 0, s>>>(fmi->d_ssa, d_text, (uint4*)d_ktab32, entries, fmi->length);
     NVB_LAUNCH_CHECK();
     return NVB_OK;
 }

@@ -41,6 +41,7 @@ class FMIndexDevice:
         self.sa_interval = int(sa_interval)        # 16 = the reference's SA_INT; 1 = full suffix array
         self.ktab, self.ktab_k = ktab, int(ktab_k)  # optional k-mer range table (an extension)
         self.ktab_located = 0                       # 1: 16-byte entries {x, y, SA[x], SA[y]} (build_ktab(k, located=True)); 2: + text context (text=...)
+        self.ktab_wide = False                      # with ktab_located == 2: 32-byte entries (nvb_fm_build_ktab_wide)
         self.rows = None                            # with a context table: {SA[r], 16 symbols before SA[r]} per row (nvb_fm_build_rows)
 
     # -- views ------------------------------------------------------------------------------
@@ -55,8 +56,10 @@ class FMIndexDevice:
         s.d_ktab = self.ktab.data_ptr() if self.ktab is not None else None
         s.ktab_k = self.ktab_k if self.ktab is not None else 0
         s.ktab_located = int(self.ktab_located) if self.ktab is not None else 0
-        if s.ktab_located == 2 and self.rows is not None:
-            s.ktab_located, s.d_rows = 3, self.rows.data_ptr()
+        if s.ktab_located == 2 and self.ktab_wide:
+            s.ktab_located = 4
+        if s.ktab_located in (2, 4) and self.rows is not None:
+            s.ktab_located, s.d_rows = s.ktab_located + 1, self.rows.data_ptr()
         return s
 
     @property
@@ -73,12 +76,27 @@ class FMIndexDevice:
         itself.  With text (the 2-bit big-endian words the index was built from) one-row entries also carry the 16 symbols before
         SA[x] (nvb_fm_build_ktab_context): such a seed needs no read of the text at all.  With the full suffix array and text, the
         per-row array `rows` (nvb_fm_build_rows, (n + 1) x 8 bytes) is built as well when it fits the device's free memory: seeds whose
-        k-mer occurs 3 to 8 times are then resolved by one gather of their rows.  Results are the same with and without it."""
+        k-mer occurs 3 to 8 times are then resolved by one gather of their rows.  Results are the same with and without it.
+        With the full suffix array and text, when a 16-byte table would not fit the device's L2 cache (so that every look-up is a DRAM
+        request) and a 32-byte one leaves ROWS_HEADROOM free, the table gets 32-byte entries instead (nvb_fm_build_ktab_wide,
+        ktab_wide): the look-up then also carries the contexts of k-mers with 3 to 8 occurrences, and most such seeds need no further
+        gather."""
         self.ktab = None                                   # release a previous table (and rows) before allocating the new one
         self.rows = None
-        tab = torch.empty((4 ** k, 4 if located else 2), dtype=torch.int32, device=self.device)
+        self.ktab_wide = False
+        full_text = located and text is not None and self.sa_interval == 1 and self.ssa is not None
+        wide = False
+        if full_text:
+            l2 = torch.cuda.get_device_properties(self.device).L2_cache_size
+            free, _ = torch.cuda.mem_get_info(self.device)
+            wide = 4 ** k * 16 > l2 and 4 ** k * 32 + ROWS_HEADROOM <= free
+        tab = torch.empty((4 ** k, 8 if wide else (4 if located else 2)), dtype=torch.int32, device=self.device)
         s = self.struct()
-        if located and text is not None:
+        if wide:
+            assert text.is_cuda and text.dtype == torch.int32
+            check(lib().nvb_fm_build_ktab_wide(C.byref(s), C.c_uint32(k), C.c_void_p(text.data_ptr()), C.c_void_p(tab.data_ptr()), _stream()),
+                  "nvb_fm_build_ktab_wide")
+        elif located and text is not None:
             assert text.is_cuda and text.dtype == torch.int32
             check(lib().nvb_fm_build_ktab_context(C.byref(s), C.c_uint32(k), C.c_void_p(text.data_ptr()), C.c_void_p(tab.data_ptr()), _stream()),
                   "nvb_fm_build_ktab_context")
@@ -87,7 +105,8 @@ class FMIndexDevice:
         else:
             check(lib().nvb_fm_build_ktab(C.byref(s), C.c_uint32(k), C.c_void_p(tab.data_ptr()), _stream()), "nvb_fm_build_ktab")
         self.ktab, self.ktab_k, self.ktab_located = tab, k, (2 if (located and text is not None) else (1 if located else 0))
-        if self.ktab_located == 2 and self.sa_interval == 1 and self.ssa is not None:
+        self.ktab_wide = wide
+        if full_text:
             need = (self.length + 1) * 8
             free, _ = torch.cuda.mem_get_info(self.device)
             if need + ROWS_HEADROOM <= free:
