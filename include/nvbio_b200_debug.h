@@ -33,10 +33,14 @@ void nvb_debug_pipeline_path(int path);
    by a second kernel, 0 = one pass.  Same results; for A/B timing and tests */
 void nvb_debug_seed_split(int on);
 
-/* extension stage of the per-read path (LOCAL, constant scheme, 2-bit reads): 1 (default) = a read that equals its window on a band
-   diagonal gets score = match * len and its sink without running the DP (exact: nothing can score more), 0 = every job through the
+/* extension stage of the per-read path (LOCAL, constant scheme, 2-bit reads): 1 (default) = a job whose result the exact shortcut
+   proves (the best segment of the seed's band diagonal beats every gapped alignment and every other diagonal) gets it without running
+   the DP, 2 = the same without the one-gap check (only jobs whose segment beats every alignment with a gap), 0 = every job through the
    DP kernels.  Same results; for A/B timing and tests */
 void nvb_debug_perfect_shortcut(int on);
+/* *n = the number of alignment jobs the last per-read call with the exact shortcut left to the DP kernels.  Reads the caller's temp
+   buffer of that call, so only while it is still allocated; synchronises the device */
+int nvb_debug_dp_jobs(uint32_t* n);
 
 /* the device build of the MAPQ function of nvb_seed_extend_mapq over n points (device arrays): d_mapq[i] = BowtieMapq2 of an unpaired
    read with best score d_best[i], a second score d_second[i] when d_has_second[i] != 0, perfect_score = d_len[i] * d_match_bonus[i],

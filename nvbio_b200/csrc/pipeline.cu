@@ -341,9 +341,11 @@ pipe_read_jobs_kernel(const FmIndex f, const PipeGeom g, const uint2* __restrict
 
 // Exact shortcut of the LOCAL extension (gapless_job_shortcut, pipeline_core.cuh): jobs whose result it proves get it here; the others
 // are compacted into the list the DP kernels run over.  (Earlier versions of the check: all band diagonals for every job 0.39 ms per
-// million reads, a symbol-by-symbol segment loop 0.29 ms, per-diagonal text reads 0.22 ms; now 0.14 ms.)
+// million reads, a symbol-by-symbol segment loop 0.29 ms, per-diagonal text reads 0.22 ms, four text words in registers 0.14 ms; with
+// the one-gap check 0.25 ms, which takes a third of the jobs off the DP.)  one_gap = false: the rule without it (nvb_debug_perfect_shortcut(2))
 __global__ void __launch_bounds__(256)
-pipe_perfect_jobs_kernel(const PipeGeom g, const int32_t match, const int32_t mismatch, const int32_t max_gap_open, const uint32_t* __restrict__ counts,
+pipe_perfect_jobs_kernel(const PipeGeom g, const int32_t match, const int32_t mismatch, const int32_t max_gap_open, const bool one_gap,
+                         const uint32_t* __restrict__ counts,
                          const uint32_t* __restrict__ str_words, const uint32_t* __restrict__ genome,
                          const uint32_t* __restrict__ jp_off, const uint32_t* __restrict__ jp_len,
                          const uint32_t* __restrict__ jt_off, const uint32_t* __restrict__ jt_len,
@@ -360,7 +362,7 @@ pipe_perfect_jobs_kernel(const PipeGeom g, const int32_t match, const int32_t mi
         if (j < n) {
             po = jp_off[j]; M = jp_len[j]; to = jt_off[j]; N = jt_len[j];
             int32_t score = 0; uint32_t sx = 0, sy = 0;
-            if (gapless_job_shortcut(str_words, genome, po, M, to, N, g.band, match, mismatch, max_gap_open, score, sx, sy)) {
+            if (gapless_job_shortcut(str_words, genome, po, M, to, N, g.band, match, mismatch, max_gap_open, score, sx, sy, one_gap)) {
                 job_score[j] = score; job_sink[j] = make_uint2(sx, sy);
             } else todo = true;
         }
@@ -898,7 +900,8 @@ extern "C" int nvb_seed_extend_stage_ms(float ms[7])
     return NVB_OK;
 }
 
-static int g_perfect_shortcut = 1;     // 0 = every alignment job through the DP kernels (nvb_debug_perfect_shortcut)
+static int g_perfect_shortcut = 1;     // 0 = every alignment job through the DP kernels, 2 = without the one-gap check (nvb_debug_perfect_shortcut)
+static const uint32_t* g_last_dp_count = nullptr;   // the last per-read call's count of jobs left to the DP (nvb_debug_dp_jobs)
 static int g_seed_split = 1;           // 0 = the located seed match in one pass (nvb_debug_seed_split)
 static int g_pipe_path = 0;            // 1 = always the per-hit path, anything else = automatic (nvb_debug_pipeline_path)
 
@@ -1076,10 +1079,12 @@ struct PipeCall {
         if (cap && eligible && g_perfect_shortcut) {
             const uint32_t jgrid = hgrid < sm_count() * 8u ? hgrid : sm_count() * 8u;
             NVB_CUDA_TRY(cudaMemsetAsync(dp_count, 0, sizeof(uint32_t), s));
-            pipe_perfect_jobs_kernel<<<jgrid, 256, 0, s>>>(g, SC.match, SC.mismatch, SC.pattern_gap_open > SC.text_gap_open ? SC.pattern_gap_open : SC.text_gap_open, counts, str_words, genome,
+            pipe_perfect_jobs_kernel<<<jgrid, 256, 0, s>>>(g, SC.match, SC.mismatch, SC.pattern_gap_open > SC.text_gap_open ? SC.pattern_gap_open : SC.text_gap_open,
+                                                           g_perfect_shortcut != 2, counts, str_words, genome,
                                                            jobs.p_off, jobs.p_len, jobs.t_off, jobs.t_len, job_score, job_sink,
                                                            dp.p_off, dp.p_len, dp.t_off, dp.t_len, dp_job, dp_count);
             NVB_LAUNCH_CHECK();
+            g_last_dp_count = dp_count;
             NVB_TRY(score_jobs(dp, dp_count, dp_score, dp_sink));
             pipe_scatter_dp_kernel<<<jgrid, 256, 0, s>>>(dp_count, dp_job, dp_score, dp_sink, job_score, job_sink);
             NVB_LAUNCH_CHECK();
@@ -1338,6 +1343,13 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
 extern "C" void nvb_debug_pipeline_path(int path) { g_pipe_path = path; }
 extern "C" void nvb_debug_seed_split(int on) { g_seed_split = on; }
 extern "C" void nvb_debug_perfect_shortcut(int on) { g_perfect_shortcut = on; }
+extern "C" int nvb_debug_dp_jobs(uint32_t* n)
+{
+    if (!n || !g_last_dp_count) return NVB_E_INVALID;
+    NVB_CUDA_TRY(cudaDeviceSynchronize());
+    NVB_CUDA_TRY(cudaMemcpy(n, g_last_dp_count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    return NVB_OK;
+}
 
 extern "C" int nvb_seed_extend(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     const nvb_string_set* reads, uint32_t n_reads,
