@@ -506,8 +506,8 @@ int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
  *     anchor).  No candidate: the pair is UNPAIRED and each mate keeps its own best alignment.
  * A mate's alignment BEGIN is taken as (end - read length, clamped at 0), not from a traceback: with soft clips or indels the true
  * start differs by a few bases, so pairs within that distance of min_frag / max_frag may be classified differently from a
- * caller that traces every alignment (nvBowtie does); callers that need the exact extent can request the traceback
- * (nvb_seed_extend_traceback) and re-check those pairs.
+ * caller that traces every alignment (nvBowtie does); callers that need the exact extent of both mates, rescued ones included, can
+ * call nvb_seed_extend_paired_traceback and re-check those pairs.
  * At most rescue_capacity full-DP jobs are run per call (in pair order; d_n_rescue[1] reports how many were wanted).
  * Outputs (mate m of pair p at index m*n_pairs + p): d_pair_score (sum of the two mates' scores, INT_MIN when unpaired),
  * d_pair_flags (NVB_PAIR_*), d_mate_score (INT_MIN = unaligned), d_mate_pos (genome coordinate one past the last aligned
@@ -569,6 +569,31 @@ int nvb_seed_extend_paired_mapq(const nvb_fm_index* fmi, const uint32_t* d_genom
                     const nvb_string_set* reads, uint32_t n_pairs,
                     const nvb_seed_extend_params* params, uint32_t hit_capacity,
                     const nvb_pair_params* pair_params, const nvb_pair_out* out,
+                    const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
+                    uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream);
+
+/* The alignment of both mates (what nvBowtie's paired aligner traces for SAM output, aligner_best_approx_paired.h:404-486).  Pairing,
+ * pair outputs and, with mapq / mapq_out (both NULL or both set), the MAPQ outputs are exactly those of nvb_seed_extend_paired /
+ * nvb_seed_extend_paired_mapq for the same inputs; concordance still uses begin = end - length.  mate_alignment is required and laid out
+ * over the 2*n_pairs mates (mate m of pair p at index m * n_pairs + p), its fields meaning what they mean in nvb_best_alignment_out;
+ * d_strand may be NULL (d_mate_strand holds the same).  Per mate:
+ *   - unaligned: n_ops = 0, begin = (0xFFFFFFFF, 0xFFFFFFFF);
+ *   - keeping its own single-end best (CONCORDANT and UNPAIRED pairs, the anchor of a rescued pair): the banded traceback of that
+ *     best (strand, window) job, equal to what nvb_seed_extend_traceback reports for the read when the 2*n_pairs mates run single end;
+ *   - rescued (NVB_PAIR_RESCUED_MATE1 / 2): the full-matrix traceback of the winning opposite-mate job (the mate on the rescue strand
+ *     against the rescue window), equal to nvb_gotoh_traceback of that job: begin = (window begin + source.x, source.y), the traced
+ *     score and end are d_mate_score / d_mate_pos.
+ * d_n_ops counts ops beyond max_ops without storing them.  NVB_E_INVALID when mate_alignment, d_ops, d_n_ops or d_begin is NULL,
+ * max_ops is 0, only one of mapq / mapq_out is set, or a validation of the two calls above fails; NVB_E_UNSUPPORTED when
+ * reads->length > 512 (nvBowtie's MAXIMUM_READ_LENGTH).  The temp size grows by the banded traceback's direction matrices for the
+ * 2*n_pairs mates (reads->length * ceil(band_len / 8) * 4 bytes per mate) plus a slot pool of the rescue traceback: one slot of
+ * (max_frag + 31) * 128 * ceil(ceil(reads->length / 32) / 8) bytes per resident warp (its occupancy times the SM count), whatever the
+ * number of rescues. */
+int nvb_seed_extend_paired_traceback(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_pairs,
+                    const nvb_seed_extend_params* params, uint32_t hit_capacity,
+                    const nvb_pair_params* pair_params, const nvb_pair_out* out,
+                    const nvb_best_alignment_out* mate_alignment,
                     const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream);
 

@@ -14,6 +14,10 @@ void nvb_debug_force_gotoh_path(int path);
 void nvb_debug_full_minb(int minb);
 /* full-matrix dispatch: 0 = by batch size, 1 = always the warp-per-pair kernel, 2 = never */
 void nvb_debug_full_warp(int mode);
+/* 1: nvb_gotoh_traceback runs the score dispatch, then the warp-per-alignment traceback of nvb_seed_extend_paired_traceback's rescued
+   mates from those sinks (its slot pool and window cuts; pattern lengths up to 512, else NVB_E_UNSUPPORTED), and its temp query answers
+   for that path; 0 (default): the one-alignment-per-thread direction-matrix kernel.  Same results; for tests of the warp kernel */
+void nvb_debug_full_traceback_warp(int on);
 /* 0: always the run-time-format pair kernel (PFMT 0); 1 (default): the compile-time 2- / 4-bit big-endian kernels where they apply */
 void nvb_debug_pair_format(int on);
 /* 1 (default): the banded pair kernels keep two pattern rows in flight per thread; 0: one row per loop iteration */

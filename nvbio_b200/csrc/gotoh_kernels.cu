@@ -11,6 +11,7 @@
 #include <atomic>
 #include "../../include/nvbio_b200_debug.h"
 #include "gotoh_full_core.cuh"
+#include "pipeline_core.cuh"
 
 namespace nvb {
 
@@ -466,6 +467,86 @@ gotoh_full_warp_kernel(const GotohScheme S, const GotohBatch b, uint32_t* __rest
     }
 }
 
+// full-matrix traceback from KNOWN sinks, one warp per alignment (FullTbLane, gotoh_full_core.cuh): item i = (alignment a, output slot);
+// a resident grid strides over the device-side item count, each warp owning one slot of `slot_words` direction words in `pool`.
+// Only text rows [r0, sink.x) are computed (full_traceback_first_row); lane 0 then walks the step-major matrix from the sink, which
+// the score pass already placed exactly where the reference does, so no LOCAL tie order is tracked here.
+// (FullTbOut, full_warp_traceback: gotoh_full_core.cuh)
+
+template <int TYPE, int W>
+__global__ void __launch_bounds__(WARP_BLOCKDIM)
+gotoh_full_warp_traceback_kernel(const GotohScheme S, const StrSet pat, const StrSet txt, const uint8_t* __restrict__ quals,
+                                 const int32_t* __restrict__ score, const uint2* __restrict__ sink,
+                                 const uint2* __restrict__ items, const uint32_t* __restrict__ n_items,
+                                 const FullTbOut o, uint32_t* __restrict__ pool, const uint32_t slot_words)
+{
+    constexpr uint32_t FULL = 0xFFFFFFFFu;
+    constexpr int NW = FullTbLane<W>::NW;
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t warp = (blockIdx.x * WARP_BLOCKDIM + threadIdx.x) >> 5, n_warps = (gridDim.x * WARP_BLOCKDIM) >> 5;
+    uint32_t* __restrict__ dirs = pool + (size_t)warp * slot_words;
+    const int32_t INF = SHRT_MIN - (S.pgo < S.pge ? S.pgo : S.pge);
+    // the largest substitution score (front cut of LOCAL windows)
+    int32_t s_max = S.match > S.mismatch ? S.match : S.mismatch;
+    if (S.qtab) {
+        s_max = INT_MIN;
+        for (uint32_t i = lane; i < 512u; i += 32u) s_max = imax2(s_max, S.qtab[i]);
+        s_max = __reduce_max_sync(FULL, s_max);
+    }
+    const uint32_t n = *n_items;
+    for (uint32_t i = warp; i < n; i += n_warps) {
+        const uint2 it = items[i];
+        const uint32_t a = it.x, out = it.y;
+        const uint2 sk = sink[a];
+        const uint32_t M = str_len(pat, a), c0 = lane * (uint32_t)W;
+        const uint32_t r0 = full_traceback_first_row(TYPE, sk.x, sk.y, score[a], s_max, S.pgo, S.pge);
+        const uint32_t R = sk.x - r0, L = (M + (uint32_t)W - 1u) / (uint32_t)W;
+        const uint32_t toff = str_off(txt, a) + r0;
+        FullTbLane<W> ln;
+        ln.template init<TYPE>(S, pat.words, pat.bits, pat.big_endian, str_off(pat, a), M, quals, c0, INF);
+        int32_t outH = 0, outE = 0;
+        uint32_t outG = 0u, myG = 0u;
+        const uint32_t steps = R + L - 1u;
+        for (uint32_t t = 0; t < steps; ++t) {
+            if ((t & 31u) == 0u) myG = (t + lane < R) ? sym_at_rt(txt.words, txt.bits, txt.big_endian, toff + t + lane) : 255u;
+            const uint32_t rowG = __shfl_sync(FULL, myG, t & 31u);
+            int32_t Hl = __shfl_up_sync(FULL, outH, 1), E = __shfl_up_sync(FULL, outE, 1);
+            uint32_t g = __shfl_up_sync(FULL, outG, 1);
+            const uint32_t r = t - lane;                                   // wraps for t < lane: then r >= R
+            if (lane == 0u) { full_first_column<TYPE>(S, r0 + r, INF, Hl, E); g = rowG; }
+            if (r < R && lane < L) {
+                uint32_t dw[NW];
+                ln.template row<TYPE>(S, g, Hl, E, dw);
+                outH = Hl; outE = E; outG = g;
+#pragma unroll
+                for (int w = 0; w < NW; ++w) dirs[((size_t)t * NW + w) * 32u + lane] = dw[w];
+            }
+        }
+        __syncwarp();
+        if (lane == 0u) {
+            SinkResult s; s.score = score[a]; s.x = R; s.y = sk.y;
+            uint32_t sx = 0u, sy = 0u;
+            const uint32_t cnt = gotoh_full_walk<TYPE>(FullDirsStepMajor{dirs, (uint32_t)W, (uint32_t)NW}, s, o.ops + (size_t)out * o.max_ops,
+                                                       o.max_ops, sx, sy);
+            o.source[out] = make_uint2((o.absolute ? str_off(txt, a) : 0u) + r0 + sx, sy);
+            o.n_ops[out] = cnt;
+        }
+        __syncwarp();                                                      // the slot is rewritten by the next item
+    }
+}
+
+// nvb_debug_full_traceback_warp: every alignment with a sink becomes an item (a, a); the others get no ops and source (-1, -1)
+__global__ void __launch_bounds__(256)
+full_tb_items_kernel(const uint32_t n, const uint2* __restrict__ sink, uint2* __restrict__ items, uint32_t* __restrict__ n_items,
+                     uint32_t* __restrict__ n_ops, uint2* __restrict__ source)
+{
+    const uint32_t a = blockIdx.x * 256 + threadIdx.x;
+    if (a >= n) return;
+    const uint2 k = sink[a];
+    if (k.x == 0xFFFFFFFFu || k.y == 0xFFFFFFFFu) { n_ops[a] = 0u; source[a] = make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu); return; }
+    items[atomicAdd(n_items, 1u)] = make_uint2(a, a);
+}
+
 template <int TYPE>
 __global__ void __launch_bounds__(GENERIC_BLOCKDIM)
 gotoh_full_todo_kernel(const GotohScheme S, const GotohBatch b, int2* __restrict__ col, const uint32_t* __restrict__ todo, const uint32_t* __restrict__ todo_count)
@@ -686,6 +767,43 @@ static int banded_impl(int band, int type, const nvb_gotoh_scheme* scheme,
     int r = dispatch_pair(band, type, S, b, sel_rows, todo, todo_count, s);
     if (r != NVB_OK) return r;
     return dispatch_generic(band, type, S, b, todo, todo_count, n_max, s);
+}
+
+// the warp traceback's launch: a resident grid (its measured occupancy times the SM count), one pool slot per warp
+template <int TYPE, int W>
+static int full_tb_launch(const FullTbArgs* a, uint32_t max_n, size_t* pool_bytes, cudaStream_t s)
+{
+    int per_sm = 0;
+    NVB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gotoh_full_warp_traceback_kernel<TYPE, W>, WARP_BLOCKDIM, 0));
+    const uint32_t grid = sm_count() * (uint32_t)(per_sm > 0 ? per_sm : 1);
+    const uint32_t slot_words = (max_n + 31u) * 32u * (uint32_t)FullTbLane<W>::NW;
+    *pool_bytes = (size_t)grid * (WARP_BLOCKDIM / 32) * slot_words * sizeof(uint32_t);
+    if (!a) return NVB_OK;
+    gotoh_full_warp_traceback_kernel<TYPE, W><<<grid, WARP_BLOCKDIM, 0, s>>>(a->S, a->pat, a->txt, a->quals, a->score, a->sink, a->items,
+                                                                            a->n_items, a->o, (uint32_t*)a->pool, slot_words);
+    NVB_LAUNCH_CHECK();
+    return NVB_OK;
+}
+
+int full_warp_traceback(int type, uint32_t max_m, uint32_t max_n, const FullTbArgs* a, size_t* pool_bytes, cudaStream_t s)
+{
+    if (max_m < 1u || max_m > FULL_TB_MAX_M || max_n > 65535u) return NVB_E_UNSUPPORTED;
+#define NVB_TB_W(T)                                                                                                                 \
+    switch ((max_m + 31u) / 32u) {                                                                                                  \
+    case 1:  return full_tb_launch<T, 1>(a, max_n, pool_bytes, s);  case 2:  return full_tb_launch<T, 2>(a, max_n, pool_bytes, s);   \
+    case 3:  return full_tb_launch<T, 3>(a, max_n, pool_bytes, s);  case 4:  return full_tb_launch<T, 4>(a, max_n, pool_bytes, s);   \
+    case 5:  return full_tb_launch<T, 5>(a, max_n, pool_bytes, s);  case 6:  return full_tb_launch<T, 6>(a, max_n, pool_bytes, s);   \
+    case 7:  return full_tb_launch<T, 7>(a, max_n, pool_bytes, s);  case 8:  return full_tb_launch<T, 8>(a, max_n, pool_bytes, s);   \
+    case 9:  return full_tb_launch<T, 9>(a, max_n, pool_bytes, s);  case 10: return full_tb_launch<T, 10>(a, max_n, pool_bytes, s);  \
+    case 11: return full_tb_launch<T, 11>(a, max_n, pool_bytes, s); case 12: return full_tb_launch<T, 12>(a, max_n, pool_bytes, s);  \
+    case 13: return full_tb_launch<T, 13>(a, max_n, pool_bytes, s); case 14: return full_tb_launch<T, 14>(a, max_n, pool_bytes, s);  \
+    case 15: return full_tb_launch<T, 15>(a, max_n, pool_bytes, s); default: return full_tb_launch<T, 16>(a, max_n, pool_bytes, s); }
+    switch (type) {
+    case NVB_GLOBAL: NVB_TB_W(NVB_GLOBAL)
+    case NVB_LOCAL:  NVB_TB_W(NVB_LOCAL)
+    default:         NVB_TB_W(NVB_SEMI_GLOBAL)
+    }
+#undef NVB_TB_W
 }
 
 } // namespace nvb
@@ -919,6 +1037,46 @@ int nvb_banded_gotoh_score_best2(int band_len, int type, const nvb_gotoh_scheme*
     }
 }
 
+static int g_full_tb_warp = 0;        // nvb_debug_full_traceback_warp(1): nvb_gotoh_traceback as the score dispatch + the warp traceback
+
+// nvb_gotoh_traceback with nvb_debug_full_traceback_warp(1): score + sink from the score dispatch, then gotoh_full_warp_traceback_kernel
+// from those sinks (its slot pool and window cuts) -- the path the paired-end traceback takes for rescued mates
+static int gotoh_traceback_warp(int type, const nvb_gotoh_scheme* scheme, const nvb_string_set* patterns, const uint8_t* d_quals,
+                                const nvb_string_set* texts, uint32_t n, int32_t* d_score, nvb_uint2* d_sink, nvb_uint2* d_source,
+                                uint8_t* d_ops, uint32_t max_ops, uint32_t* d_n_ops, void* d_temp, size_t* temp_bytes, void* stream)
+{
+    cudaStream_t s = as_stream(stream);
+    size_t score_bytes = 0, pool_bytes = 0;
+    {
+        const int r = gotoh_full_impl(type, scheme, patterns, d_quals, texts, nullptr, n, nullptr, nullptr, nullptr, &score_bytes, nullptr);
+        if (r != NVB_E_TEMP_SIZE && r != NVB_OK) return r;
+    }
+    { const int r = full_warp_traceback(type, patterns->length, texts->length, nullptr, &pool_bytes, s); if (r != NVB_OK) return r; }
+    TempCarver tc(d_temp);
+    char* score_tmp = tc.take<char>(score_bytes);
+    uint2* items = tc.take<uint2>(n ? n : 1u);
+    uint32_t* n_items = tc.take<uint32_t>(4);
+    void* pool = tc.take<char>(pool_bytes);
+    const size_t need = tc.total();
+    if (!d_temp || *temp_bytes < need) { *temp_bytes = need; return NVB_E_TEMP_SIZE; }
+    if (n == 0) return NVB_OK;
+    if (!d_score || !d_sink || !d_source || !d_ops || !d_n_ops || max_ops == 0) return NVB_E_INVALID;
+    {
+        size_t sb = score_bytes;
+        const int r = gotoh_full_impl(type, scheme, patterns, d_quals, texts, nullptr, n, d_score, d_sink, score_tmp, &sb, stream);
+        if (r != NVB_OK) return r;
+    }
+    NVB_CUDA_TRY(cudaMemsetAsync(n_items, 0, sizeof(uint32_t), s));
+    full_tb_items_kernel<<<(n + 255u) / 256u, 256, 0, s>>>(n, (const uint2*)d_sink, items, n_items, d_n_ops, (uint2*)d_source);
+    NVB_LAUNCH_CHECK();
+    FullTbArgs a;
+    a.S = make_scheme(scheme); a.pat = make_strset(patterns); a.txt = make_strset(texts); a.quals = d_quals;
+    a.score = d_score; a.sink = (const uint2*)d_sink; a.items = items; a.n_items = n_items;
+    a.o.ops = d_ops; a.o.n_ops = d_n_ops; a.o.source = (uint2*)d_source; a.o.max_ops = max_ops; a.o.absolute = 0u;
+    a.pool = pool;
+    return full_warp_traceback(type, patterns->length, texts->length, &a, &pool_bytes, s);
+}
+
 int nvb_gotoh_traceback(int type, const nvb_gotoh_scheme* scheme, const nvb_string_set* patterns, const uint8_t* d_quals, const nvb_string_set* texts, uint32_t n,
                         int32_t* d_score, nvb_uint2* d_sink, nvb_uint2* d_source,
                         uint8_t* d_ops, uint32_t max_ops, uint32_t* d_n_ops,
@@ -927,6 +1085,8 @@ int nvb_gotoh_traceback(int type, const nvb_gotoh_scheme* scheme, const nvb_stri
     if (!scheme || !temp_bytes || !valid_strset(patterns) || !valid_strset(texts)) return NVB_E_INVALID;
     if (type < 0 || type > 2) return NVB_E_INVALID;
     if (texts->length > 65535u || patterns->length > 65535u) return NVB_E_UNSUPPORTED;
+    if (g_full_tb_warp == 1)
+        return gotoh_traceback_warp(type, scheme, patterns, d_quals, texts, n, d_score, d_sink, d_source, d_ops, max_ops, d_n_ops, d_temp, temp_bytes, stream);
     const uint32_t max_m = patterns->length ? patterns->length : 1u, max_n = texts->length ? texts->length : 1u;
     const uint32_t dir_row_words = (max_m + 31u) / 32u * 4u;
     TempCarver tc(d_temp);
@@ -957,6 +1117,7 @@ int nvb_gotoh_traceback(int type, const nvb_gotoh_scheme* scheme, const nvb_stri
 void nvb_debug_force_gotoh_path(int path) { g_force_path = path; }
 void nvb_debug_full_minb(int minb) { g_full_minb = minb; }
 void nvb_debug_full_warp(int mode) { g_full_warp = mode; }
+void nvb_debug_full_traceback_warp(int on) { g_full_tb_warp = on; }
 void nvb_debug_pair_rows2(int on) { nvb::g_pair_rows2 = on; }
 void nvb_debug_traceback_fast(int on) { nvb::g_traceback_fast = on; }
 void nvb_debug_pair_extra_smem(int bytes) { nvb::g_pair_extra_smem = bytes > 0 ? bytes : 0; }

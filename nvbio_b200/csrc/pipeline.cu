@@ -12,6 +12,7 @@
 #include "fm_core.cuh"
 #include "gotoh_core.cuh"
 #include "pipeline_core.cuh"
+#include "gotoh_full_core.cuh"
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_sort.cuh>
 #include <mutex>
@@ -547,6 +548,34 @@ pipe_best_jobs_kernel(const PipeGeom g, const unsigned long long* __restrict__ b
     if (strand) strand[r] = (uint8_t)(hit_string[h] % g.strands);
 }
 
+// per-read path: the best job of every read as its traceback job (pipe_best_jobs_kernel's output; the job count lives on the device).
+// pipe_empty_jobs_kernel first gives every read an empty job; the job whose key is the read's best key then writes its own
+__global__ void __launch_bounds__(256)
+pipe_empty_jobs_kernel(const uint32_t n_reads, uint32_t* __restrict__ bp_off, uint32_t* __restrict__ bp_len, uint32_t* __restrict__ bt_off,
+                       uint32_t* __restrict__ bt_len, uint8_t* __restrict__ strand)
+{
+    const uint32_t r = blockIdx.x * 256 + threadIdx.x;
+    if (r >= n_reads) return;
+    bp_off[r] = 0; bp_len[r] = 0; bt_off[r] = 0; bt_len[r] = 0;
+    if (strand) strand[r] = 0;
+}
+__global__ void __launch_bounds__(256)
+pipe_read_best_jobs_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, const uint32_t* __restrict__ j_string,
+                           const uint32_t* __restrict__ j_first, const int32_t* __restrict__ job_score, const unsigned long long* __restrict__ best_key,
+                           const uint32_t* __restrict__ p_off, const uint32_t* __restrict__ p_len,
+                           const uint32_t* __restrict__ t_off, const uint32_t* __restrict__ t_len,
+                           uint32_t* __restrict__ bp_off, uint32_t* __restrict__ bp_len, uint32_t* __restrict__ bt_off, uint32_t* __restrict__ bt_len,
+                           uint8_t* __restrict__ strand)
+{
+    const uint32_t n = counts[2];
+    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
+        const uint32_t s = j_string[j], r = s / g.strands;
+        if (best_key[r] != make_best_key(job_score[j], j_first[j])) continue;
+        bp_off[r] = p_off[j]; bp_len[r] = p_len[j]; bt_off[r] = t_off[j]; bt_len[r] = t_len[j];
+        if (strand) strand[r] = (uint8_t)(s % g.strands);
+    }
+}
+
 // source cell (window-relative text start, read start) -> (genome coordinate, read start); reads without a hit: n_ops 0
 __global__ void __launch_bounds__(256)
 pipe_best_begin_kernel(const PipeGeom g, const unsigned long long* __restrict__ best_key, const uint32_t* __restrict__ bt_off,
@@ -758,6 +787,44 @@ pair_finalize_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const uin
 }
 
 // ---------------------------------------------------------------------------------------------
+// paired-end traceback (nvb_seed_extend_paired_traceback): mates that keep their single-end best take its banded traceback; a rescued
+// mate takes the full-matrix traceback of the winning opposite-mate job (gotoh_full_warp_traceback_kernel from its known sink)
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool pair_rescued(uint32_t flags) { return flags == NVB_PAIR_RESCUED_MATE1 || flags == NVB_PAIR_RESCUED_MATE2; }
+
+// a rescued mate's alignment is overwritten by the rescue's: its banded traceback job is emptied (mate m of pair p = read m * n_pairs + p)
+__global__ void __launch_bounds__(256)
+pair_empty_rescued_jobs_kernel(const uint32_t n_pairs, const uint32_t* __restrict__ pair_flags, uint32_t* __restrict__ bp_len, uint32_t* __restrict__ bt_len)
+{
+    const uint32_t p = blockIdx.x * 256 + threadIdx.x;
+    if (p >= n_pairs) return;
+    const uint32_t f = pair_flags[p];
+    if (!pair_rescued(f)) return;
+    const uint32_t r = (f == NVB_PAIR_RESCUED_MATE1 ? 0u : n_pairs) + p;
+    bp_len[r] = 0; bt_len[r] = 0;
+}
+
+// the winning job of every rescued pair (the job of anchor a = the mate not rescued, the one pair_finalize_kernel chose) as a traceback
+// item (job index into the rescue list, rescued mate); one atomic per warp.  The rescued mate's strand goes to ba_strand (may be NULL)
+__global__ void __launch_bounds__(256)
+pair_rescue_items_kernel(const uint32_t n_pairs, const uint32_t* __restrict__ pair_flags, const uint32_t* __restrict__ job_idx,
+                         const uint8_t* __restrict__ mate_strand, uint2* __restrict__ items, uint32_t* __restrict__ n_items, uint8_t* __restrict__ ba_strand)
+{
+    const uint32_t p = blockIdx.x * 256 + threadIdx.x, lane = threadIdx.x & 31u;
+    const uint32_t f = p < n_pairs ? pair_flags[p] : 0u;
+    const bool rescued = pair_rescued(f);
+    const uint32_t m = __ballot_sync(0xFFFFFFFFu, rescued);
+    if (!m) return;
+    uint32_t base = 0;
+    if (lane == 0) base = atomicAdd(n_items, (uint32_t)__popc(m));
+    base = __shfl_sync(0xFFFFFFFFu, base, 0);
+    if (!rescued) return;
+    const uint32_t o = f == NVB_PAIR_RESCUED_MATE1 ? 0u : 1u, out = o * n_pairs + p;
+    items[base + __popc(m & ((1u << lane) - 1u))] = make_uint2(job_idx[2u * p + (1u - o)], out);
+    if (ba_strand) ba_strand[out] = mate_strand[out];
+}
+
+// ---------------------------------------------------------------------------------------------
 // second-best pair and paired MAPQ (nvb_seed_extend_paired_mapq).  The candidates of a mate are those of the single-end stage (see
 // pipe_second_reduce_kernel) that reach the read's min score, gathered into one segment per read, sorted by (strand, end) and merged per
 // (strand, end); pair_second_kernel pairs them up (pair_combinations, pipeline_core.cuh) and adds the pair's rescues.
@@ -936,7 +1003,8 @@ struct PipeCall {
     Jobs best; int32_t* b_score; uint2 *b_sink, *b_source; char* tb_tmp; size_t tb_bytes;      // best-alignment traceback
     uint32_t *pw_want, *pw_idx, *pw_pstr, *pw_toff, *pw_tlen, *pcounts;     // paired: two opposite-mate job slots per pair
     Jobs rescue; int32_t* rs_score; uint2* rs_sink; char *pscan_tmp, *full_tmp; size_t pscan_bytes, full_bytes;
-    unsigned long long* second_key;                                         // second-best alignment of every read (MO)
+    uint2* rt_items; uint32_t* rt_count; char* rt_pool; size_t rt_pool_bytes;   // paired traceback (PP and BA): rescued mates, warp slot pool
+    unsigned long long* second_key;                                        // second-best alignment of every read (MO)
     uint32_t *pc_cnt, *pc_seg, *pc_fw, *pc_n, *pc_val[2], *pc_end, *pc_tie, *se_pos;     // paired MAPQ (PMO): candidate segments per read
     unsigned long long* pc_key[2]; int32_t* pc_score; char *pc_scan_tmp, *pc_sort_tmp; size_t pc_scan_bytes, pc_sort_bytes;
 
@@ -1010,6 +1078,10 @@ struct PipeCall {
             NVB_TRY(size_only(nvb_gotoh_score_indirect(P->type, &P->scheme, &v.pats, nullptr, &v.txts, (const uint32_t*)16, rcap, nullptr, nullptr,
                                                        nullptr, &full_bytes, s)));
             full_tmp = tc.take<char>(full_bytes);
+            if (BA) {
+                NVB_TRY(full_warp_traceback(P->type, rd.length, PP->max_frag, nullptr, &rt_pool_bytes, s));
+                rt_items = tc.take<uint2>((size_t)n_reads / 2u + 1u); rt_count = tc.take<uint32_t>(4); rt_pool = tc.take<char>(rt_pool_bytes);
+            }
         }
         if (MO) second_key = tc.take<unsigned long long>(n_reads);
         if (PMO) {
@@ -1146,12 +1218,29 @@ struct PipeCall {
     }
 
     // best-alignment traceback: the best hit of every read as a job, its banded traceback, the alignment's begin in the genome
+    // (per-read path: the best job of every read from the distinct jobs; paired: after the rescue, whose rescued mates get empty jobs)
     int best_traceback() const
     {
         const uint32_t rgrid = (g.n_reads + 255) / 256;
-        pipe_best_jobs_kernel<<<rgrid, 256, 0, s>>>(g, best_key, hit_string, hits.p_off, hits.p_len, hits.t_off, hits.t_len,
-                                                    best.p_off, best.p_len, best.t_off, best.t_len, BA->d_strand);
-        NVB_LAUNCH_CHECK();
+        if (per_read) {
+            pipe_empty_jobs_kernel<<<rgrid, 256, 0, s>>>(g.n_reads, best.p_off, best.p_len, best.t_off, best.t_len, BA->d_strand);
+            NVB_LAUNCH_CHECK();
+            const uint32_t hgrid = (hit_capacity + 255) / 256, jgrid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
+            if (jgrid) {
+                pipe_read_best_jobs_kernel<<<jgrid, 256, 0, s>>>(g, counts, j_string, j_first, job_score, best_key, jobs.p_off, jobs.p_len,
+                                                                 jobs.t_off, jobs.t_len, best.p_off, best.p_len, best.t_off, best.t_len, BA->d_strand);
+                NVB_LAUNCH_CHECK();
+            }
+        } else {
+            pipe_best_jobs_kernel<<<rgrid, 256, 0, s>>>(g, best_key, hit_string, hits.p_off, hits.p_len, hits.t_off, hits.t_len,
+                                                        best.p_off, best.p_len, best.t_off, best.t_len, BA->d_strand);
+            NVB_LAUNCH_CHECK();
+        }
+        if (PP) {
+            const uint32_t n_pairs = g.n_reads / 2u;
+            pair_empty_rescued_jobs_kernel<<<(n_pairs + 255) / 256, 256, 0, s>>>(n_pairs, PO->d_pair_flags, best.p_len, best.t_len);
+            NVB_LAUNCH_CHECK();
+        }
         const JobViews v = job_views(best, rd.length + g.band);
         size_t bytes = tb_bytes;
         NVB_TRY(nvb_banded_gotoh_traceback(g.band, P->type, &P->scheme, &v.pats, str_quals, &v.txts, g.n_reads, b_score, (nvb_uint2*)b_sink,
@@ -1255,6 +1344,25 @@ struct PipeCall {
         if (PO->d_n_rescue) NVB_CUDA_TRY(cudaMemcpyAsync(PO->d_n_rescue, pcounts, 2 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
         return NVB_OK;
     }
+
+    // paired traceback of the rescued mates (after best_traceback, whose outputs they overwrite): the winning opposite-mate job of every
+    // rescued pair, traced from the rescue score pass's sink on its window; begin = (window begin + source.x, source.y)
+    int rescue_traceback() const
+    {
+        const uint32_t n_pairs = g.n_reads / 2u;
+        NVB_CUDA_TRY(cudaMemsetAsync(rt_count, 0, sizeof(uint32_t), s));
+        pair_rescue_items_kernel<<<(n_pairs + 255) / 256, 256, 0, s>>>(n_pairs, PO->d_pair_flags, pw_idx, PO->d_mate_strand, rt_items, rt_count,
+                                                                       BA->d_strand);
+        NVB_LAUNCH_CHECK();
+        const JobViews v = job_views(rescue, PP->max_frag);
+        FullTbArgs a;
+        a.S = make_scheme(&P->scheme); a.pat = make_strset(&v.pats); a.txt = make_strset(&v.txts); a.quals = str_quals;
+        a.score = rs_score; a.sink = rs_sink; a.items = rt_items; a.n_items = rt_count;
+        a.o.ops = BA->d_ops; a.o.n_ops = BA->d_n_ops; a.o.source = (uint2*)BA->d_begin; a.o.max_ops = BA->max_ops; a.o.absolute = 1u;
+        a.pool = rt_pool;
+        size_t bytes = rt_pool_bytes;
+        return full_warp_traceback(P->type, rd.length, PP->max_frag, &a, &bytes, s);
+    }
 };
 
 static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1304,8 +1412,8 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
         c.MO = &c.se_mo;
     }
     c.dedup = P->dedup_jobs != 0;
-    // per-read path: nobody asked for per-hit outputs, so no per-hit array needs to exist
-    c.per_read = c.dedup && g_pipe_path != 1 && !d_hit_read && !d_hit_window && !d_hit_score && !d_hit_sink && !BA;
+    // per-read path: nobody asked for per-hit outputs, so no per-hit array needs to exist (the traceback takes the best of the distinct jobs)
+    c.per_read = c.dedup && g_pipe_path != 1 && !d_hit_read && !d_hit_window && !d_hit_score && !d_hit_sink;
     const nvb_gotoh_scheme& SC = P->scheme;
     c.eligible = c.per_read && P->type == NVB_LOCAL && g.bits == 2 && P->band_len <= 32 && !SC.d_qual_table && SC.match > 0 && SC.mismatch < 0 &&
                  SC.pattern_gap_open < 0 && SC.pattern_gap_ext <= 0 && SC.text_gap_open < 0 && SC.text_gap_ext <= 0;
@@ -1328,10 +1436,11 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
         pipe_export_hits_kernel<<<(hit_capacity + 255) / 256, 256, 0, s>>>(g, c.counts, c.hit_string, c.hits.t_off, c.hits.t_len, d_hit_read, (uint2*)d_hit_window);
         NVB_LAUNCH_CHECK();
     }
-    if (BA) NVB_TRY(c.best_traceback());
+    if (BA && !PP) NVB_TRY(c.best_traceback());
     if (c.MO) NVB_TRY(c.second_best());
     if (PMO) NVB_TRY(c.pair_candidates());
     if (PP) NVB_TRY(c.paired_rescue());
+    if (BA && PP) { NVB_TRY(c.best_traceback()); NVB_TRY(c.rescue_traceback()); }
     if (PMO) NVB_TRY(c.pair_second());
     if (!c.dedup) NVB_CUDA_TRY(cudaMemcpyAsync(c.counts + 2, c.counts, sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
     if (d_n_hits) NVB_CUDA_TRY(cudaMemcpyAsync(d_n_hits, c.counts, 3 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
@@ -1417,6 +1526,27 @@ extern "C" int nvb_seed_extend_paired_mapq(const nvb_fm_index* fmi, const uint32
     if (!reads || mapq->max_read_len < reads->length) return NVB_E_INVALID;           // the min-score table must cover every read length
     return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
                             nullptr, nullptr, nullptr, pair_params, out, mapq, nullptr, mapq_out, d_temp, temp_bytes, stream);
+}
+
+extern "C" int nvb_seed_extend_paired_traceback(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_pairs,
+                    const nvb_seed_extend_params* P, uint32_t hit_capacity,
+                    const nvb_pair_params* pair_params, const nvb_pair_out* out,
+                    const nvb_best_alignment_out* mate_alignment,
+                    const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
+                    uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream)
+{
+    if (!pair_params || !out || n_pairs > 0x3FFFFFFFu || !temp_bytes || !reads) return NVB_E_INVALID;
+    const nvb_best_alignment_out* BA = mate_alignment;
+    if (!BA || !BA->d_ops || !BA->d_n_ops || !BA->d_begin || BA->max_ops == 0) return NVB_E_INVALID;
+    if ((mapq == nullptr) != (mapq_out == nullptr)) return NVB_E_INVALID;
+    if (mapq) {
+        if (!mapq->d_min_score || !mapq_out->d_second_pair_score || !mapq_out->d_mate_mapq) return NVB_E_INVALID;
+        if (mapq->max_read_len < reads->length) return NVB_E_INVALID;
+    }
+    if (reads->length > FULL_TB_MAX_M) return NVB_E_UNSUPPORTED;       // nvBowtie's MAXIMUM_READ_LENGTH
+    return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
+                            nullptr, nullptr, BA, pair_params, out, mapq, nullptr, mapq_out, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_debug_mapq_eval(const int32_t* d_best, const uint8_t* d_has_second, const int32_t* d_second, const uint32_t* d_len,

@@ -304,4 +304,23 @@ __host__ __device__ inline uint32_t bowtie_mapq2(int32_t best_score, bool has_se
     return best_over >= diff * 0.5f ? 1 : 0;
 }
 
+// Window cut of a full-matrix traceback from a known sink (gotoh_full_warp_traceback_kernel): the first 0-based text row r0 it computes;
+// it computes rows [r0, sink_x) and leaves the rest out.  Rows after sink_x cannot change a cell of rows <= sink_x (every type).  LOCAL
+// with every gap charge < 0 (go, ge: the pattern gap open / extension gotoh_full_impl2 charges along both axes): an alignment of score
+// `score` ending in pattern column sink_y consumes at most sink_y text symbols on substitutions (each worth <= s_max, the largest
+// substitution score over all qualities) and, since a run of k deletions costs go + (k - 1) ge <= k max(go, ge) and insertions cost < 0,
+// at most D_max = floor((sink_y s_max - score) / -max(go, ge)) on deletions; its source row is therefore >= sink_x - (sink_y + D_max).
+// Starting from a zero row at r0 - 1 instead of the full rows above only lowers H / E / F (the recurrence is monotone and LOCAL's H >= 0),
+// while every cell of the reference path keeps its value (its own path starts at or below r0); so at each cell of the path the set of
+// maximal candidates can only shrink around the one the walk follows, and the walk retraces the same cells, ops and source.
+__host__ __device__ inline uint32_t full_traceback_first_row(int type, uint32_t sink_x, uint32_t sink_y, int32_t score, int32_t s_max,
+                                                             int32_t go, int32_t ge)
+{
+    if (type != NVB_LOCAL || go >= 0 || ge >= 0) return 0u;
+    const int64_t g = go > ge ? go : ge;                                         // the most a deleted text symbol can cost (< 0)
+    const int64_t room = (int64_t)sink_y * (s_max > 0 ? s_max : 0) - (int64_t)score;
+    const int64_t span = (int64_t)sink_y + (room > 0 ? room / -g : 0);             // text symbols an alignment ending at the sink can consume
+    return span < (int64_t)sink_x ? (uint32_t)((int64_t)sink_x - span) : 0u;
+}
+
 } // namespace nvb

@@ -217,7 +217,7 @@ class PairedWorkspace:
     """outputs + temp storage of seed_extend_paired for repeated calls on equally-shaped batches"""
 
     def __init__(self, fmi, genome, reads: PackedStringSet, params: SeedExtendParams, pair: PairParams, hit_capacity: int,
-                 mapq: Optional[MapqParams] = None):
+                 mapq: Optional[MapqParams] = None, traceback: bool = False, max_ops: Optional[int] = None):
         dev = fmi.device
         assert reads.count % 2 == 0
         self.n_pairs = n = reads.count // 2
@@ -238,6 +238,13 @@ class PairedWorkspace:
             self.second_mate_strand = torch.empty((2, n), dtype=torch.uint8, device=dev)
             self.mate_second_score = torch.empty((2, n), dtype=torch.int32, device=dev)
             self.mate_mapq = torch.empty((2, n), dtype=torch.uint8, device=dev)
+        # optional alignment of both mates (nvb_seed_extend_paired_traceback)
+        self.mate_ops = self.mate_n_ops = self.mate_begin = None
+        self.max_ops = reads.length + params.band_len + 1 if max_ops is None else max_ops
+        if traceback:
+            self.mate_ops = torch.zeros((2, n, self.max_ops), dtype=torch.uint8, device=dev)
+            self.mate_n_ops = torch.zeros((2, n), dtype=torch.int32, device=dev)
+            self.mate_begin = torch.empty((2, n, 2), dtype=torch.int32, device=dev)
         tb = C.c_size_t(0)
         r = _call_paired(fmi, genome, reads, params, pair, self, None, tb)
         if r != -2:
@@ -252,32 +259,48 @@ def _call_paired(fmi, genome, reads, params, pair, ws, temp, tb):
     po.d_pair_score, po.d_pair_flags = ws.pair_score.data_ptr(), ws.pair_flags.data_ptr()
     po.d_mate_score, po.d_mate_pos, po.d_mate_strand = ws.mate_score.data_ptr(), ws.mate_pos.data_ptr(), ws.mate_strand.data_ptr()
     po.d_n_rescue = ws.n_rescue.data_ptr()
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    mp = mo = None
     if ws.mate_mapq is not None:
         mp = ws.mapq_params.struct()
         mo = PairMapqOutStruct()
         mo.d_second_pair_score, mo.d_second_mate_pos = ws.second_pair_score.data_ptr(), ws.second_mate_pos.data_ptr()
         mo.d_second_mate_strand, mo.d_mate_second_score = ws.second_mate_strand.data_ptr(), ws.mate_second_score.data_ptr()
         mo.d_mate_mapq = ws.mate_mapq.data_ptr()
+    if ws.mate_ops is not None:
+        ba = BestAlignmentOutStruct()
+        ba.d_ops, ba.max_ops, ba.d_n_ops = ws.mate_ops.data_ptr(), ws.max_ops, ws.mate_n_ops.data_ptr()
+        ba.d_begin, ba.d_strand = ws.mate_begin.data_ptr(), None
+        return lib().nvb_seed_extend_paired_traceback(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(ws.n_pairs), C.byref(ps),
+                                                      C.c_uint32(ws.hit_capacity), C.byref(pp), C.byref(po), C.byref(ba),
+                                                      C.byref(mp) if mp is not None else None, C.byref(mo) if mo is not None else None,
+                                                      _p(ws.n_hits), _p(temp), C.byref(tb), stream)
+    if mo is not None:
         return lib().nvb_seed_extend_paired_mapq(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(ws.n_pairs), C.byref(ps),
                                                  C.c_uint32(ws.hit_capacity), C.byref(pp), C.byref(po), C.byref(mp), C.byref(mo),
-                                                 _p(ws.n_hits), _p(temp), C.byref(tb), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+                                                 _p(ws.n_hits), _p(temp), C.byref(tb), stream)
     return lib().nvb_seed_extend_paired(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(ws.n_pairs), C.byref(ps), C.c_uint32(ws.hit_capacity),
-                                        C.byref(pp), C.byref(po), _p(ws.n_hits), _p(temp), C.byref(tb),
-                                        C.c_void_p(torch.cuda.current_stream().cuda_stream))
+                                        C.byref(pp), C.byref(po), _p(ws.n_hits), _p(temp), C.byref(tb), stream)
 
 
 def seed_extend_paired(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStringSet, params: SeedExtendParams, pair: PairParams,
-                       workspace: Optional[PairedWorkspace] = None, hit_capacity: Optional[int] = None, mapq: Optional[MapqParams] = None):
+                       workspace: Optional[PairedWorkspace] = None, hit_capacity: Optional[int] = None, mapq: Optional[MapqParams] = None,
+                       traceback: bool = False):
     """paired-end seed + extend (reads = mate 1 of every pair, then mate 2 of every pair): concordant pairs straight from the two
     independent alignments, opposite-mate full-DP rescue for the rest (nvBowtie's best-approx paired flow,
     score_opposite_inl.h:90-266).  Returns the workspace: .pair_score[n], .pair_flags[n], .mate_score/.mate_pos/.mate_strand[2,n],
     .n_rescue[2] = (full-DP jobs run, wanted).  With mapq=MapqParams(...) also the second-best pair and the MAPQ of every mate
     (nvb_seed_extend_paired_mapq): .second_pair_score[n], .second_mate_pos/.second_mate_strand[2,n], .mate_second_score[2,n] (each mate's
-    single-end second score) and .mate_mapq[2,n].  A workspace made with mapq keeps computing them; a new mapq replaces its table"""
+    single-end second score) and .mate_mapq[2,n].  A workspace made with mapq keeps computing them; a new mapq replaces its table.
+    With traceback=True also the alignment of every mate (nvb_seed_extend_paired_traceback): .mate_ops[2,n,max_ops] (END->START, 0 M,
+    1 I, 2 D), .mate_n_ops[2,n] and .mate_begin[2,n,2] = (genome start, read start) -- a rescued mate's from the full-matrix DP that
+    placed it.  A workspace made with traceback keeps computing them"""
     if workspace is None:
         if hit_capacity is None:
             hit_capacity = 32 * reads.count + 1024
-        workspace = PairedWorkspace(fmi, genome, reads, params, pair, hit_capacity, mapq)
+        workspace = PairedWorkspace(fmi, genome, reads, params, pair, hit_capacity, mapq, traceback)
+    elif traceback and workspace.mate_ops is None:
+        raise ValueError("seed_extend_paired(traceback=True): the workspace was created without traceback outputs")
     elif mapq is not None:
         if workspace.mate_mapq is None:
             raise ValueError("seed_extend_paired(mapq=...): the workspace was created without mapq outputs")
