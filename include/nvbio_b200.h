@@ -417,6 +417,10 @@ typedef struct nvb_seed_extend_params {
 /* reads: n_reads strings (2- or 4-bit).  genome: 2-bit big-endian packed text of fmi->length symbols.
  * Outputs: d_best_score[n_reads] (INT_MIN when a read has no hit), d_best_pos[n_reads] = genome
  * coordinate of the best alignment's end (window begin + sink.x; 0xFFFFFFFF when none).
+ * A job the banded DP reports empty (sink.x == 0xFFFFFFFF, score NVB_SINK_MIN: its window is shorter than the read, as for a read
+ * running more than band_len/2 symbols past the genome's end) is not an alignment: it keeps its per-hit outputs and counts as a hit,
+ * but is never a read's best or second-best alignment nor a paired-end candidate.  A read whose jobs are all empty is unaligned
+ * (INT_MIN, 0xFFFFFFFF; n_ops 0 and MAPQ 0 in the calls below; an unaligned mate in the paired ones).
  * Optional per-hit outputs (may be NULL) of capacity hit_capacity: d_hit_read (string id = read*strands
  * + strand), d_hit_window (begin,end), d_hit_score, d_hit_sink; d_n_hits[0] receives the number of hits
  * kept (<= hit_capacity), d_n_hits[1] the number found and d_n_hits[2] the number of distinct alignment jobs

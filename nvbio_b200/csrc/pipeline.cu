@@ -142,6 +142,10 @@ __device__ __forceinline__ unsigned long long make_best_key(int32_t score, uint3
 __device__ __forceinline__ int32_t  best_key_score(unsigned long long key) { return (int32_t)((uint32_t)(key >> 32) ^ 0x80000000u); }
 __device__ __forceinline__ uint32_t best_key_index(unsigned long long key) { return 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull); }
 
+// a scored job is an alignment unless the DP reported it empty (window shorter than the read: NVB_SINK_MIN, sink 0xFFFFFFFF) -- a read
+// running more than band/2 symbols past the genome's end gets such a window; it never becomes a best, second-best or pair candidate
+__device__ __forceinline__ bool job_aligned(uint2 sink) { return sink.x != 0xFFFFFFFFu; }
+
 // one thread per (string, seed slot): SA range of the seed, and its clamped size.
 // genome != NULL (the per-read path on an index with the full suffix array): single-row ranges are located on the spot --
 // ranges[q] = (text position, 0xFFFFFFFF), see fm_match_locate_one -- so that neither the remaining LF steps nor the later SA
@@ -399,10 +403,11 @@ pipe_scatter_dp_kernel(const uint32_t* __restrict__ dp_count, const uint32_t* __
 // best job per read: max score, ties -> the job whose first hit comes first (the per-hit path's "smallest hit index")
 __global__ void __launch_bounds__(256)
 pipe_reduce_jobs_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, const uint32_t* __restrict__ j_string, const uint32_t* __restrict__ j_first,
-                        const int32_t* __restrict__ job_score, unsigned long long* __restrict__ best_key)
+                        const int32_t* __restrict__ job_score, const uint2* __restrict__ job_sink, unsigned long long* __restrict__ best_key)
 {
     const uint32_t n = counts[2];
     for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
+        if (!job_aligned(job_sink[j])) continue;
         const unsigned long long key = make_best_key(job_score[j], j_first[j]);
         atomicMax(best_key + j_string[j] / g.strands, key);
     }
@@ -501,18 +506,19 @@ pipe_scatter_scores_kernel(const PipeGeom g, const uint32_t* __restrict__ counts
     for (uint32_t nx = leader[l]; nx != l; nx = leader[l]) l = nx;
     const uint32_t j = job_idx[l];
     const int32_t sc = job_score[j];
+    const uint2 sk = job_sink[j];
     score[h] = sc;
-    sink[h]  = job_sink[j];
-    atomicMax(best_key + hit_string[h] / g.strands, make_best_key(sc, h));
+    sink[h]  = sk;
+    if (job_aligned(sk)) atomicMax(best_key + hit_string[h] / g.strands, make_best_key(sc, h));
 }
 
 // best hit per read: max score, ties -> smallest hit index (deterministic)
 __global__ void __launch_bounds__(256)
 pipe_reduce_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, const uint32_t* __restrict__ hit_string,
-                   const int32_t* __restrict__ score, unsigned long long* __restrict__ best_key)
+                   const int32_t* __restrict__ score, const uint2* __restrict__ sink, unsigned long long* __restrict__ best_key)
 {
     const uint32_t h = blockIdx.x * 256 + threadIdx.x;
-    if (h >= counts[0]) return;
+    if (h >= counts[0] || !job_aligned(sink[h])) return;
     atomicMax(best_key + hit_string[h] / g.strands, make_best_key(score[h], h));
 }
 
@@ -625,7 +631,8 @@ pipe_second_reduce_kernel(const PipeGeom g, const uint32_t* __restrict__ count, 
     for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
         const uint32_t s = c_string[j], read = s / g.strands;
         const int32_t sc = score[j];
-        if (second_candidate(sc, t_off[j] + sink[j].x, s % g.strands, str_len[s], best_pos[read], best_strand[read], min_score))
+        const uint2 sk = sink[j];
+        if (job_aligned(sk) && second_candidate(sc, t_off[j] + sk.x, s % g.strands, str_len[s], best_pos[read], best_strand[read], min_score))
             atomicMax(second_key + read, make_best_key(sc, index ? index[j] : j));
     }
 }
@@ -840,7 +847,7 @@ pair_cand_scatter_kernel(const PipeGeom g, const uint32_t* __restrict__ count, c
     const uint32_t n = *count;
     for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
         const uint32_t s = c_string[j], read = s / g.strands;
-        if (score[j] < min_score[str_len[s]]) continue;
+        if (!job_aligned(sink[j]) || score[j] < min_score[str_len[s]]) continue;
         const uint32_t slot = atomicAdd(cursor + read, 1u);
         if (!seg) continue;
         key[seg[read] + slot] = ((unsigned long long)(s % g.strands) << 32) | (t_off[j] + sink[j].x);
@@ -1168,7 +1175,7 @@ struct PipeCall {
         if (cap) {
             // the job count lives on the device: a resident grid striding over it instead of hit_capacity / 256 mostly empty CTAs
             const uint32_t jgrid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
-            pipe_reduce_jobs_kernel<<<jgrid, 256, 0, s>>>(g, counts, j_string, j_first, job_score, best_key);
+            pipe_reduce_jobs_kernel<<<jgrid, 256, 0, s>>>(g, counts, j_string, j_first, job_score, job_sink, best_key);
             NVB_LAUNCH_CHECK();
             pipe_finalize_jobs_kernel<<<jgrid, 256, 0, s>>>(g, counts, j_string, j_first, jobs.t_off, job_score, job_sink, best_key,
                                                             best_score, best_pos, rb_strand);
@@ -1210,7 +1217,7 @@ struct PipeCall {
         NVB_TRY(stage(6));
         // with job de-duplication the best-per-read reduction already happened in the scatter kernel
         if (cap && !dedup) {
-            pipe_reduce_kernel<<<hgrid, 256, 0, s>>>(g, counts, hit_string, h_score, best_key);
+            pipe_reduce_kernel<<<hgrid, 256, 0, s>>>(g, counts, hit_string, h_score, h_sink, best_key);
             NVB_LAUNCH_CHECK();
         }
         pipe_finalize_kernel<<<(g.n_reads + 255) / 256, 256, 0, s>>>(g, best_key, hits.t_off, h_sink, hit_string, best_score, best_pos, rb_strand);

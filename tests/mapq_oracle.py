@@ -2,6 +2,7 @@
 (nvBowtie/bowtie2/cuda/mapq.h:142-331) in numpy float32, and the second-best rule of include/nvbio_b200.h applied to the per-hit
 outputs of the oracle composition (tests/pipeline_oracle.py)."""
 import numpy as np
+from tests.pipeline_oracle import best_hits, EMPTY_SINK
 
 INT_MIN = -2**31
 
@@ -63,11 +64,7 @@ def mapq_oracle(se, lengths, strands, min_score, match_bonus):
     n = len(lengths)
     hs, score = se["hit_string"], se["hit_score"]
     end = se["hit_window"][:, 0] + se["hit_sink"][:, 0] if len(hs) else np.zeros(0, np.int64)
-    best_h = np.full(n, -1, np.int64)
-    for h, s in enumerate(hs):
-        r = int(s) // strands
-        if best_h[r] < 0 or score[h] > score[best_h[r]]:
-            best_h[r] = h
+    best_h = best_hits(se, n, strands)
     out = {k: np.zeros(n, np.int64) for k in ("best_score", "best_pos", "best_strand", "second_score", "second_pos", "second_strand")}
     out["best_score"][:] = INT_MIN; out["best_pos"][:] = 0xFFFFFFFF
     out["second_score"][:] = INT_MIN; out["second_pos"][:] = 0xFFFFFFFF
@@ -79,7 +76,7 @@ def mapq_oracle(se, lengths, strands, min_score, match_bonus):
     for h, s in enumerate(hs):
         r = int(s) // strands
         ln = int(lengths[r])
-        if score[h] < min_score[ln] or not distinct(int(end[h]), int(s) % strands, int(out["best_pos"][r]), int(out["best_strand"][r]), ln):
+        if se["hit_sink"][h][0] == EMPTY_SINK or score[h] < min_score[ln] or not distinct(int(end[h]), int(s) % strands, int(out["best_pos"][r]), int(out["best_strand"][r]), ln):
             continue
         if second_h[r] < 0 or score[h] > score[second_h[r]]:
             second_h[r] = h

@@ -3,7 +3,7 @@ include/nvbio_b200.h by brute force over every combination of the mates' candida
 composition of the paired stage (tests/pipeline_oracle.py) and nvBowtie's BowtieMapq2 restated in tests/mapq_oracle.py."""
 import numpy as np
 from tests.mapq_oracle import bowtie_mapq2, mapq_oracle, INT_MIN
-from tests.pipeline_oracle import seed_extend_oracle, seed_extend_paired_oracle, _scheme_args
+from tests.pipeline_oracle import seed_extend_oracle, seed_extend_paired_oracle, _scheme_args, best_hits, EMPTY_SINK
 
 NONE_TIE = 0xFFFFFFFF
 
@@ -82,18 +82,14 @@ def pair_mapq_oracle(O, idx, genome_sym, reads, params, pair, n_pairs, min_score
     lens = np.array([len(r) for r in reads], np.int64)
     ms = np.asarray(min_score, np.int64)
     single = mapq_oracle(se, lens, 2, ms, match_bonus)
-    best_h = np.full(len(reads), -1, np.int64)                     # every read's best hit (its tie index): max score, then smallest hit
-    for h, s in enumerate(se["hit_string"]):
-        r = int(s) // 2
-        if best_h[r] < 0 or se["hit_score"][h] > se["hit_score"][best_h[r]]:
-            best_h[r] = h
+    best_h = best_hits(se, len(reads))                             # every read's best hit (its tie index): max score, then smallest hit
     rescues, wanted = rescue_jobs(O, idx, genome_sym, reads, params, pair, n_pairs, single, pe["pair_flags"] != 1, quals=quals)
     assert (len(rescues), wanted) == tuple(pe["n_rescue"])         # the same jobs as the paired composition ran
     end = se["hit_window"][:, 0] + se["hit_sink"][:, 0] if len(se["hit_string"]) else np.zeros(0, np.int64)
     cands = [[] for _ in reads]
     for h, s in enumerate(se["hit_string"]):
         r = int(s) // 2
-        if se["hit_score"][h] >= ms[lens[r]]:
+        if se["hit_sink"][h][0] != EMPTY_SINK and se["hit_score"][h] >= ms[lens[r]]:
             cands[r].append((int(se["hit_score"][h]), int(s) % 2, int(end[h]), h))
     resc = {}
     for p, a, to, rs, x in rescues:

@@ -2,11 +2,28 @@
 nvbio_b200/csrc/pipeline.cu, each stage computed by the CPU oracle / reference library."""
 import numpy as np
 
+EMPTY_SINK = 0xFFFFFFFF      # sink.x of a job the banded DP reports empty (window shorter than the read)
+
+
+def best_hits(se, n_reads, strands=2):
+    """every read's best hit (index into se's hits, -1 = none): max score, ties -> smallest hit index; empty jobs are skipped"""
+    best_h = np.full(n_reads, -1, np.int64)
+    for h, s in enumerate(se["hit_string"]):
+        r = int(s) // strands
+        if se["hit_sink"][h][0] == EMPTY_SINK:
+            continue
+        if best_h[r] < 0 or se["hit_score"][h] > se["hit_score"][best_h[r]]:
+            best_h[r] = h
+    return best_h
+
 
 def _scheme_args(sch):
-    """(scheme tuple, qtab or None) of a SimpleGotohScheme / QualityGotohScheme"""
+    """(scheme tuple, qtab or None) of a SimpleGotohScheme / QualityGotohScheme / a scheme object with separate pattern and text gap
+    costs (match, mismatch, pgo, pge, tgo, tge)"""
     if hasattr(sch, "table_host"):
         return (sch.match_bonus, int(sch.table_host[0, 1]), sch.pgo, sch.pge, sch.tgo, sch.tge), sch.table_host
+    if hasattr(sch, "tgo"):
+        return (sch.match, sch.mismatch, sch.pgo, sch.pge, sch.tgo, sch.tge), None
     return (sch.match, sch.mismatch, sch.gap_open, sch.gap_ext), None
 
 
@@ -72,6 +89,8 @@ def seed_extend_oracle(O, idx, genome_sym, reads, params, quals=None):
     best_pos = np.full(len(reads), 0xFFFFFFFF, np.int64)
     for h, s in enumerate(hit_string):
         r = s // strands
+        if int(sx[h]) == EMPTY_SINK:                 # a window shorter than the read: the DP's empty result is not an alignment
+            continue
         if int(score[h]) > best_score[r]:
             best_score[r] = int(score[h]); best_pos[r] = t_off[h] + int(sx[h])
     return dict(best_score=best_score, best_pos=best_pos, hit_string=np.array(hit_string, np.int64),
@@ -88,12 +107,7 @@ def seed_extend_paired_oracle(O, idx, genome_sym, reads, params, pair, n_pairs, 
     se = seed_extend_oracle(O, idx, genome_sym, reads, params, quals=quals)
     glen = idx.n
     strands = 2
-    # best hit of every read: max score, ties -> smallest hit index
-    best_h = np.full(len(reads), -1, np.int64)
-    for h, s in enumerate(se["hit_string"]):
-        r = int(s) // strands
-        if best_h[r] < 0 or se["hit_score"][h] > se["hit_score"][best_h[r]]:
-            best_h[r] = h
+    best_h = best_hits(se, len(reads), strands)
     INT_MIN = -2**31
 
     def mate(r):

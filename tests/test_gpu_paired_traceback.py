@@ -13,6 +13,7 @@ from nvbio_b200 import aln, synth
 from nvbio_b200._lib import lib
 from nvbio_b200.strings import PackedStringSet, unpack_symbols
 from tests.gpu_util import require_gpu, host_u32
+from tests.pipeline_oracle import _scheme_args
 
 INT_MIN = -2**31
 NONE = 0xFFFFFFFF
@@ -86,16 +87,20 @@ def strand_string(r, q, strand):
     return np.where(r < 4, 3 - r, r)[::-1].astype(np.uint8), q[::-1]
 
 
-def replay(ops, n_ops, begin, pat, pq, gsym, scheme):
-    """score and genome end of an alignment (ops END->START) from its begin"""
-    tab = getattr(scheme, "table_host", None)
-    go, ge = (scheme.pgo, scheme.pge) if tab is not None else (scheme.gap_open, scheme.gap_ext)
+def replay(ops, n_ops, begin, pat, pq, gsym, scheme, typ=aln.LOCAL, window=0):
+    """score and genome end of an alignment (ops END->START) from its begin.  Both kinds of gap cost the pattern gap, as in the banded DP;
+    a GLOBAL banded alignment that begins past its window's begin (genome coordinate `window`) also pays the text gap its first row
+    starts with"""
+    sch, tab = _scheme_args(scheme)
+    match, mismatch, go, ge, tgo, tge = sch if len(sch) == 6 else sch + sch[2:]
     j, i = int(begin[0]), int(begin[1])
     s, prev = 0, -1
+    if typ == aln.GLOBAL and j > window:
+        s += tgo + (j - window - 1) * tge
     for op in ops[:n_ops][::-1]:
         if op == 0:
-            eq = pat[i] == gsym[j]
-            s += (int(tab[pq[i], 0 if eq else 1]) if tab is not None else (scheme.match if eq else scheme.mismatch)); i += 1; j += 1
+            eq = j < len(gsym) and pat[i] == gsym[j]                 # (a band running past the genome's end meets pad symbols)
+            s += (int(tab[pq[i], 0 if eq else 1]) if tab is not None else (match if eq else mismatch)); i += 1; j += 1
         elif op == 1:
             s += ge if prev == 1 else go; i += 1
         else:

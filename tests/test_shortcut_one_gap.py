@@ -7,7 +7,9 @@ subset of it with the same results.  The host build (tests/host/shortcut_harness
 Cases built to break the bound: two substitutions at every spacing, three or four with some in the clip rows, a 1-2 base indel a few
 rows from either end (the gapless diagonal then shows one or two differences and a one-gap alignment is perfect) with the seed's diagonal
 on either side of it, indels and substitutions inside homopolymers and period-2 / 3 / 7 repeats, ragged and short reads, windows longer
-than needed and too short; bands 31, 15 and 8, four schemes."""
+than needed and too short; bands 31, 15, 8 and the pipeline's 7, 5 and 3; four schemes with one gap cost and two whose pattern and text
+gap costs differ (the routine bounds every gap by the cheaper open, max(pattern_gap_open, text_gap_open), as pipe_perfect_jobs_kernel
+passes it)."""
 import ctypes as C
 import os
 import subprocess
@@ -19,7 +21,9 @@ from nvbio_b200.strings import pack_symbols
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, "host", "libshortcut_harness.so")
 SRC = os.path.join(HERE, "host", "shortcut_harness.cu")
-SCHEMES = ((2, -2, -5, -3), (1, -4, -6, -1), (2, -6, -8, -3), (3, -1, -2, -2))
+SCHEMES = ((2, -2, -5, -3), (1, -4, -6, -1), (2, -6, -8, -3), (3, -1, -2, -2),
+           (2, -2, -5, -3, -9, -1), (2, -2, -9, -1, -5, -3))       # (match, mismatch, gap open, gap ext) or (..., pattern gap, text gap)
+BANDS = [31, 15, 8, 7, 5, 3]
 STRIDE = 160
 
 
@@ -47,10 +51,15 @@ def R():
     return orc.Ref() if orc.Ref.available() else None
 
 
+def six(scheme):
+    """(match, mismatch, pattern gap open, pattern gap ext, text gap open, text gap ext)"""
+    return tuple(scheme) if len(scheme) == 6 else tuple(scheme) + (scheme[2], scheme[3])
+
+
 def one_gap_limit(scheme):
-    """delta = match * M - T below which the rule with the check claims (and below o without it)"""
-    m, s, go = scheme[0], scheme[1], scheme[2]
-    o = -go
+    """delta = match * M - T below which the rule with the check claims (and below o without it); o = the cheaper gap open"""
+    m, s, pgo, _, tgo, _ = six(scheme)
+    o = -max(pgo, tgo)
     return min(2 * o, o + m - s), o
 
 
@@ -89,14 +98,15 @@ def shortcut(H, J, scheme, one_gap):
     gw = np.concatenate([pack_symbols(np.concatenate([J.text, np.zeros(64, np.uint8)]), 2, True), np.zeros(2, np.uint32)])
     solved = np.zeros(n, np.uint8); score = np.zeros(n, np.int32); sink = np.zeros((n, 2), np.uint32)
     H.hs_gapless_job_shortcut(_p(sw), _p(gw), _p(po), _p(M), _p(to), _p(N), C.c_uint32(n), C.c_uint32(J.band), C.c_int32(scheme[0]),
-                              C.c_int32(scheme[1]), C.c_int32(scheme[2]), C.c_int(1 if one_gap else 0), _p(solved), _p(score), _p(sink))
+                              C.c_int32(scheme[1]), C.c_int32(six(scheme)[2]), C.c_int(1 if one_gap else 0), _p(solved), _p(score), _p(sink),
+                              C.c_int32(six(scheme)[4]))
     return solved.astype(bool), score, sink
 
 
 def check(H, O, R, J, scheme):
     """both rules against the DP; returns (claimed with the check, claimed without it)"""
     flat, po, M, to, N = J.arrays()
-    ws, wx, wy, _ = O.banded_gotoh(J.band, 1, scheme, flat, po, M, J.text, to, N)
+    ws, wx, wy, _ = O.banded_gotoh(J.band, 1, six(scheme), flat, po, M, J.text, to, N)
     new, sc, sk = shortcut(H, J, scheme, True)
     old, osc, osk = shortcut(H, J, scheme, False)
     bad = np.flatnonzero(new & ((sc != ws) | (sk[:, 0] != wx) | (sk[:, 1] != wy)))
@@ -104,7 +114,7 @@ def check(H, O, R, J, scheme):
     assert not new[N < M + J.band - 1].any()
     assert not (old & ~new).any(), "the rule without the check claims a job the rule with it does not"
     assert np.array_equal(sc[old], osc[old]) and np.array_equal(sk[old], osk[old])
-    if R is not None and J.band in (31, 15):
+    if R is not None and J.band in (31, 15) and len(scheme) == 4:          # (the reference shim instantiates one gap cost)
         full = N >= M + J.band - 1
         rs, rx, ry, _ = R.banded_gotoh(J.band, 1, scheme, flat, po, M, J.text, to, N)
         assert np.array_equal(rs[full], ws[full]) and np.array_equal(rx[full], wx[full]) and np.array_equal(ry[full], wy[full])
@@ -126,12 +136,12 @@ def indel_read(text, p, M, cut, L, insert, rng):
     return np.concatenate([text[p:p + cut], text[p + cut + L:p + M + L]])
 
 
-@pytest.mark.parametrize("band", [31, 15, 8])
+@pytest.mark.parametrize("band", BANDS)
 @pytest.mark.parametrize("scheme", SCHEMES)
 def test_two_substitutions_every_spacing(H, O, R, band, scheme):
     """every pair of rows (adjacent, at and next to both ends); reads with exactly two interior substitutions on random text are all
     claimed whenever their delta lies in the claimed region"""
-    rng = np.random.default_rng(band * 7 + scheme[0])
+    rng = np.random.default_rng(band * 7 + scheme[0] + (0 if len(scheme) == 4 else 100 - scheme[2]))
     text = random_text(rng)
     M = 150
     J = Jobs(text, band)
@@ -203,10 +213,10 @@ def crafted(rng, text, band):
     return J
 
 
-@pytest.mark.parametrize("band", [31, 15, 8])
+@pytest.mark.parametrize("band", BANDS)
 @pytest.mark.parametrize("scheme", SCHEMES)
 def test_crafted_cases(H, O, R, band, scheme):
-    rng = np.random.default_rng(1000 + band * 10 + scheme[0])
+    rng = np.random.default_rng(1000 + band * 10 + scheme[0] + (0 if len(scheme) == 4 else 100 - scheme[2]))
     J = crafted(rng, random_text(rng, repeats=True), band)
     new, old = check(H, O, R, J, scheme)
     print("band %d scheme %s: crafted, %d of %d claimed (without the check %d)" % (band, scheme, new.sum(), len(new), old.sum()))
