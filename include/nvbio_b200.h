@@ -602,6 +602,55 @@ int nvb_seed_extend_paired_traceback(const nvb_fm_index* fmi, const uint32_t* d_
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream);
 
 /* -------------------------------------------------------------------------------------------
+ * Finishing traced alignments for SAM / BAM output (nvBowtie's finish_alignment_kernel, nvBowtie/bowtie2/cuda/traceback_inl.h:520-723,
+ * and what its writers derive from the result, nvbio/io/output/output_sam.cpp:198-315, output_bam.cpp:66-91,
+ * nvbio/io/output/output_utils.h:42-121).  One thread per alignment; no temp buffer; asynchronous on `stream`.
+ *
+ * Inputs: the outputs of nvb_seed_extend_traceback / nvb_seed_extend_paired_traceback as they are (`alignment`: d_ops, max_ops, d_n_ops,
+ * d_begin, d_strand -- all required here; a paired caller passes d_mate_strand as d_strand) and the `reads` passed to that call: n
+ * alignments, alignment i of read i (paired: n = 2 * n_pairs, mate m of pair p at m * n_pairs + p).  d_genome is the 2-bit big-endian
+ * genome of genome_len symbols.  For strand 1 the read is reverse-complemented here (c < 4 ? 3 - c : c, as the traceback call does).
+ * Per alignment, with len = the read's length and M, I, D = the numbers of columns of each op:
+ *   - read span:    the aligned read symbols are [begin.y, begin.y + M + I) of the strand's string; the genome span is
+ *                   [begin.x, begin.x + M + D);
+ *   - CIGAR:        S(begin.y), the ops run-length encoded START -> END, S(len - begin.y - M - I); an S of length 0 is omitted.  BAM
+ *                   encoding: run length << 4 | op (0 M, 1 I, 2 D, 4 S).  d_n_cigar counts the runs, also those beyond max_cigar, which
+ *                   are not stored;
+ *   - MD:Z:         as the SAM specification has it, [0-9]+(([A-Z]|\^[A-Z]+)[0-9]+)*: match counts, the REFERENCE base at a mismatch,
+ *                   ^ and the reference bases of a deletion; a 0 separates adjacent tokens and stands at either end when needed;
+ *                   insertions and soft clips do not appear.  Not NUL-terminated; d_md_len is the full length, also when it exceeds max_md
+ *                   (then only max_md bytes are stored).  MD is at most 2 M + 3 D + 1 <= 3 n_ops + 1 bytes, so max_md = 3 max_ops + 1
+ *                   and max_cigar = max_ops + 2 never truncate;
+ *   - d_edits[4i..] = NM, XM, XO, XG: NM = mismatched M columns + I + D (clips excluded), XM = mismatched M columns, XO = number of I
+ *                   runs + D runs, XG = the sum of (run length - 1) over those runs -- nvBowtie's edit distance (traceback_inl.h:579-660)
+ *                   and analyze_md_string (output_utils.h:77-121);
+ *   - a read N (4-bit reads) in an M column is a mismatch.  So is an M column at a genome coordinate >= genome_len: the banded DP reads
+ *     past a window's end at the genome's end, and such an alignment still runs past the reference (the MD shows N there); clipping it
+ *     is the caller's choice;
+ *   - unaligned (n_ops == 0): n_cigar = 0, md_len = 0, edits all 0;
+ *   - not finishable -- n_ops > max_ops (truncated by the traceback), begin.x == 0xFFFFFFFF with ops, an op byte > 2, or ops consuming more
+ *     read symbols than len - begin.y: n_cigar = 0, md_len = 0, edits = (0xFFFFFFFF, 0, 0, 0).  Nothing is read or written out of bounds.
+ * Deliberate deviations from nvBowtie (DESIGN.md): its MDS keeps the READ base of a mismatch (traceback_inl.h:644-645) and its SAM writer
+ * prints that, omits the 0 between adjacent mismatches and before a leading one, appends a 0 after every deletion (output_sam.cpp:303)
+ * and mis-merges match tokens longer than 255 (output_sam.cpp:263-265); here the MD is spec-conformant.  NM / XM / XO / XG equal nvBowtie's.
+ * NVB_E_INVALID (before any CUDA call) for a NULL genome, reads, alignment, d_ops, d_n_ops, d_begin or d_strand, a NULL output array, or a
+ * max_ops / max_cigar / max_md of 0; NVB_E_UNSUPPORTED for 8-bit reads. */
+typedef struct nvb_finish_out {
+    uint32_t* d_cigar;     /* [n * max_cigar]  BAM encoding (run length << 4 | op), op 0 M, 1 I, 2 D, 4 S; START -> END (genome order) */
+    uint32_t  max_cigar;
+    uint32_t* d_n_cigar;   /* [n]  runs, counted beyond max_cigar without storing them (as d_n_ops) */
+    char*     d_md;        /* [n * max_md]  the MD:Z value, not NUL-terminated */
+    uint32_t  max_md;
+    uint32_t* d_md_len;    /* [n]  full length, also when > max_md (then only max_md bytes are stored) */
+    uint32_t* d_edits;     /* [4 * n]  NM, XM, XO, XG */
+} nvb_finish_out;
+
+int nvb_finish_alignments(const uint32_t* d_genome, uint32_t genome_len,
+                          const nvb_string_set* reads, uint32_t n,
+                          const nvb_best_alignment_out* alignment,
+                          const nvb_finish_out* out, void* stream);
+
+/* -------------------------------------------------------------------------------------------
  * Host-buffer entry point: batches of reads in HOST memory in, per-read results in HOST memory out.
  * Replaces nvBowtie's input thread -> compute thread hand-off and its per-stage cudaDeviceSynchronize
  * (nvBowtie/bowtie2/cuda/compute_thread.cu:213-243, nvBowtie/bowtie2/cuda/defs.h:64, aligner_best_approx.h:219-241):

@@ -9,3 +9,4 @@ from .fmindex import (FMIndexDevice, FMIndexFilterDevice, rank, rank4, match, ma
                       MATCH_FORWARD_ORDER, MATCH_COMPLEMENT)
 from . import aln                                                                # noqa: F401
 from .pipeline import SeedExtendParams, seed_extend, StreamingSeedExtend, PairParams, seed_extend_paired, MapqParams     # noqa: F401
+from .finish import finish_alignments, FinishedAlignments                        # noqa: F401

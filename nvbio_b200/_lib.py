@@ -15,6 +15,7 @@ EXPORTS = [
     "nvb_dict_rank", "nvb_dict_rank4", "nvb_dict_build_occ",
     "nvb_map_seeds", "nvb_fm_locate_init", "nvb_fm_locate_lookup", "nvb_fm_locate_sorted",
     "nvb_pipeline_create", "nvb_pipeline_submit", "nvb_pipeline_wait", "nvb_pipeline_traffic", "nvb_pipeline_destroy",
+    "nvb_finish_alignments",
 ]
 
 
@@ -49,6 +50,11 @@ class SeedExtendParamsStruct(C.Structure):  # nvb_seed_extend_params
 class BestAlignmentOutStruct(C.Structure):   # nvb_best_alignment_out
     _fields_ = [("d_ops", C.c_void_p), ("max_ops", C.c_uint32), ("d_n_ops", C.c_void_p), ("d_begin", C.c_void_p),
                 ("d_strand", C.c_void_p)]
+
+
+class FinishOutStruct(C.Structure):        # nvb_finish_out
+    _fields_ = [("d_cigar", C.c_void_p), ("max_cigar", C.c_uint32), ("d_n_cigar", C.c_void_p), ("d_md", C.c_void_p), ("max_md", C.c_uint32),
+                ("d_md_len", C.c_void_p), ("d_edits", C.c_void_p)]
 
 
 class MapqParamsStruct(C.Structure):       # nvb_mapq_params
