@@ -278,7 +278,9 @@ int nvb_banded_gotoh_score_indirect(int band_len, int type, const nvb_gotoh_sche
  * SHRT_MIN+32 when stored), the BestSink in d_score / d_sink (in/out) and the reference's bool result in d_alive
  * (0 = text shorter than pattern, or the band maximum can no longer reach d_min_score[i] + remaining_rows * match; such
  * alignments are skipped by later passes).  window_begin == 0 initialises score / sink / alive.  d_min_score may be NULL
- * (= INT_MIN: never give up).  Scoring a pattern in consecutive windows yields exactly nvb_banded_gotoh_score's result.
+ * (= INT_MIN: never give up).  Scoring a pattern in consecutive windows yields exactly nvb_banded_gotoh_score's result as long as
+ * every H and F stored in a checkpoint lies in [SHRT_MIN+32, 32767]; a larger value wraps when stored, as in the reference (whose
+ * checkpoints are short2 as well), and the later windows then follow the reference rather than the one-pass score.
  * Replaces aln::banded_alignment_score<BAND_LEN>(aligner, pattern, quals, text, min_score, window_begin, window_end, sink,
  * checkpoint) (nvbio/alignment/banded_inl.h:178-218, gotoh_banded_inl.h:132-199,616-634,706-739), the per-pass body of
  * BatchedBandedAlignmentScore<..., DeviceStagedThreadScheduler> (batched_banded_inl.h:170-241).  bands 3, 5, 7, 15, 31. */

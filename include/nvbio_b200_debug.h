@@ -10,6 +10,12 @@ extern "C" {
 
 /* banded / full-matrix Gotoh: 0 = automatic, 1 = the int32 one-alignment-per-thread kernels for everything */
 void nvb_debug_force_gotoh_path(int path);
+/* route of the last nvb_banded_gotoh_score(_indirect) / nvb_gotoh_score(_indirect) call (also the score pass inside the tracebacks):
+ * *packed = 0 when no 16-bit packed kernel ran (the batch was refused by the admission rules or nvb_debug_force_gotoh_path(1)),
+ * 1 = gotoh_pair_kernel / gotoh_full_pair_kernel, 2 = gotoh_full_warp_kernel; *n_int32 = the alignments that packed kernel put on the
+ * int32 todo list (0 when *packed == 0).  Reads the caller's temp buffer of that call, so only while it is still allocated; synchronises
+ * the device; changes no result */
+int nvb_debug_gotoh_last_route(int* packed, uint32_t* n_int32);
 /* full-matrix pair kernel occupancy variant: 0 = per-type default, 2 / 3 / 4 = minimum CTAs per SM */
 void nvb_debug_full_minb(int minb);
 /* full-matrix dispatch: 0 = by batch size, 1 = always the warp-per-pair kernel, 2 = never */

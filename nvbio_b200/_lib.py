@@ -17,6 +17,12 @@ EXPORTS = [
     "nvb_pipeline_create", "nvb_pipeline_submit", "nvb_pipeline_wait", "nvb_pipeline_traffic", "nvb_pipeline_destroy",
     "nvb_finish_alignments",
 ]
+# test / tuning hooks of include/nvbio_b200_debug.h (not part of the drop-in ABI)
+DEBUG_EXPORTS = [
+    "nvb_debug_gotoh_last_route", "nvb_debug_force_gotoh_path", "nvb_debug_full_minb", "nvb_debug_full_warp", "nvb_debug_full_traceback_warp",
+    "nvb_debug_pair_format", "nvb_debug_pair_rows2", "nvb_debug_traceback_fast", "nvb_debug_pair_extra_smem",
+    "nvb_debug_pipeline_path", "nvb_debug_seed_split", "nvb_debug_perfect_shortcut", "nvb_debug_dp_jobs", "nvb_debug_mapq_eval",
+]
 
 
 class NvbError(RuntimeError):
@@ -98,7 +104,7 @@ def lib():
         _lib.nvb_error_string.restype = C.c_char_p
         _lib.nvb_pipeline_destroy.restype = None
         _lib.nvb_pipeline_traffic.restype = None
-        for name in EXPORTS:
+        for name in EXPORTS + DEBUG_EXPORTS:
             getattr(_lib, name)            # raises AttributeError if a symbol is not exported
     return _lib
 

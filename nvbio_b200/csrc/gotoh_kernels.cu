@@ -730,6 +730,11 @@ static int g_force_path = 0;
 static int g_full_warp = 0;           // 0 = by batch size, 1 = always the warp-per-pair kernel, 2 = never (nvb_debug_full_warp)
 static uint32_t g_full_warp_max_pairs = 30000u;   // measured cross-over with the thread-per-pair kernel: ~50-60 K alignments
 static int g_full_minb = 0;          // 0 = per-type default; tuning knob of gotoh_full_pair_kernel's occupancy (nvb_debug_full_minb)
+// route of the last banded / full-matrix score call (nvb_debug_gotoh_last_route): 0 = no packed kernel, 1 = pair kernel, 2 = warp
+// kernel, and the todo-list count of that call (in the caller's temp buffer)
+static int g_route_packed = 0;
+static const uint32_t* g_route_todo_count = nullptr;
+static void set_route(int packed, const uint32_t* todo_count) { g_route_packed = packed; g_route_todo_count = todo_count; }
 
 static int banded_impl(int band, int type, const nvb_gotoh_scheme* scheme,
                        const nvb_string_set* patterns, const uint8_t* d_quals, const nvb_string_set* texts,
@@ -761,8 +766,9 @@ static int banded_impl(int band, int type, const nvb_gotoh_scheme* scheme,
     const size_t smem = (size_t)((sel_rows + 15u) & ~15u) * PAIR_BLOCKDIM * sizeof(uint16_t);          // as launch_pair_fmt sizes it (two-byte selectors)
     const bool fast = (g_force_path != 1) && texts->bits == 2 && max_m >= 1 && smem <= 200u * 1024u &&
                       pair_path_ok(band, type, scheme, max_m);
-    if (!fast) return dispatch_generic(band, type, S, b, nullptr, nullptr, n_max, s);
+    if (!fast) { set_route(0, nullptr); return dispatch_generic(band, type, S, b, nullptr, nullptr, n_max, s); }
 
+    set_route(1, todo_count);
     NVB_CUDA_TRY(cudaMemsetAsync(todo_count, 0, sizeof(uint32_t), s));
     int r = dispatch_pair(band, type, S, b, sel_rows, todo, todo_count, s);
     if (r != NVB_OK) return r;
@@ -855,6 +861,7 @@ static int gotoh_full_impl(int type, const nvb_gotoh_scheme* scheme, const nvb_s
     cudaStream_t s = as_stream(stream);
     const bool packed = g_force_path != 1 && full_pair_path_ok(type, scheme, patterns->length, texts->length);
     if (!packed) {
+        set_route(0, nullptr);
         switch (type) {
         case NVB_GLOBAL:      gotoh_full_kernel<NVB_GLOBAL><<<grid, GENERIC_BLOCKDIM, 0, s>>>(S, b, col); break;
         case NVB_LOCAL:       gotoh_full_kernel<NVB_LOCAL><<<grid, GENERIC_BLOCKDIM, 0, s>>>(S, b, col); break;
@@ -871,6 +878,7 @@ static int gotoh_full_impl(int type, const nvb_gotoh_scheme* scheme, const nvb_s
     // with a device-side count (`n` is then only a capacity) the batch is usually much smaller than its capacity: allow 4x
     const bool use_warp = g_full_warp == 1 || (g_full_warp == 0 && n_pairs <= (d_n ? 4u : 1u) * g_full_warp_max_pairs);
     if (use_warp && max_m >= 1u && max_m <= 256u && !S.qtab) {           // (the warp kernel has no quality-table form)
+        set_route(2, todo_count);
         const uint32_t Wc = (max_m + 31u) / 32u;
         const uint32_t wgrid = (uint32_t)(((uint64_t)n_pairs * 32u + WARP_BLOCKDIM - 1) / WARP_BLOCKDIM);
         const uint32_t tgrid2 = grid < sm_count() * 8u ? grid : sm_count() * 8u;
@@ -892,6 +900,7 @@ static int gotoh_full_impl(int type, const nvb_gotoh_scheme* scheme, const nvb_s
         NVB_LAUNCH_CHECK();
         return NVB_OK;
     }
+    set_route(1, todo_count);
     const uint32_t pgrid = (n_pairs + PAIR_BLOCKDIM - 1) / PAIR_BLOCKDIM;
     uint32_t tgrid = grid < sm_count() * 8u ? grid : sm_count() * 8u;
     // occupancy: with two text rows in flight every type fits spill-free at 2 CTAs per SM (210-250 registers); tools/bench_full.py
@@ -972,8 +981,10 @@ int nvb_banded_gotoh_traceback(int band_len, int type, const nvb_gotoh_scheme* s
     TracebackOut o;
     o.source = (uint2*)d_source; o.ops = d_ops; o.n_ops = d_n_ops; o.max_ops = max_ops; o.dirs = dirs; o.dir_rows = max_m;
     const GotohScheme S = make_scheme(scheme);
-    if (!g_traceback_fast || type == NVB_GLOBAL)
+    if (!g_traceback_fast || type == NVB_GLOBAL) {
+        set_route(0, nullptr);
         return dispatch_traceback(band_len, type, S, b, o, nullptr, nullptr, s);
+    }
     // 1. score + sink with the score kernels (DPX where admitted); 2. the gapless fast path resolves every alignment whose optimal path
     // has no gap (most reads) from the sink alone; 3. the rest goes through the direction-matrix traceback
     {
@@ -1104,6 +1115,7 @@ int nvb_gotoh_traceback(int type, const nvb_gotoh_scheme* scheme, const nvb_stri
     const GotohScheme S = make_scheme(scheme);
     const uint32_t grid = (n + GENERIC_BLOCKDIM - 1) / GENERIC_BLOCKDIM;
     cudaStream_t s = as_stream(stream);
+    set_route(0, nullptr);
     switch (type) {
     case NVB_GLOBAL: gotoh_full_traceback_kernel<NVB_GLOBAL><<<grid, GENERIC_BLOCKDIM, 0, s>>>(S, b, col, o, dir_row_words); break;
     case NVB_LOCAL:  gotoh_full_traceback_kernel<NVB_LOCAL><<<grid, GENERIC_BLOCKDIM, 0, s>>>(S, b, col, o, dir_row_words); break;
@@ -1122,5 +1134,15 @@ void nvb_debug_pair_rows2(int on) { nvb::g_pair_rows2 = on; }
 void nvb_debug_traceback_fast(int on) { nvb::g_traceback_fast = on; }
 void nvb_debug_pair_extra_smem(int bytes) { nvb::g_pair_extra_smem = bytes > 0 ? bytes : 0; }
 void nvb_debug_pair_format(int on) { nvb::g_pair_fmt_ok = on != 0; }
+int nvb_debug_gotoh_last_route(int* packed, uint32_t* n_int32)
+{
+    if (!packed || !n_int32) return NVB_E_INVALID;
+    *packed = g_route_packed;
+    *n_int32 = 0u;
+    if (!g_route_packed) return NVB_OK;
+    NVB_CUDA_TRY(cudaDeviceSynchronize());
+    NVB_CUDA_TRY(cudaMemcpy(n_int32, g_route_todo_count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    return NVB_OK;
+}
 
 } // extern "C"

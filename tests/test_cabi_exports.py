@@ -7,8 +7,8 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def declared_symbols():
-    src = open(os.path.join(ROOT, "include", "nvbio_b200.h")).read()
+def declared_symbols(header="nvbio_b200.h"):
+    src = open(os.path.join(ROOT, "include", header)).read()
     src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
     return sorted(set(re.findall(r"\b(nvb_[a-z0-9_]+)\s*\(", src)))
 
@@ -31,6 +31,11 @@ def test_library_builds_and_exports_everything():
 def test_python_mirror_lists_same_exports():
     from nvbio_b200 import _lib
     assert set(_lib.EXPORTS) == set(declared_symbols())
+    # the test / tuning hooks: listed apart, and every one of them exported (lib() resolves both lists)
+    assert set(_lib.DEBUG_EXPORTS) == set(declared_symbols("nvbio_b200_debug.h"))
+    L = _lib.lib()
+    for n in _lib.DEBUG_EXPORTS:
+        assert hasattr(L, n), "missing export %s" % n
 
 
 def test_argument_validation_without_gpu():
