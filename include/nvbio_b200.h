@@ -653,6 +653,77 @@ int nvb_finish_alignments(const uint32_t* d_genome, uint32_t genome_len,
                           const nvb_finish_out* out, void* stream);
 
 /* -------------------------------------------------------------------------------------------
+ * BAM alignment records of traced and finished alignments (the bam1_t wire layout of the SAM / BAM specification, what htslib's
+ * bam_write1 writes after its BGZF framing, contrib/htslib/sam.c:335-361; nvBowtie's BAM and SAM writers, output_bam.cpp:234-446,
+ * output_sam.cpp:354-530).  Asynchronous on `stream`, no host round trip; NVB_E_TEMP_SIZE protocol.
+ *
+ * Inputs (nvb_bam_in): the `reads` passed to the traceback call and optional base qualities d_read_quals (phred values indexed like the
+ * read symbols); the traceback outputs d_n_ops / d_begin / d_strand; the nvb_finish_out of nvb_finish_alignments; the alignment score
+ * (d_best_score, or d_mate_score when paired); optional d_mapq (or d_mate_mapq) and second score (d_second_score / d_mate_second_score);
+ * paired only: d_pair_flags.  The contig table d_contig_begin[n_contigs + 1] holds concatenated coordinates, increasing, [0] = 0,
+ * [n_contigs] = genome length.  Read names: bytes d_names, name j = [d_name_offsets[j], d_name_offsets[j + 1]), one per read when single
+ * end and one per pair when paired, 1-254 printable bytes (longer names are cut at 254 bytes).
+ * n alignments: single end, alignment i is read i and record i; paired (d_pair_flags != NULL, n even), alignment m * n / 2 + p (mate m of
+ * pair p) becomes record 2p + m.
+ *
+ * Placement of an alignment, with M / D the columns of its CIGAR: span = [begin.x, begin.x + M + D); refID = upper_bound(contig_begin,
+ * begin.x) - 1; pos = begin.x - contig_begin[refID].  It is MAPPED only if n_ops > 0, finish wrote it whole (NM != 0xFFFFFFFF, n_cigar <=
+ * max_cigar and <= 65535, md_len <= max_md) and its span lies inside one contig (contig_begin[refID] <= begin.x < contig_begin[refID + 1]
+ * and begin.x + M + D <= contig_begin[refID + 1]).  A span that crosses a contig boundary or runs past the genome (the genome-end M
+ * columns of nvb_finish_alignments) is reported unmapped, as nvBowtie does (output_sam.cpp:457-464, output_bam.cpp:351-366); so the
+ * mate sees an unmapped mate.
+ * A mapped record:
+ *   FLAG   0x10 on strand 1; paired: 0x1, 0x40 / 0x80 for mate 1 / 2, 0x2 when the pair is CONCORDANT or RESCUED and both mates are
+ *          mapped, 0x8 when the mate is unmapped, 0x20 when the mate is mapped on strand 1;
+ *   MAPQ   d_mapq, 255 without it;   bin = reg2bin(pos, pos + M + D) (the specification's, hts_reg2bin(beg, end, 14, 5));
+ *   CIGAR  the finish output;  SEQ the strand's string (strand 1 reverse-complemented, as the traceback saw it) in BAM's 4-bit
+ *          =ACMGRSVTWYHKDBN code (A 1, C 2, G 4, T 8, N 15);  QUAL reversed for strand 1, all 0xFF without qualities;
+ *   mate   mate mapped: next_refID / next_pos = its placement; TLEN = +-(max end - min begin) on the same contig (+ for the smaller
+ *          begin, mate 1 on equal begins), 0 on different contigs.  Mate unmapped: its own placement, TLEN 0.  Single end: -1 / -1 / 0;
+ *   tags   NM, AS, XS (only when the second score is given and not INT_MIN), XM, XO, XG, MD:Z (when not empty), in nvBowtie's order
+ *          (output_sam.cpp:354-363); an integer tag has the type htslib's SAM parser picks: the smallest of c / s / i for a negative
+ *          value, of C / S / I otherwise (contrib/htslib/sam.c:783-806), so a record is byte-identical to htslib's encoding of its SAM line.
+ * An unmapped record: FLAG 0x4 plus the paired bits above (0x20 / 0x8 describe the mate), MAPQ 0, no CIGAR, no tags, SEQ / QUAL of the
+ * read as given; with a mapped mate it takes the mate's refID / pos as its own and as next_refID / next_pos, bin = reg2bin(pos, pos + 1);
+ * otherwise refID, pos, next_refID and next_pos are -1 and bin = 4680.
+ * Deliberate deviations from nvBowtie's writers, which the specification decides (DESIGN.md section 3.13): a real bin (nvBowtie: 0),
+ * next_refID = the mate's contig (output_bam.cpp:400 writes a difference of contig indices), NM typed by value (nvBowtie: c, which wraps
+ * above 127), paired bits and the mate's placement on unmapped records, no MD:Z:* for an empty MD, TLEN signed on equal begins, no 0x2
+ * when a mate was unmapped by the contig rule, and XS from the MAPQ calls' second score (nvBowtie never writes it).
+ *
+ * Outputs (nvb_bam_out): record i occupies bytes [d_offsets[i], d_offsets[i + 1]) of d_records (16-byte aligned), starting with its
+ * block_size; d_offsets[n] is the total size.  d_offsets is always written whole; a record is stored only if it fits whole within
+ * `capacity` (d_records may be NULL when capacity is 0: a sizing call).  d_counts[4] = records, mapped, unmapped because the span left
+ * its contig or the genome, unmapped because the finish outputs were missing or truncated.
+ * NVB_E_INVALID (before any CUDA call) for a NULL in / out / temp_bytes, NULL required pointers (reads, d_n_ops, d_begin, d_strand, the
+ * finish arrays, d_score, d_contig_begin, d_names, d_name_offsets, d_offsets, d_counts, d_records with capacity > 0), a misaligned
+ * d_records, n_contigs == 0, max_cigar / max_md == 0, 8-bit reads, or an odd n when paired. */
+typedef struct nvb_bam_in {
+    nvb_string_set   reads;
+    const uint8_t*   d_read_quals;     /* may be NULL */
+    const uint32_t*  d_n_ops;          /* [n] */
+    const nvb_uint2* d_begin;          /* [n] */
+    const uint8_t*   d_strand;         /* [n] */
+    nvb_finish_out   finish;           /* the outputs of nvb_finish_alignments over the same n alignments */
+    const int32_t*   d_score;          /* [n] AS */
+    const uint8_t*   d_mapq;           /* [n], may be NULL: MAPQ 255 */
+    const int32_t*   d_second_score;   /* [n], may be NULL: no XS */
+    const uint32_t*  d_pair_flags;     /* [n / 2] NVB_PAIR_*; NULL: single end */
+    const uint32_t*  d_contig_begin;   /* [n_contigs + 1] */
+    uint32_t         n_contigs;
+    const char*      d_names;
+    const uint32_t*  d_name_offsets;   /* [n_names + 1] */
+} nvb_bam_in;
+typedef struct nvb_bam_out {
+    uint8_t*  d_records;
+    uint64_t  capacity;
+    uint64_t* d_offsets;               /* [n + 1] */
+    uint32_t* d_counts;                /* [4] */
+} nvb_bam_out;
+
+int nvb_bam_records(const nvb_bam_in* in, uint32_t n, const nvb_bam_out* out, void* d_temp, size_t* temp_bytes, void* stream);
+
+/* -------------------------------------------------------------------------------------------
  * Host-buffer entry point: batches of reads in HOST memory in, per-read results in HOST memory out.
  * Replaces nvBowtie's input thread -> compute thread hand-off and its per-stage cudaDeviceSynchronize
  * (nvBowtie/bowtie2/cuda/compute_thread.cu:213-243, nvBowtie/bowtie2/cuda/defs.h:64, aligner_best_approx.h:219-241):

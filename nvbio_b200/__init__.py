@@ -10,3 +10,4 @@ from .fmindex import (FMIndexDevice, FMIndexFilterDevice, rank, rank4, match, ma
 from . import aln                                                                # noqa: F401
 from .pipeline import SeedExtendParams, seed_extend, StreamingSeedExtend, PairParams, seed_extend_paired, MapqParams     # noqa: F401
 from .finish import finish_alignments, FinishedAlignments                        # noqa: F401
+from .bam import ContigTable, BamRecords, bam_records, bam_header, write_bam, numbered_names    # noqa: F401

@@ -15,7 +15,7 @@ EXPORTS = [
     "nvb_dict_rank", "nvb_dict_rank4", "nvb_dict_build_occ",
     "nvb_map_seeds", "nvb_fm_locate_init", "nvb_fm_locate_lookup", "nvb_fm_locate_sorted",
     "nvb_pipeline_create", "nvb_pipeline_submit", "nvb_pipeline_wait", "nvb_pipeline_traffic", "nvb_pipeline_destroy",
-    "nvb_finish_alignments",
+    "nvb_finish_alignments", "nvb_bam_records",
 ]
 # test / tuning hooks of include/nvbio_b200_debug.h (not part of the drop-in ABI)
 DEBUG_EXPORTS = [
@@ -61,6 +61,17 @@ class BestAlignmentOutStruct(C.Structure):   # nvb_best_alignment_out
 class FinishOutStruct(C.Structure):        # nvb_finish_out
     _fields_ = [("d_cigar", C.c_void_p), ("max_cigar", C.c_uint32), ("d_n_cigar", C.c_void_p), ("d_md", C.c_void_p), ("max_md", C.c_uint32),
                 ("d_md_len", C.c_void_p), ("d_edits", C.c_void_p)]
+
+
+class BamInStruct(C.Structure):           # nvb_bam_in
+    _fields_ = [("reads", StringSetStruct), ("d_read_quals", C.c_void_p), ("d_n_ops", C.c_void_p), ("d_begin", C.c_void_p),
+                ("d_strand", C.c_void_p), ("finish", FinishOutStruct), ("d_score", C.c_void_p), ("d_mapq", C.c_void_p),
+                ("d_second_score", C.c_void_p), ("d_pair_flags", C.c_void_p), ("d_contig_begin", C.c_void_p), ("n_contigs", C.c_uint32),
+                ("d_names", C.c_void_p), ("d_name_offsets", C.c_void_p)]
+
+
+class BamOutStruct(C.Structure):          # nvb_bam_out
+    _fields_ = [("d_records", C.c_void_p), ("capacity", C.c_uint64), ("d_offsets", C.c_void_p), ("d_counts", C.c_void_p)]
 
 
 class MapqParamsStruct(C.Structure):       # nvb_mapq_params

@@ -67,3 +67,21 @@ def load_index(prefix: str, device="cuda") -> FMIndexDevice:
     if not np.array_equal(got, f["cum"].astype(np.uint64)):
         raise IOError("cumulative symbol counts of %s.bwt do not match its header" % prefix)
     return fmi
+
+
+def read_ann(path: str):
+    """the contig annotations of an nvBWT / BWA .ann file (nvbio's save_bns / load_bns, nvbio/basic/bnt.cpp:37-160): a line
+    "l_pac n_seqs seed", then per sequence "gi name [comment]" and "offset len n_ambs".  A name ends at the first white space.  Returns
+    dict(l_pac, names, offsets, lengths)."""
+    with open(path) as f:
+        head = f.readline().split()
+        if len(head) < 2:
+            raise IOError("%s: missing the l_pac / n_seqs line" % path)
+        l_pac, n_seqs = int(head[0]), int(head[1])
+        names, offsets, lengths = [], [], []
+        for i in range(n_seqs):
+            a, b = f.readline().split(), f.readline().split()
+            if len(a) < 2 or len(b) < 2:
+                raise IOError("%s: sequence %d of %d is truncated" % (path, i, n_seqs))
+            names.append(a[1]); offsets.append(int(b[0])); lengths.append(int(b[1]))
+    return dict(l_pac=l_pac, names=names, offsets=np.array(offsets, np.int64), lengths=np.array(lengths, np.int64))
