@@ -13,6 +13,8 @@
 #include "gotoh_core.cuh"
 #include "pipeline_core.cuh"
 #include "gotoh_full_core.cuh"
+#include <cub/agent/single_pass_scan_operators.cuh>
+#include <cub/block/block_scan.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_sort.cuh>
 #include <mutex>
@@ -146,7 +148,8 @@ __device__ __forceinline__ uint32_t best_key_index(unsigned long long key) { ret
 // running more than band/2 symbols past the genome's end gets such a window; it never becomes a best, second-best or pair candidate
 __device__ __forceinline__ bool job_aligned(uint2 sink) { return sink.x != 0xFFFFFFFFu; }
 
-// one thread per (string, seed slot): SA range of the seed, and its clamped size.
+// one thread per (string, seed slot): SA range of the seed, and its clamped size (sizes == NULL on the per-read path, which sums the
+// sizes of a read's ranges itself).
 // genome != NULL (the per-read path on an index with the full suffix array): single-row ranges are located on the spot --
 // ranges[q] = (text position, 0xFFFFFFFF), see fm_match_locate_one -- so that neither the remaining LF steps nor the later SA
 // gather of that hit are needed; wider ranges stay SA ranges.
@@ -189,7 +192,7 @@ pipe_seed_match_kernel(const FmIndex f, const PipeGeom g, const uint32_t* __rest
                     fm_match_one<BITS, true>(f, words, s * g.stride + pos, g.seed_len, 0u, x, y);
             }
             ranges[q] = make_uint2(x, y);
-            if (!deferred) sizes[q] = seed_range_hits(make_uint2(x, y), g.max_seed_hits);
+            if (sizes && !deferred) sizes[q] = seed_range_hits(make_uint2(x, y), g.max_seed_hits);
         }
         if (DEFER) {
             // one atomic per warp, spread over SEED_TODO_LISTS counters, each in its own 128-byte line: same-line atomics serialise
@@ -225,7 +228,7 @@ pipe_seed_match_wide_kernel(const FmIndex f, const PipeGeom g, const uint32_t* _
         uint32_t x = r.x, y = r.y;
         if (fm_match_locate_one<BITS, true, FM_RESUME>(f, genome, words, s * g.stride + k * g.seed_interval, g.seed_len, x, y) == FM_EMPTY) { x = 1; y = 0; }
         ranges[q] = make_uint2(x, y);
-        sizes[q] = seed_range_hits(make_uint2(x, y), g.max_seed_hits);
+        if (sizes) sizes[q] = seed_range_hits(make_uint2(x, y), g.max_seed_hits);
     }
 }
 
@@ -275,39 +278,95 @@ pipe_expand_hits_kernel(const FmIndex f, const PipeGeom g, const uint2* __restri
 }
 
 // ---------------------------------------------------------------------------------------------
-// per-read path (no per-hit outputs requested): one thread per read locates its hits and keeps only the distinct (strand, window)
-// alignment jobs -- no per-hit array is written at all.  Jobs are staged per CTA in shared memory and appended to the global
-// job list with one atomic per CTA; their order varies from run to run, the results do not (every job carries the index of the
-// first hit that produced it, and the best-per-read reduction breaks score ties by it exactly as the per-hit path does).
+// per-read path (no per-hit outputs requested): pipe_resolve_reads_kernel takes the seed ranges to the distinct (strand, window)
+// alignment jobs of every read, their results where the exact shortcut proves them, and the best of those per read -- no per-seed
+// size, no hit-slot scan and no per-hit array.  The jobs it leaves to the DP are scored after it; pipe_scatter_dp_kernel and
+// pipe_finalize_dp_kernel then let a DP job replace a read's result when it beats the claimed best.  Job order varies from run to run,
+// the results do not (every job carries the index of its first hit, and the best-per-read key breaks score ties by it exactly as the
+// per-hit path breaks them by the hit index).
 // ---------------------------------------------------------------------------------------------
-constexpr uint32_t RJ_BLOCK = 128;          // reads per CTA
-constexpr uint32_t RJ_STAGE = 640;          // staged jobs per CTA (average: ~1.2 per read)
-constexpr int      RJ_LOCAL = 6;            // distinct windows remembered per read (more are still scored, just not de-duplicated)
+struct Jobs { uint32_t *p_off, *p_len, *t_off, *t_len; };   // alignment jobs: a read string (offset, length) against a genome window
 
-__global__ void __launch_bounds__(RJ_BLOCK)
-pipe_read_jobs_kernel(const FmIndex f, const PipeGeom g, const uint2* __restrict__ ranges, const uint32_t* __restrict__ sizes,
-                      const uint32_t* __restrict__ excl, const uint32_t* __restrict__ slen, uint32_t* __restrict__ counts,
-                      uint32_t* __restrict__ j_string, uint32_t* __restrict__ j_first,
-                      uint32_t* __restrict__ jp_off, uint32_t* __restrict__ jp_len, uint32_t* __restrict__ jt_off, uint32_t* __restrict__ jt_len)
+constexpr uint32_t RJ_BLOCK = 128;          // reads per tile (one CTA, one thread per read in phase A)
+constexpr uint32_t RJ_STAGE = 640;          // staged jobs per CTA (average: ~1.2 per read); more go straight to the global lists
+constexpr int      RJ_LOCAL = 6;            // distinct windows remembered per read (more are still scored, just not de-duplicated)
+constexpr uint32_t RJ_CLAIMED = 0xFFFFFFFFu, RJ_CLAIMED_EMPTY = 0xFFFFFFFEu;   // st_slot of a job the shortcut resolved (else: DP slot)
+using RjTileState = cub::ScanTileState<uint32_t>;
+using RjPrefixOp  = cub::TilePrefixCallbackOp<uint32_t, ::cuda::std::plus<uint32_t>, RjTileState>;
+
+// the tile states of the hit-slot look-back and the counters of one call, reset in stream order: counts[2] = jobs, counts[3] = tile ticket
+__global__ void __launch_bounds__(256)
+pipe_resolve_init_kernel(RjTileState tiles, const uint32_t n_tiles, uint32_t* __restrict__ counts, uint32_t* __restrict__ dp_count)
 {
-    __shared__ uint32_t st_string[RJ_STAGE], st_first[RJ_STAGE], st_toff[RJ_STAGE], st_tlen[RJ_STAGE];
-    __shared__ uint32_t s_cnt, s_base;
-    if (threadIdx.x == 0) s_cnt = 0u;
+    tiles.InitializeStatus((int)n_tiles);
+    if (blockIdx.x == 0 && threadIdx.x == 0) { counts[2] = 0u; counts[3] = 0u; *dp_count = 0u; }
+}
+
+// One tile of RJ_BLOCK reads per CTA.
+//  * Hit slots: each read sums its clamped range sizes (its ranges are read from global memory: staging the tile's 28 KB of ranges in
+//    shared memory measured 0.71 ms against 0.53 on the headline step: it cut the CTAs per SM from 7 to 5); a block scan plus a single-pass decoupled look-back over the tiles gives its first
+//    slot (the per-hit path's exclusive scan at the read's first seed).  The tile index comes from a ticket, so every tile a CTA waits
+//    on belongs to a CTA that is already running.  The last tile writes counts[0] = min(total, capacity), counts[1] = total.
+//  * Phase A, one thread per read: locate, window and the RJ_LOCAL-window de-duplication (strands shared) of every kept hit
+//    (slot < hit_capacity); jobs are staged in shared memory, a job that does not fit goes straight to the job list and the DP list.
+//  * Phase B, the whole CTA over the staged jobs: append them to the job list (one atomic), run the exact shortcut (shortcut: 0 = off,
+//    1 = with its one-gap check, 2 = without), compact the others into the DP list (one atomic) and reduce the claimed results per read
+//    (64-bit make_best_key in shared memory).  Every read's best_key / score / end / strand is written here (none: 0 / INT_MIN /
+//    0xFFFFFFFF / 0); a DP job replaces it later only with a larger key.
+// 8 CTAs (32 warps) per SM, 64 registers, no spills: measured against 7 and 10 CTAs and against 64-read tiles at 14, 16 and 20 (DESIGN 5)
+__global__ void __launch_bounds__(RJ_BLOCK, 8)
+pipe_resolve_reads_kernel(const FmIndex f, const PipeGeom g, const uint2* __restrict__ ranges, const uint32_t* __restrict__ slen,
+                          const uint32_t hit_capacity, RjTileState tiles, const uint32_t n_tiles, uint32_t* __restrict__ counts,
+                          const int shortcut, const int32_t match, const int32_t mismatch, const int32_t max_gap_open,
+                          const uint32_t* __restrict__ str_words, const uint32_t* __restrict__ genome,
+                          uint32_t* __restrict__ j_string, uint32_t* __restrict__ j_first, const Jobs jobs,
+                          int32_t* __restrict__ job_score, uint2* __restrict__ job_sink,
+                          const Jobs dp, uint32_t* __restrict__ dp_job, uint32_t* __restrict__ dp_count,
+                          unsigned long long* __restrict__ best_key, int32_t* best_score, uint32_t* best_pos, uint8_t* __restrict__ best_strand)
+{
+    using BlockScan = cub::BlockScan<uint32_t, RJ_BLOCK>;
+    __shared__ struct { typename RjPrefixOp::TempStorage prefix; typename BlockScan::TempStorage scan; } s_tmp;
+    __shared__ uint32_t st_string[RJ_STAGE], st_first[RJ_STAGE], st_toff[RJ_STAGE], st_tlen[RJ_STAGE], st_slot[RJ_STAGE];
+    __shared__ unsigned long long s_key[RJ_BLOCK];
+    __shared__ int32_t s_score[RJ_BLOCK];
+    __shared__ uint32_t s_pos[RJ_BLOCK];
+    __shared__ uint8_t s_strand[RJ_BLOCK];
+    __shared__ uint32_t s_tile, s_cnt, s_base, s_dp_cnt, s_dp_base;
+    if (threadIdx.x == 0) { s_tile = atomicAdd(counts + 3, 1u); s_cnt = 0u; s_dp_cnt = 0u; }
+    s_key[threadIdx.x] = 0ull;
     __syncthreads();
-    const uint32_t r = blockIdx.x * RJ_BLOCK + threadIdx.x;
-    const uint32_t kept = counts[0];
-    if (r < g.n_reads) {
+    const uint32_t tile = s_tile, r0 = tile * RJ_BLOCK, r = r0 + threadIdx.x;
+    const uint32_t per_read = g.strands * g.seeds_per_string;
+    const bool live = r < g.n_reads;
+    const uint2* rr = ranges + (size_t)r * per_read;            // this read's ranges: q = (r * strands + strand) * seeds + k
+
+    // hit slots
+    uint32_t hits = 0, run = 0;
+    if (live)
+        for (uint32_t q = 0; q < per_read; ++q) hits += seed_range_hits(rr[q], g.max_seed_hits);
+    if (tile == 0) {
+        uint32_t aggregate;
+        BlockScan(s_tmp.scan).ExclusiveSum(hits, run, aggregate);
+        if (threadIdx.x == 0) tiles.SetInclusive(0, aggregate);
+    } else {
+        RjPrefixOp prefix(tiles, s_tmp.prefix, ::cuda::std::plus<uint32_t>{}, (int)tile);
+        BlockScan(s_tmp.scan).ExclusiveSum(hits, run, prefix);
+    }
+    if (tile == n_tiles - 1u && threadIdx.x == RJ_BLOCK - 1u) {  // dead threads add 0: the last thread's inclusive sum is the total
+        const uint32_t total = run + hits;
+        counts[1] = total;
+        counts[0] = total < hit_capacity ? total : hit_capacity;
+    }
+
+    // phase A
+    if (live) {
         uint32_t lk_s[RJ_LOCAL], lk_b[RJ_LOCAL], lk_e[RJ_LOCAL];
         int n_local = 0;
-        // hit slots of this read: the scan's value at its first seed plus a running sum of the (clamped) range sizes, which are
-        // recomputed from the ranges exactly as the match kernel stored them -- one 8-byte load per seed instead of 16
-        uint32_t run = excl[r * g.strands * g.seeds_per_string];
         for (uint32_t strand = 0; strand < g.strands; ++strand) {
             const uint32_t s = r * g.strands + strand;
             const uint32_t len = slen[s];
             for (uint32_t k = 0; k < g.seeds_per_string; ++k) {
-                const uint32_t q = s * g.seeds_per_string + k;
-                const uint2 rq = ranges[q];
+                const uint2 rq = rr[strand * g.seeds_per_string + k];
                 const bool located = rq.y == 0xFFFFFFFFu;                              // already a text position (fm_match_locate_one)
                 const uint32_t sz = seed_range_hits(rq, g.max_seed_hits);
                 if (sz == 0u) continue;
@@ -315,7 +374,7 @@ pipe_read_jobs_kernel(const FmIndex f, const PipeGeom g, const uint2* __restrict
                 run += sz;
                 for (uint32_t j = 0; j < sz; ++j) {
                     const uint32_t h = base + j;
-                    if (h >= kept) break;                                              // beyond the caller's capacity
+                    if (h >= hit_capacity) break;                                      // beyond the caller's capacity
                     const uint2 w = hit_window(located ? x : fm_locate_one(f, x + j), seed_begin, len, g);
                     bool seen = false;
 #pragma unroll
@@ -326,114 +385,92 @@ pipe_read_jobs_kernel(const FmIndex f, const PipeGeom g, const uint2* __restrict
                     if (n_local < RJ_LOCAL) ++n_local;
                     const uint32_t slot = atomicAdd(&s_cnt, 1u);
                     if (slot < RJ_STAGE) { st_string[slot] = s; st_first[slot] = h; st_toff[slot] = w.x; st_tlen[slot] = w.y - w.x; }
-                    else {                                                             // staging full: straight to the global list
-                        const uint32_t o = atomicAdd(counts + 2, 1u);
-                        j_string[o] = s; j_first[o] = h; jp_off[o] = s * g.stride; jp_len[o] = len; jt_off[o] = w.x; jt_len[o] = w.y - w.x;
+                    else {                                                             // staging full: straight to both global lists
+                        const uint32_t o = atomicAdd(counts + 2, 1u), d = atomicAdd(dp_count, 1u);
+                        j_string[o] = s; j_first[o] = h;
+                        jobs.p_off[o] = s * g.stride; jobs.p_len[o] = len; jobs.t_off[o] = w.x; jobs.t_len[o] = w.y - w.x;
+                        dp.p_off[d] = s * g.stride; dp.p_len[d] = len; dp.t_off[d] = w.x; dp.t_len[d] = w.y - w.x; dp_job[d] = o;
                     }
                 }
             }
         }
     }
     __syncthreads();
+
+    // phase B: job list, exact shortcut, claimed best per read
     const uint32_t n = s_cnt < RJ_STAGE ? s_cnt : RJ_STAGE;
     if (threadIdx.x == 0) s_base = n ? atomicAdd(counts + 2, n) : 0u;
     __syncthreads();
     for (uint32_t i = threadIdx.x; i < n; i += RJ_BLOCK) {
-        const uint32_t o = s_base + i, s = st_string[i];
-        j_string[o] = s; j_first[o] = st_first[i]; jp_off[o] = s * g.stride; jp_len[o] = slen[s]; jt_off[o] = st_toff[i]; jt_len[o] = st_tlen[i];
+        const uint32_t o = s_base + i, s = st_string[i], first = st_first[i], len = slen[s], to = st_toff[i], N = st_tlen[i];
+        j_string[o] = s; j_first[o] = first; jobs.p_off[o] = s * g.stride; jobs.p_len[o] = len; jobs.t_off[o] = to; jobs.t_len[o] = N;
+        int32_t score = 0; uint32_t sx = 0, sy = 0;
+        if (shortcut && gapless_job_shortcut(str_words, genome, s * g.stride, len, to, N, g.band, match, mismatch, max_gap_open, score, sx, sy,
+                                             shortcut != 2)) {
+            const uint2 sk = make_uint2(sx, sy);
+            job_score[o] = score; job_sink[o] = sk;
+            if (job_aligned(sk)) {
+                st_slot[i] = RJ_CLAIMED; st_toff[i] = to + sx; st_tlen[i] = (uint32_t)score;   // (the DP list never reads a claimed job)
+                atomicMax(&s_key[s / g.strands - r0], make_best_key(score, first));
+            } else st_slot[i] = RJ_CLAIMED_EMPTY;
+        } else st_slot[i] = atomicAdd(&s_dp_cnt, 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) s_dp_base = s_dp_cnt ? atomicAdd(dp_count, s_dp_cnt) : 0u;
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < n; i += RJ_BLOCK) {
+        const uint32_t slot = st_slot[i], s = st_string[i];
+        if (slot == RJ_CLAIMED) {                                // the claimed job whose key won writes its read's result
+            const uint32_t rl = s / g.strands - r0;
+            const int32_t score = (int32_t)st_tlen[i];
+            if (s_key[rl] == make_best_key(score, st_first[i])) { s_score[rl] = score; s_pos[rl] = st_toff[i]; s_strand[rl] = (uint8_t)(s % g.strands); }
+        } else if (slot != RJ_CLAIMED_EMPTY) {
+            const uint32_t d = s_dp_base + slot;
+            dp.p_off[d] = s * g.stride; dp.p_len[d] = slen[s]; dp.t_off[d] = st_toff[i]; dp.t_len[d] = st_tlen[i]; dp_job[d] = s_base + i;
+        }
+    }
+    __syncthreads();
+    if (live) {
+        const unsigned long long key = s_key[threadIdx.x];
+        best_key[r] = key;
+        best_score[r] = key ? s_score[threadIdx.x] : INT_MIN;
+        best_pos[r] = key ? s_pos[threadIdx.x] : 0xFFFFFFFFu;
+        best_strand[r] = key ? s_strand[threadIdx.x] : (uint8_t)0;
     }
 }
 
-// Exact shortcut of the LOCAL extension (gapless_job_shortcut, pipeline_core.cuh): jobs whose result it proves get it here; the others
-// are compacted into the list the DP kernels run over.  (Earlier versions of the check: all band diagonals for every job 0.39 ms per
-// million reads, a symbol-by-symbol segment loop 0.29 ms, per-diagonal text reads 0.22 ms, four text words in registers 0.14 ms; with
-// the one-gap check 0.25 ms, which takes a third of the jobs off the DP.)  one_gap = false: the rule without it (nvb_debug_perfect_shortcut(2))
+// the DP's results back into the job list, and its aligned jobs into the best-per-read reduction
 __global__ void __launch_bounds__(256)
-pipe_perfect_jobs_kernel(const PipeGeom g, const int32_t match, const int32_t mismatch, const int32_t max_gap_open, const bool one_gap,
-                         const uint32_t* __restrict__ counts,
-                         const uint32_t* __restrict__ str_words, const uint32_t* __restrict__ genome,
-                         const uint32_t* __restrict__ jp_off, const uint32_t* __restrict__ jp_len,
-                         const uint32_t* __restrict__ jt_off, const uint32_t* __restrict__ jt_len,
-                         int32_t* __restrict__ job_score, uint2* __restrict__ job_sink,
-                         uint32_t* __restrict__ dp_p_off, uint32_t* __restrict__ dp_p_len, uint32_t* __restrict__ dp_t_off, uint32_t* __restrict__ dp_t_len,
-                         uint32_t* __restrict__ dp_job, uint32_t* __restrict__ dp_count)
-{
-    __shared__ uint32_t s_warp[8], s_base;
-    const uint32_t n = counts[2];
-    for (uint32_t base = blockIdx.x * 256; base < n; base += gridDim.x * 256) {       // (whole CTAs stay in the loop: barriers below)
-        const uint32_t j = base + threadIdx.x;
-        bool todo = false;
-        uint32_t po = 0, M = 0, to = 0, N = 0;
-        if (j < n) {
-            po = jp_off[j]; M = jp_len[j]; to = jt_off[j]; N = jt_len[j];
-            int32_t score = 0; uint32_t sx = 0, sy = 0;
-            if (gapless_job_shortcut(str_words, genome, po, M, to, N, g.band, match, mismatch, max_gap_open, score, sx, sy, one_gap)) {
-                job_score[j] = score; job_sink[j] = make_uint2(sx, sy);
-            } else todo = true;
-        }
-        // compaction of the others: one atomic per CTA (same-address atomics serialise, ~2.4 ns each on this part)
-        const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-        const uint32_t m = __ballot_sync(0xFFFFFFFFu, todo);
-        if (lane == 0) s_warp[warp] = (uint32_t)__popc(m);
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            uint32_t tot = 0;
-            for (int w = 0; w < 8; ++w) { const uint32_t c = s_warp[w]; s_warp[w] = tot; tot += c; }
-            s_base = tot ? atomicAdd(dp_count, tot) : 0u;
-        }
-        __syncthreads();
-        if (todo) {
-            const uint32_t slot = s_base + s_warp[warp] + __popc(m & ((1u << lane) - 1u));
-            dp_p_off[slot] = po; dp_p_len[slot] = M; dp_t_off[slot] = to; dp_t_len[slot] = N; dp_job[slot] = j;
-        }
-        __syncthreads();                                                           // s_warp / s_base are rewritten by the next round
-    }
-}
-__global__ void __launch_bounds__(256)
-pipe_scatter_dp_kernel(const uint32_t* __restrict__ dp_count, const uint32_t* __restrict__ dp_job, const int32_t* __restrict__ dp_score,
-                       const uint2* __restrict__ dp_sink, int32_t* __restrict__ job_score, uint2* __restrict__ job_sink)
+pipe_scatter_dp_kernel(const PipeGeom g, const uint32_t* __restrict__ dp_count, const uint32_t* __restrict__ dp_job,
+                       const int32_t* __restrict__ dp_score, const uint2* __restrict__ dp_sink,
+                       const uint32_t* __restrict__ j_string, const uint32_t* __restrict__ j_first,
+                       int32_t* __restrict__ job_score, uint2* __restrict__ job_sink, unsigned long long* __restrict__ best_key)
 {
     const uint32_t n = *dp_count;
     for (uint32_t a = blockIdx.x * 256 + threadIdx.x; a < n; a += gridDim.x * 256) {
         const uint32_t j = dp_job[a];
-        job_score[j] = dp_score[a]; job_sink[j] = dp_sink[a];
+        const int32_t sc = dp_score[a];
+        const uint2 sk = dp_sink[a];
+        job_score[j] = sc; job_sink[j] = sk;
+        if (job_aligned(sk)) atomicMax(best_key + j_string[j] / g.strands, make_best_key(sc, j_first[j]));
     }
 }
 
-// best job per read: max score, ties -> the job whose first hit comes first (the per-hit path's "smallest hit index")
+// a DP job whose key is its read's best key writes the read's result (first-hit indices are unique: at most one job of the read matches,
+// and none does when a claimed job won -- that one already wrote it)
 __global__ void __launch_bounds__(256)
-pipe_reduce_jobs_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, const uint32_t* __restrict__ j_string, const uint32_t* __restrict__ j_first,
-                        const int32_t* __restrict__ job_score, const uint2* __restrict__ job_sink, unsigned long long* __restrict__ best_key)
+pipe_finalize_dp_kernel(const PipeGeom g, const uint32_t* __restrict__ dp_count, const uint32_t* __restrict__ dp_job,
+                        const int32_t* __restrict__ dp_score, const uint2* __restrict__ dp_sink, const uint32_t* __restrict__ dp_t_off,
+                        const uint32_t* __restrict__ j_string, const uint32_t* __restrict__ j_first,
+                        const unsigned long long* __restrict__ best_key,
+                        int32_t* __restrict__ best_score, uint32_t* __restrict__ best_pos, uint8_t* __restrict__ best_strand)
 {
-    const uint32_t n = counts[2];
-    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
-        if (!job_aligned(job_sink[j])) continue;
-        const unsigned long long key = make_best_key(job_score[j], j_first[j]);
-        atomicMax(best_key + j_string[j] / g.strands, key);
-    }
-}
-
-__global__ void __launch_bounds__(256)
-pipe_init_best_kernel(const uint32_t n_reads, int32_t* __restrict__ best_score, uint32_t* __restrict__ best_pos, uint8_t* __restrict__ best_strand)
-{
-    const uint32_t r = blockIdx.x * 256 + threadIdx.x;
-    if (r >= n_reads) return;
-    best_score[r] = INT_MIN; best_pos[r] = 0xFFFFFFFFu; best_strand[r] = 0;
-}
-
-// the winning job of every read writes the read's result (first-hit indices are unique, so exactly one job matches the key)
-__global__ void __launch_bounds__(256)
-pipe_finalize_jobs_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, const uint32_t* __restrict__ j_string, const uint32_t* __restrict__ j_first,
-                          const uint32_t* __restrict__ jt_off, const int32_t* __restrict__ job_score, const uint2* __restrict__ job_sink,
-                          const unsigned long long* __restrict__ best_key,
-                          int32_t* __restrict__ best_score, uint32_t* __restrict__ best_pos, uint8_t* __restrict__ best_strand)
-{
-    const uint32_t n = counts[2];
-    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
-        const uint32_t s = j_string[j], read = s / g.strands;
-        const unsigned long long key = make_best_key(job_score[j], j_first[j]);
-        if (best_key[read] != key) continue;
-        best_score[read] = job_score[j]; best_pos[read] = jt_off[j] + job_sink[j].x; best_strand[read] = (uint8_t)(s % g.strands);
+    const uint32_t n = *dp_count;
+    for (uint32_t a = blockIdx.x * 256 + threadIdx.x; a < n; a += gridDim.x * 256) {
+        const uint32_t j = dp_job[a], s = j_string[j], read = s / g.strands;
+        const int32_t sc = dp_score[a];
+        if (best_key[read] != make_best_key(sc, j_first[j])) continue;
+        best_score[read] = sc; best_pos[read] = dp_t_off[a] + dp_sink[a].x; best_strand[read] = (uint8_t)(s % g.strands);
     }
 }
 
@@ -983,8 +1020,6 @@ static int g_pipe_path = 0;            // 1 = always the per-hit path, anything 
 static int size_only(int r) { return r == NVB_E_TEMP_SIZE ? NVB_OK : r; }     // a temp-size query's answer: its error, if any
 static int launched() { return (int)cudaGetLastError(); }                       // the launches' error, if any (cudaSuccess == NVB_OK)
 
-// alignment jobs: a read string (offset into the [fw, rc] stream, length) against a genome window (offset, length)
-struct Jobs { uint32_t *p_off, *p_len, *t_off, *t_len; };
 static Jobs take_jobs(TempCarver& tc, size_t n) { return Jobs{tc.take<uint32_t>(n), tc.take<uint32_t>(n), tc.take<uint32_t>(n), tc.take<uint32_t>(n)}; }
 struct JobViews { nvb_string_set pats, txts; };
 
@@ -992,14 +1027,16 @@ struct JobViews { nvb_string_set pats, txts; };
 struct PipeCall {
     PipeGeom g; cudaStream_t s; const nvb_seed_extend_params* P; FmIndex f; StrSet rd; const uint32_t* genome;
     uint32_t nq, hit_capacity;
-    bool dedup, per_read, eligible;                                         // eligible: the exact shortcut applies (pipe_perfect_jobs_kernel)
+    bool dedup, per_read, eligible;                                         // eligible: the exact shortcut applies (gapless_job_shortcut)
+    bool seed_split;                                                        // the located seed match in two passes (match_seeds)
     int32_t* best_score; uint32_t* best_pos; int32_t* hit_score; nvb_uint2* hit_sink;   // the caller's outputs (per-hit ones may be NULL)
     const nvb_best_alignment_out* BA; const nvb_pair_params* PP; const nvb_pair_out* PO;
     const nvb_mapq_params* MP; const nvb_mapq_out* MO; const nvb_pair_mapq_out* PMO;
     nvb_mapq_out se_mo;                                                     // paired MAPQ: the single-end stage's outputs (MO = &se_mo)
     StageEvents* SE;
     uint32_t *str_words, *str_len; uint8_t* str_quals;                      // [fw, rc] strings
-    uint2* ranges; uint32_t *sizes, *excl, *counts, *seed_todo_n;           // counts: [0] hits kept, [1] hits found, [2] alignment jobs
+    uint2* ranges; uint32_t *sizes, *excl, *counts, *seed_todo, *seed_todo_n;   // counts: [0] hits kept, [1] hits found, [2] alignment jobs
+    char* rj_tiles; size_t rj_tile_bytes;                                   // per-read path: tile states of the hit-slot look-back
     uint32_t *j_string, *j_first;                                           // per-read path: string and first hit of every job
     uint32_t *leader, *flag, *job_idx;                                      // per-hit path: job de-duplication
     Jobs jobs; int32_t* job_score; uint2* job_sink;                         // the distinct jobs (dedup_jobs)
@@ -1045,13 +1082,18 @@ struct PipeCall {
         str_words = tc.take<uint32_t>((size_t)g.n_strings * (g.stride / (32u / g.bits)) + 4);
         str_len   = tc.take<uint32_t>(g.n_strings);
         str_quals = P->d_read_quals ? tc.take<uint8_t>((size_t)g.n_strings * g.stride + 16) : nullptr;
-        ranges = tc.take<uint2>(nq); sizes = tc.take<uint32_t>(nq);
-        excl   = tc.take<uint32_t>((size_t)nq + (SEED_TODO_LISTS + 1u) * SEED_BLOCK * SEED_ITER);   // (+ slack: before the scan it holds the seed-match todo lists)
+        ranges = tc.take<uint2>(nq);
+        if (!per_read) { sizes = tc.take<uint32_t>(nq); excl = tc.take<uint32_t>(nq); }
+        if (seed_split) seed_todo = tc.take<uint32_t>((size_t)nq + (SEED_TODO_LISTS + 1u) * SEED_BLOCK * SEED_ITER);   // lists' capacity, see pipe_seed_match_kernel
         counts = tc.take<uint32_t>(4); seed_todo_n = tc.take<uint32_t>(SEED_TODO_LISTS * SEED_TODO_PITCH);
+        if (per_read) {
+            NVB_CUDA_TRY(RjTileState::AllocationSize((int)((n_reads + RJ_BLOCK - 1u) / RJ_BLOCK), rj_tile_bytes));
+            rj_tiles = tc.take<char>(rj_tile_bytes);
+        }
         if (per_read) { j_string = tc.take<uint32_t>(cap); j_first = tc.take<uint32_t>(cap); }
         else if (dedup) { leader = tc.take<uint32_t>(cap); flag = tc.take<uint32_t>(cap); job_idx = tc.take<uint32_t>(cap); }
         if (dedup) { jobs = take_jobs(tc, cap); job_score = tc.take<int32_t>(cap); job_sink = tc.take<uint2>(cap); }
-        if (eligible) {                                              // (whether or not nvb_debug_perfect_shortcut turned the shortcut off)
+        if (per_read) {                                              // the jobs the exact shortcut leaves to the DP (all of them when it is off)
             dp = take_jobs(tc, cap); dp_job = tc.take<uint32_t>(cap); dp_score = tc.take<int32_t>(cap); dp_sink = tc.take<uint2>(cap);
             dp_count = tc.take<uint32_t>(4);
         }
@@ -1059,7 +1101,8 @@ struct PipeCall {
         h_score = hit_score ? hit_score : (per_read ? nullptr : tc.take<int32_t>(cap));
         h_sink  = hit_sink ? (uint2*)hit_sink : (per_read ? nullptr : tc.take<uint2>(cap));
         best_key = tc.take<unsigned long long>(n_reads); rb_strand = tc.take<uint8_t>((size_t)n_reads + 16);
-        NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, sizes, excl, (int)nq, s));
+        scan_bytes = 0;
+        if (!per_read) NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, sizes, excl, (int)nq, s));
         if (dedup && !per_read && cap) {
             size_t scan2_bytes = 0;
             NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, scan2_bytes, flag, job_idx, (int)cap, s));
@@ -1121,20 +1164,20 @@ struct PipeCall {
     }
 
     // 2. seed ranges.  Per-read path + full suffix array: single-row ranges are located inside the match kernel; with a k-mer table in
-    // two passes, seeds on k-mers with >= 3 occurrences finished by a second kernel (lists in `excl`, which the hit-slot scan overwrites)
+    // two passes (seed_split), seeds on k-mers with >= 3 occurrences finished by a second kernel.  The per-read path stores no sizes
     int match_seeds() const
     {
         const uint32_t grid = (nq + SEED_BLOCK - 1) / SEED_BLOCK;
         const uint32_t* loc_genome = (per_read && f.sa_shift == 0u) ? genome : nullptr;
-        if (loc_genome && f.ktab_k && g.seed_len > f.ktab_k && g_seed_split) {
+        if (seed_split) {
             NVB_CUDA_TRY(cudaMemsetAsync(seed_todo_n, 0, SEED_TODO_LISTS * SEED_TODO_PITCH * sizeof(uint32_t), s));
             const uint32_t grid1 = (grid + SEED_ITER - 1u) / SEED_ITER;
-            if (g.bits == 2) pipe_seed_match_kernel<2, true><<<grid1, SEED_BLOCK, 0, s>>>(f, g, str_words, str_len, loc_genome, ranges, sizes, excl, seed_todo_n);
-            else             pipe_seed_match_kernel<4, true><<<grid1, SEED_BLOCK, 0, s>>>(f, g, str_words, str_len, loc_genome, ranges, sizes, excl, seed_todo_n);
+            if (g.bits == 2) pipe_seed_match_kernel<2, true><<<grid1, SEED_BLOCK, 0, s>>>(f, g, str_words, str_len, loc_genome, ranges, sizes, seed_todo, seed_todo_n);
+            else             pipe_seed_match_kernel<4, true><<<grid1, SEED_BLOCK, 0, s>>>(f, g, str_words, str_len, loc_genome, ranges, sizes, seed_todo, seed_todo_n);
             NVB_LAUNCH_CHECK();
             const uint32_t wgrid = (sm_count() * 16u + SEED_TODO_LISTS - 1u) / SEED_TODO_LISTS * SEED_TODO_LISTS;   // 16 resident CTAs per SM (H100: 2112), whole lists
-            if (g.bits == 2) pipe_seed_match_wide_kernel<2><<<wgrid, SEED_BLOCK, 0, s>>>(f, g, str_words, loc_genome, ranges, sizes, excl, seed_todo_n, grid1);
-            else             pipe_seed_match_wide_kernel<4><<<wgrid, SEED_BLOCK, 0, s>>>(f, g, str_words, loc_genome, ranges, sizes, excl, seed_todo_n, grid1);
+            if (g.bits == 2) pipe_seed_match_wide_kernel<2><<<wgrid, SEED_BLOCK, 0, s>>>(f, g, str_words, loc_genome, ranges, sizes, seed_todo, seed_todo_n, grid1);
+            else             pipe_seed_match_wide_kernel<4><<<wgrid, SEED_BLOCK, 0, s>>>(f, g, str_words, loc_genome, ranges, sizes, seed_todo, seed_todo_n, grid1);
         } else {
             if (g.bits == 2) pipe_seed_match_kernel<2, false><<<grid, SEED_BLOCK, 0, s>>>(f, g, str_words, str_len, loc_genome, ranges, sizes, nullptr, nullptr);
             else             pipe_seed_match_kernel<4, false><<<grid, SEED_BLOCK, 0, s>>>(f, g, str_words, str_len, loc_genome, ranges, sizes, nullptr, nullptr);
@@ -1142,43 +1185,36 @@ struct PipeCall {
         return launched();
     }
 
-    // 4'-6'. per-read path: locate, window and distinct jobs per read (stages 4 and 5), extension (6), the best job per read
+    // 4'-6'. per-read path: hit slots, locate, window, distinct jobs, exact shortcut and the claimed best per read in one kernel (stage 4),
+    // the DP over the jobs left to it and their scatter into the best per read (6), the DP winners' results (7)
     int extend_per_read() const
     {
         const nvb_gotoh_scheme& SC = P->scheme;
-        const uint32_t cap = hit_capacity, n_reads = g.n_reads, hgrid = (cap + 255) / 256;
-        NVB_CUDA_TRY(cudaMemsetAsync(counts + 2, 0, sizeof(uint32_t), s));
-        NVB_CUDA_TRY(cudaMemsetAsync(best_key, 0, sizeof(unsigned long long) * n_reads, s));
+        const uint32_t cap = hit_capacity, n_tiles = (g.n_reads + RJ_BLOCK - 1u) / RJ_BLOCK;
+        RjTileState tiles;
+        NVB_CUDA_TRY(tiles.Init((int)n_tiles, rj_tiles, rj_tile_bytes));
+        pipe_resolve_init_kernel<<<(n_tiles + 255u) / 256u, 256, 0, s>>>(tiles, n_tiles, counts, dp_count);
+        NVB_LAUNCH_CHECK();
+        const int shortcut = eligible ? g_perfect_shortcut : 0;
+        const int32_t max_gap_open = SC.pattern_gap_open > SC.text_gap_open ? SC.pattern_gap_open : SC.text_gap_open;
+        pipe_resolve_reads_kernel<<<n_tiles, RJ_BLOCK, 0, s>>>(f, g, ranges, str_len, cap, tiles, n_tiles, counts, shortcut, SC.match,
+                SC.mismatch, max_gap_open, str_words, genome, j_string, j_first, jobs, job_score, job_sink, dp, dp_job, dp_count,
+                best_key, best_score, best_pos, rb_strand);
+        NVB_LAUNCH_CHECK();
+        g_last_dp_count = dp_count;
+        NVB_TRY(stage(4)); NVB_TRY(stage(5));
+        // the DP list's length lives on the device: resident grids striding over it instead of hit_capacity / 256 mostly empty CTAs
+        const uint32_t hgrid = (cap + 255) / 256, jgrid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
         if (cap) {
-            pipe_read_jobs_kernel<<<(n_reads + RJ_BLOCK - 1) / RJ_BLOCK, RJ_BLOCK, 0, s>>>(f, g, ranges, sizes, excl, str_len, counts,
-                                                                                          j_string, j_first, jobs.p_off, jobs.p_len, jobs.t_off, jobs.t_len);
+            NVB_TRY(score_jobs(dp, dp_count, dp_score, dp_sink));
+            pipe_scatter_dp_kernel<<<jgrid, 256, 0, s>>>(g, dp_count, dp_job, dp_score, dp_sink, j_string, j_first, job_score, job_sink, best_key);
             NVB_LAUNCH_CHECK();
         }
-        NVB_TRY(stage(4)); NVB_TRY(stage(5));
-        if (cap && eligible && g_perfect_shortcut) {
-            const uint32_t jgrid = hgrid < sm_count() * 8u ? hgrid : sm_count() * 8u;
-            NVB_CUDA_TRY(cudaMemsetAsync(dp_count, 0, sizeof(uint32_t), s));
-            pipe_perfect_jobs_kernel<<<jgrid, 256, 0, s>>>(g, SC.match, SC.mismatch, SC.pattern_gap_open > SC.text_gap_open ? SC.pattern_gap_open : SC.text_gap_open,
-                                                           g_perfect_shortcut != 2, counts, str_words, genome,
-                                                           jobs.p_off, jobs.p_len, jobs.t_off, jobs.t_len, job_score, job_sink,
-                                                           dp.p_off, dp.p_len, dp.t_off, dp.t_len, dp_job, dp_count);
-            NVB_LAUNCH_CHECK();
-            g_last_dp_count = dp_count;
-            NVB_TRY(score_jobs(dp, dp_count, dp_score, dp_sink));
-            pipe_scatter_dp_kernel<<<jgrid, 256, 0, s>>>(dp_count, dp_job, dp_score, dp_sink, job_score, job_sink);
-            NVB_LAUNCH_CHECK();
-        } else if (cap)
-            NVB_TRY(score_jobs(jobs, counts + 2, job_score, job_sink));
         NVB_TRY(stage(6));
-        pipe_init_best_kernel<<<(n_reads + 255) / 256, 256, 0, s>>>(n_reads, best_score, best_pos, rb_strand);
-        NVB_LAUNCH_CHECK();
         if (cap) {
-            // the job count lives on the device: a resident grid striding over it instead of hit_capacity / 256 mostly empty CTAs
-            const uint32_t jgrid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
-            pipe_reduce_jobs_kernel<<<jgrid, 256, 0, s>>>(g, counts, j_string, j_first, job_score, job_sink, best_key);
+            pipe_finalize_dp_kernel<<<jgrid, 256, 0, s>>>(g, dp_count, dp_job, dp_score, dp_sink, dp.t_off, j_string, j_first, best_key,
+                                                          best_score, best_pos, rb_strand);
             NVB_LAUNCH_CHECK();
-            pipe_finalize_jobs_kernel<<<jgrid, 256, 0, s>>>(g, counts, j_string, j_first, jobs.t_off, job_score, job_sink, best_key,
-                                                            best_score, best_pos, rb_strand);
         }
         return launched();
     }
@@ -1424,6 +1460,7 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     const nvb_gotoh_scheme& SC = P->scheme;
     c.eligible = c.per_read && P->type == NVB_LOCAL && g.bits == 2 && P->band_len <= 32 && !SC.d_qual_table && SC.match > 0 && SC.mismatch < 0 &&
                  SC.pattern_gap_open < 0 && SC.pattern_gap_ext <= 0 && SC.text_gap_open < 0 && SC.text_gap_ext <= 0;
+    c.seed_split = c.per_read && c.f.sa_shift == 0u && c.f.ktab_k && g.seed_len > c.f.ktab_k && g_seed_split;
     size_t need = 0;
     NVB_TRY(c.carve(d_temp, need));
     if (!d_temp || *temp_bytes < need) { *temp_bytes = need; return NVB_E_TEMP_SIZE; }
@@ -1433,11 +1470,14 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     NVB_TRY(c.stage(0));
     NVB_TRY(c.make_strings()); NVB_TRY(c.stage(1));
     NVB_TRY(c.match_seeds());  NVB_TRY(c.stage(2));
-    // 3. hit slots: exclusive sum of the clamped range sizes
-    size_t scan_bytes = c.scan_bytes;
-    NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c.scan_tmp, scan_bytes, c.sizes, c.excl, (int)c.nq, s));
-    pipe_count_kernel<<<1, 32, 0, s>>>(c.excl, c.sizes, c.nq, hit_capacity, c.counts);
-    NVB_LAUNCH_CHECK(); NVB_TRY(c.stage(3));
+    // 3. per-hit path: hit slots, the exclusive sum of the clamped range sizes (the per-read path takes them inside its stage 4)
+    if (!c.per_read) {
+        size_t scan_bytes = c.scan_bytes;
+        NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c.scan_tmp, scan_bytes, c.sizes, c.excl, (int)c.nq, s));
+        pipe_count_kernel<<<1, 32, 0, s>>>(c.excl, c.sizes, c.nq, hit_capacity, c.counts);
+        NVB_LAUNCH_CHECK();
+    }
+    NVB_TRY(c.stage(3));
     NVB_TRY(c.per_read ? c.extend_per_read() : c.extend_per_hit());       // records stages 4 to 6
     if (hit_capacity && (d_hit_read || d_hit_window)) {
         pipe_export_hits_kernel<<<(hit_capacity + 255) / 256, 256, 0, s>>>(g, c.counts, c.hit_string, c.hits.t_off, c.hits.t_len, d_hit_read, (uint2*)d_hit_window);

@@ -74,7 +74,7 @@ __host__ __device__ __forceinline__ uint32_t text_window16(const uint32_t g0, co
 // (sink_inl.h:39-65).  A read without any difference (score m * M, only reachable in the last row) may tie with other equal diagonals
 // (tandem repeats): the largest one wins.
 // The job: read = 2-bit big-endian symbols [po, po + M) of str_words (po a multiple of 16), window = text[to, to + N), the seed's
-// diagonal band/2 into the window (pipe_read_jobs_kernel cuts it there; a window clamped at the text start, to == 0, has it somewhere
+// diagonal band/2 into the window (pipe_resolve_reads_kernel cuts it there; a window clamped at the text start, to == 0, has it somewhere
 // below and is left to the DP), band <= 32.  Returns true and (score, sink = (text end, pattern end), both 1-based ends as BestSink
 // reports them) when the result is proven; false = run the DP.  Only full windows qualify (N >= M + band - 1: no pad symbol in the band).
 __host__ __device__ inline bool gapless_job_shortcut(const uint32_t* __restrict__ str_words, const uint32_t* __restrict__ genome,

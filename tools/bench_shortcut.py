@@ -1,7 +1,7 @@
 """Extension split on bench.py's headline workload (1M x 150 bp reads, 1.9 Gbp genome, band 31 LOCAL, (2, -2, -5, -3)) with the exact
 shortcut's one-gap check on and off (nvb_debug_perfect_shortcut 1 / 2), alternating over the rounds in one process on the same index.
 Reports per rule the step and extension-stage times from device events, the jobs left to the DP per step (nvb_debug_dp_jobs), the
-per-kernel device time of the shortcut kernel, the banded DP kernels and the scatter from torch.profiler, and checks that the per-read
+per-kernel device time of the kernel that runs the shortcut (pipe_resolve_reads_kernel), the banded DP kernels, the scatter and the finalize from torch.profiler, and checks that the per-read
 results are identical.  Prints one JSON line with the card and its power limit.
 
     python tools/bench_shortcut.py [--rounds 3] [--steps 10] [--warmup 3]
@@ -21,7 +21,7 @@ if ROOT not in sys.path:
 import bench  # noqa: E402
 from tools.bench_mapq import power_limit_w  # noqa: E402
 
-KERNELS = ("pipe_perfect_jobs_kernel", "gotoh_pair_kernel", "gotoh_generic_kernel", "pipe_scatter_dp_kernel")
+KERNELS = ("pipe_resolve_reads_kernel", "gotoh_pair_kernel", "gotoh_generic_kernel", "pipe_scatter_dp_kernel", "pipe_finalize_dp_kernel")
 RULES = {"one_gap": 1, "gap_free": 2}
 
 
