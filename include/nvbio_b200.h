@@ -333,8 +333,9 @@ int nvb_gotoh_traceback(int type, const nvb_gotoh_scheme* scheme, const nvb_stri
 /* Banded Gotoh traceback (SURVEY 8f-4).  For i < n: score, sink (end cells) as nvb_banded_gotoh_score, plus the
  * source (start cells) and the alignment as the backtracer's pushes in END -> START order, one byte per op
  * (0 = SUBSTITUTION 'M', 1 = INSERTION 'I', 2 = DELETION 'D'; nvbio::aln::DirectionVector) at d_ops[i*max_ops ..];
- * d_n_ops[i] = number of ops (ops beyond max_ops are counted, not stored; max_ops >= pattern length + band_len always
- * suffices).  The soft clips the reference passes to Backtracer::clip are (pattern_len - sink.y) and source.y.
+ * d_n_ops[i] = number of ops (ops beyond max_ops are counted, not stored).  An alignment takes one op per pattern row (M or I)
+ * plus one per D, and its M and D ops consume at most pattern length + band_len - 1 text columns, so max_ops >= 2 * pattern length
+ * + band_len always suffices; pattern length + band_len does not when an alignment pairs insertions with deletions.  The soft clips the reference passes to Backtracer::clip are (pattern_len - sink.y) and source.y.
  * `patterns->length` must bound the pattern lengths (it sizes the per-alignment direction matrix in d_temp).
  * Replaces aln::banded_alignment_traceback<BAND_LEN,MAX_PATTERN_LEN,CHECKPOINTS> and
  * BatchedBandedAlignmentTraceback (nvbio/alignment/banded_inl.h:352-489, gotoh/gotoh_banded_inl.h:763-962,

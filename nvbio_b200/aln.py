@@ -128,7 +128,7 @@ def batch_banded_alignment_traceback(band_len: int, aligner: GotohAligner, patte
     n = patterns.count
     dev = patterns.words.device
     if max_ops is None:
-        max_ops = patterns.length + band_len + 1
+        max_ops = 2 * patterns.length + band_len           # every row (M / I) and every column (M / D) of the band: never truncated
     out = dict(score=torch.empty(n, dtype=torch.int32, device=dev), sink=torch.empty((n, 2), dtype=torch.int32, device=dev),
                source=torch.empty((n, 2), dtype=torch.int32, device=dev), ops=torch.zeros((n, max_ops), dtype=torch.uint8, device=dev),
                n_ops=torch.empty(n, dtype=torch.int32, device=dev))

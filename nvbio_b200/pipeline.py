@@ -120,7 +120,8 @@ class SeedExtendWorkspace:
             self.hit_sink = torch.empty((hit_capacity, 2), dtype=torch.int32, device=dev)
         # optional alignment (CIGAR ops, begin, strand) of every read's best hit
         self.best_ops = self.best_n_ops = self.best_begin = self.best_strand = None
-        self.max_ops = reads.length + params.band_len + 1
+        # an alignment's ops: one per read row (M or I) plus one per D, and M + D <= the window's length + band - 1 columns
+        self.max_ops = 2 * reads.length + params.band_len
         if traceback:
             self.best_ops = torch.zeros((n, self.max_ops), dtype=torch.uint8, device=dev)
             self.best_n_ops = torch.zeros(n, dtype=torch.int32, device=dev)
@@ -240,7 +241,7 @@ class PairedWorkspace:
             self.mate_mapq = torch.empty((2, n), dtype=torch.uint8, device=dev)
         # optional alignment of both mates (nvb_seed_extend_paired_traceback)
         self.mate_ops = self.mate_n_ops = self.mate_begin = None
-        self.max_ops = reads.length + params.band_len + 1 if max_ops is None else max_ops
+        self.max_ops = 2 * reads.length + params.band_len if max_ops is None else max_ops      # (as SeedExtendWorkspace)
         if traceback:
             self.mate_ops = torch.zeros((2, n, self.max_ops), dtype=torch.uint8, device=dev)
             self.mate_n_ops = torch.zeros((2, n), dtype=torch.int32, device=dev)
