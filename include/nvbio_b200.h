@@ -725,6 +725,34 @@ typedef struct nvb_bam_out {
 int nvb_bam_records(const nvb_bam_in* in, uint32_t n, const nvb_bam_out* out, void* d_temp, size_t* temp_bytes, void* stream);
 
 /* -------------------------------------------------------------------------------------------
+ * BGZF compression on the device (SAMv1 section 4.1; the framing of htslib's writer, contrib/htslib/bgzf.c:59 header and
+ * bgzf.c:216-240 deflate_block, htslib/bgzf.h:36-37 block sizes; nvBowtie compresses on the host, output_bam.cpp:581-601).
+ * Asynchronous on `stream`, no host round trip; NVB_E_TEMP_SIZE protocol.
+ *
+ * Input: n_bytes bytes at d_in, cut into blocks of exactly 0xFF00 bytes (BGZF_BLOCK_SIZE), the last one possibly shorter; n_blocks =
+ * ceil(n_bytes / 0xFF00).  Block i becomes member i, one gzip member (RFC 1952) with the BGZF extra field:
+ *   the 18-byte header 1f 8b 08 04 | 00 00 00 00 | 00 ff 06 00 | 'B' 'C' 02 00 | BSIZE = member length - 1 (little-endian);
+ *   one raw deflate block (RFC 1951) with BFINAL = 1: dynamic Huffman codes (LZ77 matches up to 258 bytes at distances up to 32768,
+ *   code lengths of at most 15 bits, 7 for the code-length code), or a stored block when the dynamic block would not be smaller;
+ *   CRC-32 of the block's input, then ISIZE = its length.
+ * So no member exceeds 18 + 5 + 65280 + 8 = 65,311 bytes, and each inflates to its block; the members concatenated are a BGZF stream
+ * without the 28-byte EOF block, which a file writer appends once.  The output depends only on the input bytes: not on the stream, the
+ * grid or timing.
+ *
+ * Output (nvb_bgzf_out): member i occupies bytes [d_block_offsets[i], d_block_offsets[i + 1]) of d_out; d_block_offsets[n_blocks] is the
+ * total.  d_block_offsets is always written whole; a member is stored only if it fits whole within `capacity` (d_out may be NULL when
+ * capacity is 0: a sizing call).  A capacity of 65,311 * n_blocks never truncates.
+ * NVB_E_INVALID (before any CUDA call) for a NULL out / temp_bytes / d_block_offsets, a NULL d_in with n_bytes > 0, a NULL d_out with
+ * capacity > 0, or n_blocks >= 2^32. */
+typedef struct nvb_bgzf_out {
+    uint8_t*  d_out;
+    uint64_t  capacity;
+    uint64_t* d_block_offsets;         /* [n_blocks + 1] */
+} nvb_bgzf_out;
+
+int nvb_bgzf_compress(const uint8_t* d_in, uint64_t n_bytes, const nvb_bgzf_out* out, void* d_temp, size_t* temp_bytes, void* stream);
+
+/* -------------------------------------------------------------------------------------------
  * Host-buffer entry point: batches of reads in HOST memory in, per-read results in HOST memory out.
  * Replaces nvBowtie's input thread -> compute thread hand-off and its per-stage cudaDeviceSynchronize
  * (nvBowtie/bowtie2/cuda/compute_thread.cu:213-243, nvBowtie/bowtie2/cuda/defs.h:64, aligner_best_approx.h:219-241):

@@ -58,6 +58,9 @@ int nvb_debug_dp_jobs(uint32_t* n);
 int nvb_debug_mapq_eval(const int32_t* d_best, const uint8_t* d_has_second, const int32_t* d_second, const uint32_t* d_len,
                         const int32_t* d_match_bonus, const int32_t* d_min_score, uint32_t n, uint8_t* d_mapq, void* stream);
 
+/* nvb_bgzf_compress: CTAs of the resident compression grid, 0 (default) = one per SM.  Same output at every grid size; for tests */
+void nvb_debug_bgzf_grid(uint32_t ctas);
+
 #ifdef __cplusplus
 }
 #endif

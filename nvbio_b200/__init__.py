@@ -11,3 +11,4 @@ from . import aln                                                               
 from .pipeline import SeedExtendParams, seed_extend, StreamingSeedExtend, PairParams, seed_extend_paired, MapqParams     # noqa: F401
 from .finish import finish_alignments, FinishedAlignments                        # noqa: F401
 from .bam import ContigTable, BamRecords, bam_records, bam_header, write_bam, numbered_names    # noqa: F401
+from .bgzf import BgzfBlocks, BgzfCall, bgzf_compress                           # noqa: F401

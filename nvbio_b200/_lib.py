@@ -15,13 +15,14 @@ EXPORTS = [
     "nvb_dict_rank", "nvb_dict_rank4", "nvb_dict_build_occ",
     "nvb_map_seeds", "nvb_fm_locate_init", "nvb_fm_locate_lookup", "nvb_fm_locate_sorted",
     "nvb_pipeline_create", "nvb_pipeline_submit", "nvb_pipeline_wait", "nvb_pipeline_traffic", "nvb_pipeline_destroy",
-    "nvb_finish_alignments", "nvb_bam_records",
+    "nvb_finish_alignments", "nvb_bam_records", "nvb_bgzf_compress",
 ]
 # test / tuning hooks of include/nvbio_b200_debug.h (not part of the drop-in ABI)
 DEBUG_EXPORTS = [
     "nvb_debug_gotoh_last_route", "nvb_debug_force_gotoh_path", "nvb_debug_full_minb", "nvb_debug_full_warp", "nvb_debug_full_traceback_warp",
     "nvb_debug_pair_format", "nvb_debug_pair_rows2", "nvb_debug_traceback_fast", "nvb_debug_pair_extra_smem",
     "nvb_debug_pipeline_path", "nvb_debug_seed_split", "nvb_debug_perfect_shortcut", "nvb_debug_dp_jobs", "nvb_debug_mapq_eval",
+    "nvb_debug_bgzf_grid",
 ]
 
 
@@ -72,6 +73,10 @@ class BamInStruct(C.Structure):           # nvb_bam_in
 
 class BamOutStruct(C.Structure):          # nvb_bam_out
     _fields_ = [("d_records", C.c_void_p), ("capacity", C.c_uint64), ("d_offsets", C.c_void_p), ("d_counts", C.c_void_p)]
+
+
+class BgzfOutStruct(C.Structure):         # nvb_bgzf_out
+    _fields_ = [("d_out", C.c_void_p), ("capacity", C.c_uint64), ("d_block_offsets", C.c_void_p)]
 
 
 class MapqParamsStruct(C.Structure):       # nvb_mapq_params

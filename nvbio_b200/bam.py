@@ -1,6 +1,7 @@
 """BAM output of traced and finished alignments (nvb_bam_records): the records are built on the device in the bam1_t wire layout of the
 SAM / BAM specification, with contig coordinates, the pair fields and TLEN; a small host-side writer frames them as a .bam file (BGZF
-blocks compressed with zlib).  The record rules are stated once, in include/nvbio_b200.h."""
+blocks compressed with zlib on the host, or members compressed on the device by nvbio_b200.bgzf).  The record rules are stated once,
+in include/nvbio_b200.h."""
 import ctypes as C
 import struct
 import zlib
@@ -206,7 +207,9 @@ def _bgzf_block(data: bytes) -> bytes:
 
 def write_bam(path: str, header: bytes, batches: Iterable) -> int:
     """write a .bam file: header (bam_header) then the records of every batch (BamRecords, or bytes), BGZF-framed on the host with zlib
-    (blocks of at most 64 KiB, then the 28-byte EOF block).  Raises if a batch did not store all its records.  Returns the bytes written."""
+    (blocks of at most 64 KiB, then the 28-byte EOF block).  A BgzfBlocks batch (bgzf_compress on the device) is written verbatim.  Raises
+    if a batch did not store all its records or members.  Returns the bytes written."""
+    from .bgzf import BgzfBlocks
     total = 0
     with open(path, "wb") as f:
         def emit(buf):
@@ -216,6 +219,12 @@ def write_bam(path: str, header: bytes, batches: Iterable) -> int:
                 f.write(blk); total += len(blk)
         emit(header)
         for b in batches:
+            if isinstance(b, BgzfBlocks):
+                if b.stored() != b.n_blocks:
+                    raise ValueError("write_bam: a batch stored %d of %d BGZF members (capacity too small)" % (b.stored(), b.n_blocks))
+                z = b.to_bytes()
+                f.write(z); total += len(z)
+                continue
             if isinstance(b, BamRecords):
                 if b.stored() != b.offsets.numel() - 1:
                     raise ValueError("write_bam: a batch stored %d of %d records (capacity too small)" % (b.stored(), b.offsets.numel() - 1))
