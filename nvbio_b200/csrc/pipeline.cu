@@ -591,8 +591,17 @@ pipe_best_jobs_kernel(const PipeGeom g, const unsigned long long* __restrict__ b
     if (strand) strand[r] = (uint8_t)(hit_string[h] % g.strands);
 }
 
-// per-read path: the best job of every read as its traceback job (pipe_best_jobs_kernel's output; the job count lives on the device).
-// pipe_empty_jobs_kernel first gives every read an empty job; the job whose key is the read's best key then writes its own
+// The alignments the extension scored, as every later stage reads them: the per-read path's distinct jobs (tie index: the job's first
+// hit) or the per-hit path's kept hits (tie == NULL: the hit itself).  Both paths see the same (score, strand, end, smallest tie index)
+// set, so what is derived from it does not depend on the path, the job order or the de-duplication.  The count lives on the device.
+struct Scored {
+    const uint32_t* count; const uint32_t* string; const uint32_t* tie_index; Jobs jobs; const int32_t* score; const uint2* sink;
+    __device__ __forceinline__ uint32_t tie(uint32_t j) const { return tie_index ? tie_index[j] : j; }
+    __device__ __forceinline__ uint32_t end(uint32_t j) const { return jobs.t_off[j] + sink[j].x; }
+};
+
+// per-read path: the best job of every read as its traceback job (pipe_best_jobs_kernel's output).  pipe_empty_jobs_kernel first gives
+// every read an empty job; pipe_winner_kernel then lets the best job write its own
 __global__ void __launch_bounds__(256)
 pipe_empty_jobs_kernel(const uint32_t n_reads, uint32_t* __restrict__ bp_off, uint32_t* __restrict__ bp_len, uint32_t* __restrict__ bt_off,
                        uint32_t* __restrict__ bt_len, uint8_t* __restrict__ strand)
@@ -602,19 +611,19 @@ pipe_empty_jobs_kernel(const uint32_t n_reads, uint32_t* __restrict__ bp_off, ui
     bp_off[r] = 0; bp_len[r] = 0; bt_off[r] = 0; bt_len[r] = 0;
     if (strand) strand[r] = 0;
 }
+
+// the candidate whose make_best_key is its read's key writes the read's job, end and strand (each skipped when NULL); tie indices are
+// unique, so at most one candidate of a read matches.  Resident grid striding over the device-side count
 __global__ void __launch_bounds__(256)
-pipe_read_best_jobs_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, const uint32_t* __restrict__ j_string,
-                           const uint32_t* __restrict__ j_first, const int32_t* __restrict__ job_score, const unsigned long long* __restrict__ best_key,
-                           const uint32_t* __restrict__ p_off, const uint32_t* __restrict__ p_len,
-                           const uint32_t* __restrict__ t_off, const uint32_t* __restrict__ t_len,
-                           uint32_t* __restrict__ bp_off, uint32_t* __restrict__ bp_len, uint32_t* __restrict__ bt_off, uint32_t* __restrict__ bt_len,
-                           uint8_t* __restrict__ strand)
+pipe_winner_kernel(const PipeGeom g, const Scored c, const unsigned long long* __restrict__ key, const Jobs out,
+                   uint32_t* __restrict__ end, uint8_t* __restrict__ strand)
 {
-    const uint32_t n = counts[2];
+    const uint32_t n = *c.count;
     for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
-        const uint32_t s = j_string[j], r = s / g.strands;
-        if (best_key[r] != make_best_key(job_score[j], j_first[j])) continue;
-        bp_off[r] = p_off[j]; bp_len[r] = p_len[j]; bt_off[r] = t_off[j]; bt_len[r] = t_len[j];
+        const uint32_t s = c.string[j], r = s / g.strands;
+        if (key[r] != make_best_key(c.score[j], c.tie(j))) continue;
+        if (out.p_off) { out.p_off[r] = c.jobs.p_off[j]; out.p_len[r] = c.jobs.p_len[j]; out.t_off[r] = c.jobs.t_off[j]; out.t_len[r] = c.jobs.t_len[j]; }
+        if (end) end[r] = c.end(j);
         if (strand) strand[r] = (uint8_t)(s % g.strands);
     }
 }
@@ -643,9 +652,7 @@ pipe_export_hits_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, c
 }
 
 // ---------------------------------------------------------------------------------------------
-// second-best distinct alignment and MAPQ (nvb_seed_extend_mapq).  The candidates are the scored alignments of a read: the per-read
-// path's distinct jobs (tie index: the job's first hit) or the per-hit path's kept hits (tie index: the hit).  Both paths see the
-// same (score, strand, end, smallest index) set, so the result does not depend on the path, the job order or the de-duplication.
+// second-best distinct alignment and MAPQ (nvb_seed_extend_mapq).  The candidates are the scored alignments of a read (Scored).
 // ---------------------------------------------------------------------------------------------
 
 // a candidate competes for the second-best alignment when it reaches the read's min score and is distinct from the best alignment
@@ -655,38 +662,18 @@ __device__ __forceinline__ bool second_candidate(int32_t score, uint32_t end, ui
     return score >= min_score[len] && distinct_alignment(end, strand, best_end, best_strand, len);
 }
 
-// best qualifying candidate per read (64-bit atomicMax of make_best_key); the count lives on the device: resident grid striding over it.
-// index == NULL: the candidate's own index is its tie index (per-hit path)
+// best qualifying candidate per read (64-bit atomicMax of make_best_key); resident grid striding over the device-side count
 __global__ void __launch_bounds__(256)
-pipe_second_reduce_kernel(const PipeGeom g, const uint32_t* __restrict__ count, const uint32_t* __restrict__ c_string,
-                          const uint32_t* __restrict__ index, const uint32_t* __restrict__ t_off, const int32_t* __restrict__ score,
-                          const uint2* __restrict__ sink, const uint32_t* __restrict__ str_len, const uint32_t* __restrict__ best_pos,
+pipe_second_reduce_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict__ str_len, const uint32_t* __restrict__ best_pos,
                           const uint8_t* __restrict__ best_strand, const int32_t* __restrict__ min_score,
                           unsigned long long* __restrict__ second_key)
 {
-    const uint32_t n = *count;
+    const uint32_t n = *c.count;
     for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
-        const uint32_t s = c_string[j], read = s / g.strands;
-        const int32_t sc = score[j];
-        const uint2 sk = sink[j];
-        if (job_aligned(sk) && second_candidate(sc, t_off[j] + sk.x, s % g.strands, str_len[s], best_pos[read], best_strand[read], min_score))
-            atomicMax(second_key + read, make_best_key(sc, index ? index[j] : j));
-    }
-}
-
-// the winning candidate of every read writes its end and strand (tie indices are unique, so exactly one candidate matches the key)
-__global__ void __launch_bounds__(256)
-pipe_second_finalize_kernel(const PipeGeom g, const uint32_t* __restrict__ count, const uint32_t* __restrict__ c_string,
-                            const uint32_t* __restrict__ index, const uint32_t* __restrict__ t_off, const int32_t* __restrict__ score,
-                            const uint2* __restrict__ sink, const unsigned long long* __restrict__ second_key,
-                            uint32_t* __restrict__ second_pos, uint8_t* __restrict__ second_strand)
-{
-    const uint32_t n = *count;
-    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
-        const uint32_t s = c_string[j], read = s / g.strands;
-        if (second_key[read] != make_best_key(score[j], index ? index[j] : j)) continue;
-        if (second_pos) second_pos[read] = t_off[j] + sink[j].x;
-        if (second_strand) second_strand[read] = (uint8_t)(s % g.strands);
+        const uint32_t s = c.string[j], read = s / g.strands;
+        const int32_t sc = c.score[j];
+        if (job_aligned(c.sink[j]) && second_candidate(sc, c.end(j), s % g.strands, str_len[s], best_pos[read], best_strand[read], min_score))
+            atomicMax(second_key + read, make_best_key(sc, c.tie(j)));
     }
 }
 
@@ -801,6 +788,21 @@ pair_compact_kernel(const PipeGeom g, const uint32_t n_slots, const uint32_t cap
     jp_off[j] = w_pstr[i] * g.stride; jp_len[j] = str_len[w_pstr[i]]; jt_off[j] = w_toff[i]; jt_len[j] = w_tlen[i];
 }
 
+// slot i = 2p + a (anchor a of pair p): whether its opposite-mate job was run (within the rescue capacity) and reached min_mate_score;
+// if so, the rescued alignment's score and end
+__device__ __forceinline__ bool usable_rescue(const nvb_pair_params& pp, const uint32_t* __restrict__ want, const uint32_t* __restrict__ job_idx,
+                                              const uint32_t* __restrict__ w_toff, const int32_t* __restrict__ rs_score,
+                                              const uint2* __restrict__ rs_sink, uint32_t i, int32_t& score, uint32_t& end)
+{
+    if (!want[i]) return false;
+    const uint32_t j = job_idx[i];
+    if (j >= pp.rescue_capacity) return false;
+    score = rs_score[j];
+    if (score < pp.min_mate_score) return false;
+    end = w_toff[i] + rs_sink[j].x;
+    return true;
+}
+
 __global__ void __launch_bounds__(256)
 pair_finalize_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const uint32_t* __restrict__ want, const uint32_t* __restrict__ job_idx,
                      const uint32_t* __restrict__ w_toff, const int32_t* __restrict__ rs_score, const uint2* __restrict__ rs_sink,
@@ -812,14 +814,10 @@ pair_finalize_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const uin
     int best_a = -1; int32_t best_sum = INT_MIN, best_rs = 0; uint32_t best_pos = 0;
 #pragma unroll
     for (int a = 0; a < 2; ++a) {
-        const uint32_t i = 2 * p + a;
-        if (!want[i]) continue;
-        const uint32_t j = job_idx[i];
-        if (j >= pp.rescue_capacity) continue;
-        const int32_t rs = rs_score[j];
-        if (rs < pp.min_mate_score) continue;
+        int32_t rs; uint32_t end;
+        if (!usable_rescue(pp, want, job_idx, w_toff, rs_score, rs_sink, 2 * p + a, rs, end)) continue;
         const int32_t sum = mate_score[a * n_pairs + p] + rs;
-        if (sum > best_sum) { best_sum = sum; best_a = a; best_rs = rs; best_pos = w_toff[i] + rs_sink[j].x; }
+        if (sum > best_sum) { best_sum = sum; best_a = a; best_rs = rs; best_pos = end; }
     }
     if (best_a < 0) return;
     const int o = 1 - best_a;
@@ -876,18 +874,17 @@ pair_rescue_items_kernel(const uint32_t n_pairs, const uint32_t* __restrict__ pa
 
 // candidates per read (counts) or their place in the read's segment (seg != NULL: cursor = counts zeroed, key = (strand << 32) | end)
 __global__ void __launch_bounds__(256)
-pair_cand_scatter_kernel(const PipeGeom g, const uint32_t* __restrict__ count, const uint32_t* __restrict__ c_string,
-                         const uint32_t* __restrict__ t_off, const int32_t* __restrict__ score, const uint2* __restrict__ sink,
-                         const uint32_t* __restrict__ str_len, const int32_t* __restrict__ min_score, const uint32_t* __restrict__ seg,
-                         uint32_t* __restrict__ cursor, unsigned long long* __restrict__ key, uint32_t* __restrict__ val)
+pair_cand_scatter_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict__ str_len, const int32_t* __restrict__ min_score,
+                         const uint32_t* __restrict__ seg, uint32_t* __restrict__ cursor, unsigned long long* __restrict__ key,
+                         uint32_t* __restrict__ val)
 {
-    const uint32_t n = *count;
+    const uint32_t n = *c.count;
     for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
-        const uint32_t s = c_string[j], read = s / g.strands;
-        if (!job_aligned(sink[j]) || score[j] < min_score[str_len[s]]) continue;
+        const uint32_t s = c.string[j], read = s / g.strands;
+        if (!job_aligned(c.sink[j]) || c.score[j] < min_score[str_len[s]]) continue;
         const uint32_t slot = atomicAdd(cursor + read, 1u);
         if (!seg) continue;
-        key[seg[read] + slot] = ((unsigned long long)(s % g.strands) << 32) | (t_off[j] + sink[j].x);
+        key[seg[read] + slot] = ((unsigned long long)(s % g.strands) << 32) | c.end(j);
         val[seg[read] + slot] = j;
     }
 }
@@ -896,8 +893,8 @@ pair_cand_scatter_kernel(const PipeGeom g, const uint32_t* __restrict__ count, c
 // / m_tie from the segment's start; n_fw / n_merged = forward / all merged candidates
 __global__ void __launch_bounds__(256)
 pair_cand_merge_kernel(const uint32_t n_reads, const uint32_t* __restrict__ seg, const uint32_t* __restrict__ cnt,
-                       const unsigned long long* __restrict__ key, const uint32_t* __restrict__ val, const uint32_t* __restrict__ index,
-                       const int32_t* __restrict__ score, uint32_t* __restrict__ m_end, int32_t* __restrict__ m_score, uint32_t* __restrict__ m_tie,
+                       const unsigned long long* __restrict__ key, const uint32_t* __restrict__ val, const Scored c,
+                       uint32_t* __restrict__ m_end, int32_t* __restrict__ m_score, uint32_t* __restrict__ m_tie,
                        uint32_t* __restrict__ n_fw, uint32_t* __restrict__ n_merged)
 {
     const uint32_t r = blockIdx.x * 256 + threadIdx.x;
@@ -906,8 +903,8 @@ pair_cand_merge_kernel(const uint32_t n_reads, const uint32_t* __restrict__ seg,
     uint32_t m = 0, fw = 0; unsigned long long prev = ~0ull;
     for (uint32_t k = b; k < b + n; ++k) {
         const unsigned long long kk = key[k];
-        const uint32_t j = val[k], tie = index ? index[j] : j;
-        const int32_t sc = score[j];
+        const uint32_t j = val[k], tie = c.tie(j);
+        const int32_t sc = c.score[j];
         if (kk == prev) {
             const uint32_t o = b + m - 1u;
             if (sc > m_score[o] || (sc == m_score[o] && tie < m_tie[o])) { m_score[o] = sc; m_tie[o] = tie; }
@@ -952,14 +949,11 @@ pair_second_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const nvb_m
         pair_combinations(m, pp.min_frag, pp.max_frag, ps);
         // rescues: the anchor's single-end best with the rescued alignment of the other mate (tie index 0xFFFFFFFF)
         for (int a = 0; a < 2; ++a) {
-            const uint32_t i = 2u * p + a, ra = a ? r1 : r0;
-            if (!want[i]) continue;
-            const uint32_t j = job_idx[i];
-            if (j >= pp.rescue_capacity) continue;
-            const int32_t rs = rs_score[j];
-            if (rs < pp.min_mate_score || rs < mp.d_min_score[len[1 - a]]) continue;
+            const uint32_t ra = a ? r1 : r0;
+            int32_t rs; uint32_t end;
+            if (!usable_rescue(pp, want, job_idx, w_toff, rs_score, rs_sink, 2u * p + a, rs, end) || rs < mp.d_min_score[len[1 - a]]) continue;
             const unsigned long long key = best_key[ra];
-            ps.offer_rescue(a, best_key_score(key) + rs, se_pos[ra], se_strand[ra], best_key_index(key), w_toff[i] + rs_sink[j].x);
+            ps.offer_rescue(a, best_key_score(key) + rs, se_pos[ra], se_strand[ra], best_key_index(key), end);
         }
         const uint8_t q = (uint8_t)bowtie_mapq2(pair_score[p], ps.has, ps.score, (int32_t)(len[0] + len[1]) * mp.match_bonus,
                                                 mp.d_min_score[len[0]] + mp.d_min_score[len[1]], mp.match_bonus == 0);
@@ -1019,6 +1013,10 @@ static int g_pipe_path = 0;            // 1 = always the per-hit path, anything 
 #define NVB_TRY(expr) do { const int _r = (expr); if (_r != NVB_OK) return _r; } while (0)
 static int size_only(int r) { return r == NVB_E_TEMP_SIZE ? NVB_OK : r; }     // a temp-size query's answer: its error, if any
 static int launched() { return (int)cudaGetLastError(); }                       // the launches' error, if any (cudaSuccess == NVB_OK)
+
+// a list whose length (<= n) lives on the device: a resident grid of 256-thread CTAs striding over it (16 per SM) instead of n / 256
+// mostly empty CTAs
+static uint32_t resident_grid(uint32_t n) { const uint32_t grid = (n + 255) / 256, cap = sm_count() * 16u; return grid < cap ? grid : cap; }
 
 static Jobs take_jobs(TempCarver& tc, size_t n) { return Jobs{tc.take<uint32_t>(n), tc.take<uint32_t>(n), tc.take<uint32_t>(n), tc.take<uint32_t>(n)}; }
 struct JobViews { nvb_string_set pats, txts; };
@@ -1203,8 +1201,7 @@ struct PipeCall {
         NVB_LAUNCH_CHECK();
         g_last_dp_count = dp_count;
         NVB_TRY(stage(4)); NVB_TRY(stage(5));
-        // the DP list's length lives on the device: resident grids striding over it instead of hit_capacity / 256 mostly empty CTAs
-        const uint32_t hgrid = (cap + 255) / 256, jgrid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
+        const uint32_t jgrid = resident_grid(cap);
         if (cap) {
             NVB_TRY(score_jobs(dp, dp_count, dp_score, dp_sink));
             pipe_scatter_dp_kernel<<<jgrid, 256, 0, s>>>(g, dp_count, dp_job, dp_score, dp_sink, j_string, j_first, job_score, job_sink, best_key);
@@ -1268,10 +1265,9 @@ struct PipeCall {
         if (per_read) {
             pipe_empty_jobs_kernel<<<rgrid, 256, 0, s>>>(g.n_reads, best.p_off, best.p_len, best.t_off, best.t_len, BA->d_strand);
             NVB_LAUNCH_CHECK();
-            const uint32_t hgrid = (hit_capacity + 255) / 256, jgrid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
+            const uint32_t jgrid = resident_grid(hit_capacity);
             if (jgrid) {
-                pipe_read_best_jobs_kernel<<<jgrid, 256, 0, s>>>(g, counts, j_string, j_first, job_score, best_key, jobs.p_off, jobs.p_len,
-                                                                 jobs.t_off, jobs.t_len, best.p_off, best.p_len, best.t_off, best.t_len, BA->d_strand);
+                pipe_winner_kernel<<<jgrid, 256, 0, s>>>(g, scored(), best_key, best, nullptr, BA->d_strand);
                 NVB_LAUNCH_CHECK();
             }
         } else {
@@ -1292,24 +1288,22 @@ struct PipeCall {
         return launched();
     }
 
-    // second-best distinct alignment and MAPQ of every read: one more pass over the candidates the extension scored (the per-read path's
-    // jobs, tie index = their first hit; the per-hit path's kept hits), after the best alignment is known
+    // the alignments the extension scored: the per-read path's distinct jobs, the per-hit path's kept hits
+    Scored scored() const
+    {
+        return per_read ? Scored{counts + 2, j_string, j_first, jobs, job_score, job_sink} : Scored{counts, hit_string, nullptr, hits, h_score, h_sink};
+    }
+
+    // second-best distinct alignment and MAPQ of every read: one more pass over the scored alignments, after the best alignment is known
     int second_best() const
     {
-        const uint32_t cap = hit_capacity, hgrid = (cap + 255) / 256;
         NVB_CUDA_TRY(cudaMemsetAsync(second_key, 0, sizeof(unsigned long long) * g.n_reads, s));
-        if (cap) {
-            const uint32_t* n   = per_read ? counts + 2 : counts;
-            const uint32_t* cs  = per_read ? j_string : hit_string;
-            const uint32_t* idx = per_read ? j_first : nullptr;
-            const uint32_t* to  = per_read ? jobs.t_off : hits.t_off;
-            const int32_t* sc   = per_read ? job_score : h_score;
-            const uint2* sk     = per_read ? job_sink : h_sink;
-            const uint32_t grid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
-            pipe_second_reduce_kernel<<<grid, 256, 0, s>>>(g, n, cs, idx, to, sc, sk, str_len, best_pos, rb_strand, MP->d_min_score, second_key);
+        if (hit_capacity) {
+            const uint32_t grid = resident_grid(hit_capacity);
+            pipe_second_reduce_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, best_pos, rb_strand, MP->d_min_score, second_key);
             NVB_LAUNCH_CHECK();
             if (MO->d_second_pos || MO->d_second_strand) {
-                pipe_second_finalize_kernel<<<grid, 256, 0, s>>>(g, n, cs, idx, to, sc, sk, second_key, MO->d_second_pos, MO->d_second_strand);
+                pipe_winner_kernel<<<grid, 256, 0, s>>>(g, scored(), second_key, Jobs{}, MO->d_second_pos, MO->d_second_strand);
                 NVB_LAUNCH_CHECK();
             }
         }
@@ -1326,26 +1320,21 @@ struct PipeCall {
         NVB_CUDA_TRY(cudaMemcpyAsync(se_pos, best_pos, sizeof(uint32_t) * n_reads, cudaMemcpyDeviceToDevice, s));
         NVB_CUDA_TRY(cudaMemsetAsync(pc_cnt, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
         if (cap) {
-            const uint32_t* n  = per_read ? counts + 2 : counts;
-            const uint32_t* cs = per_read ? j_string : hit_string;
-            const uint32_t* to = per_read ? jobs.t_off : hits.t_off;
-            const int32_t* sc  = per_read ? job_score : h_score;
-            const uint2* sk    = per_read ? job_sink : h_sink;
-            const uint32_t hgrid = (cap + 255) / 256, grid = hgrid < sm_count() * 16u ? hgrid : sm_count() * 16u;
-            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, n, cs, to, sc, sk, str_len, MP->d_min_score, nullptr, pc_cnt, nullptr, nullptr);
+            const uint32_t grid = resident_grid(cap);
+            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, nullptr, pc_cnt, nullptr, nullptr);
             NVB_LAUNCH_CHECK();
             size_t bytes = pc_scan_bytes;
             NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(pc_scan_tmp, bytes, pc_cnt, pc_seg, (int)n_reads + 1, s));
             NVB_CUDA_TRY(cudaMemsetAsync(pc_cnt, 0, sizeof(uint32_t) * n_reads, s));
-            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, n, cs, to, sc, sk, str_len, MP->d_min_score, pc_seg, pc_cnt, pc_key[0], pc_val[0]);
+            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, pc_seg, pc_cnt, pc_key[0], pc_val[0]);
             NVB_LAUNCH_CHECK();
             bytes = pc_sort_bytes;
             NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairs(pc_sort_tmp, bytes, pc_key[0], pc_key[1], pc_val[0], pc_val[1], (int)cap, (int)n_reads,
                                                              pc_seg, pc_seg + 1, s));
         } else
             NVB_CUDA_TRY(cudaMemsetAsync(pc_seg, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
-        pair_cand_merge_kernel<<<(n_reads + 255) / 256, 256, 0, s>>>(n_reads, pc_seg, pc_cnt, pc_key[1], pc_val[1], per_read ? j_first : nullptr,
-                                                                      per_read ? job_score : h_score, pc_end, pc_score, pc_tie, pc_fw, pc_n);
+        pair_cand_merge_kernel<<<(n_reads + 255) / 256, 256, 0, s>>>(n_reads, pc_seg, pc_cnt, pc_key[1], pc_val[1], scored(), pc_end, pc_score,
+                                                                      pc_tie, pc_fw, pc_n);
         return launched();
     }
 
@@ -1419,12 +1408,21 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     const nvb_mapq_params* MP, const nvb_mapq_out* MO, const nvb_pair_mapq_out* PMO,
                     void* d_temp, size_t* temp_bytes, void* stream)
 {
+    // The entry points check only what cannot be seen here: that the structs they require are there, and the pair count before
+    // 2 * n_pairs is formed.  The order below decides which code a call with several faults gets: the paired traceback's read length
+    // limit comes after the outputs and MAPQ inputs and before everything else.
+    if (!reads || !temp_bytes) return NVB_E_INVALID;
+    if (BA && (!BA->d_ops || !BA->d_n_ops || !BA->d_begin || BA->max_ops == 0)) return NVB_E_INVALID;
+    if ((MP == nullptr) != (MO == nullptr && PMO == nullptr)) return NVB_E_INVALID;
+    if (MP && (!MP->d_min_score || MP->max_read_len < reads->length)) return NVB_E_INVALID;   // the min-score table must cover every read length
+    if (MO && (!MO->d_second_score || !MO->d_mapq)) return NVB_E_INVALID;
+    if (PMO && (!PMO->d_second_pair_score || !PMO->d_mate_mapq)) return NVB_E_INVALID;
+    if (PP && BA && reads->length > FULL_TB_MAX_M) return NVB_E_UNSUPPORTED;                 // nvBowtie's MAXIMUM_READ_LENGTH
     if (PP) {
-        if (!PO || !PO->d_pair_score || !PO->d_pair_flags || !PO->d_mate_score || !PO->d_mate_pos || !PO->d_mate_strand) return NVB_E_INVALID;
+        if (!PO->d_pair_score || !PO->d_pair_flags || !PO->d_mate_score || !PO->d_mate_pos || !PO->d_mate_strand) return NVB_E_INVALID;
         if (!P || !P->both_strands || (n_reads & 1u) || PP->max_frag == 0 || PP->min_frag > PP->max_frag) return NVB_E_INVALID;
     }
-    if (BA && (!BA->d_ops || !BA->d_n_ops || !BA->d_begin || BA->max_ops == 0)) return NVB_E_INVALID;
-    if (!valid_fmindex(fmi) || !fmi->d_ssa || !d_genome || !valid_strset(reads) || !P || !temp_bytes) return NVB_E_INVALID;
+    if (!valid_fmindex(fmi) || !fmi->d_ssa || !d_genome || !valid_strset(reads) || !P) return NVB_E_INVALID;
     if (reads->bits == 8) return NVB_E_UNSUPPORTED;
     if (P->seed_len == 0 || P->seed_interval == 0 || P->max_seed_hits == 0) return NVB_E_INVALID;
     if (n_reads && (!d_best_score || !d_best_pos)) return NVB_E_INVALID;
@@ -1539,7 +1537,7 @@ extern "C" int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d
                     const nvb_pair_params* pair_params, const nvb_pair_out* out,
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream)
 {
-    if (!pair_params || !out || n_pairs > 0x3FFFFFFFu || !temp_bytes) return NVB_E_INVALID;
+    if (!pair_params || !out || n_pairs > 0x3FFFFFFFu) return NVB_E_INVALID;
     // the per-read best (score, end) of the single-end stage lands in the mate arrays first and is then refined per pair
     return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
                             nullptr, nullptr, nullptr, pair_params, out, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
@@ -1555,8 +1553,7 @@ extern "C" int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_g
                     const nvb_mapq_params* mapq, const nvb_mapq_out* mapq_out,
                     void* d_temp, size_t* temp_bytes, void* stream)
 {
-    if (!mapq || !mapq_out || !mapq->d_min_score || !mapq_out->d_second_score || !mapq_out->d_mapq) return NVB_E_INVALID;
-    if (!reads || mapq->max_read_len < reads->length) return NVB_E_INVALID;           // the min-score table must cover every read length
+    if (!mapq || !mapq_out) return NVB_E_INVALID;
     return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
                             d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, mapq, mapq_out, nullptr, d_temp, temp_bytes, stream);
 }
@@ -1568,9 +1565,7 @@ extern "C" int nvb_seed_extend_paired_mapq(const nvb_fm_index* fmi, const uint32
                     const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream)
 {
-    if (!pair_params || !out || n_pairs > 0x3FFFFFFFu || !temp_bytes) return NVB_E_INVALID;
-    if (!mapq || !mapq_out || !mapq->d_min_score || !mapq_out->d_second_pair_score || !mapq_out->d_mate_mapq) return NVB_E_INVALID;
-    if (!reads || mapq->max_read_len < reads->length) return NVB_E_INVALID;           // the min-score table must cover every read length
+    if (!pair_params || !out || !mapq || !mapq_out || n_pairs > 0x3FFFFFFFu) return NVB_E_INVALID;
     return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
                             nullptr, nullptr, nullptr, pair_params, out, mapq, nullptr, mapq_out, d_temp, temp_bytes, stream);
 }
@@ -1583,17 +1578,9 @@ extern "C" int nvb_seed_extend_paired_traceback(const nvb_fm_index* fmi, const u
                     const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream)
 {
-    if (!pair_params || !out || n_pairs > 0x3FFFFFFFu || !temp_bytes || !reads) return NVB_E_INVALID;
-    const nvb_best_alignment_out* BA = mate_alignment;
-    if (!BA || !BA->d_ops || !BA->d_n_ops || !BA->d_begin || BA->max_ops == 0) return NVB_E_INVALID;
-    if ((mapq == nullptr) != (mapq_out == nullptr)) return NVB_E_INVALID;
-    if (mapq) {
-        if (!mapq->d_min_score || !mapq_out->d_second_pair_score || !mapq_out->d_mate_mapq) return NVB_E_INVALID;
-        if (mapq->max_read_len < reads->length) return NVB_E_INVALID;
-    }
-    if (reads->length > FULL_TB_MAX_M) return NVB_E_UNSUPPORTED;       // nvBowtie's MAXIMUM_READ_LENGTH
+    if (!pair_params || !out || !mate_alignment || n_pairs > 0x3FFFFFFFu) return NVB_E_INVALID;
     return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
-                            nullptr, nullptr, BA, pair_params, out, mapq, nullptr, mapq_out, d_temp, temp_bytes, stream);
+                            nullptr, nullptr, mate_alignment, pair_params, out, mapq, nullptr, mapq_out, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_debug_mapq_eval(const int32_t* d_best, const uint8_t* d_has_second, const int32_t* d_second, const uint32_t* d_len,

@@ -48,10 +48,12 @@ def test_argument_validation_without_gpu():
 
 
 def test_argument_validation_of_the_widened_api():
-    """full-matrix score / traceback, windowed score and the paired-end composition reject bad arguments with NVB_E_INVALID (-1) or
-    NVB_E_UNSUPPORTED (-4) before any CUDA call; size queries answer NVB_E_TEMP_SIZE (-2) without touching the device"""
+    """full-matrix score / traceback, windowed score, the seed + extend traceback and the paired-end composition reject bad arguments
+    with NVB_E_INVALID (-1) or NVB_E_UNSUPPORTED (-4) before any CUDA call; size queries answer NVB_E_TEMP_SIZE (-2) without touching the
+    device"""
     from nvbio_b200 import _lib
-    from nvbio_b200._lib import StringSetStruct, GotohSchemeStruct, PairParamsStruct, PairOutStruct, SeedExtendParamsStruct, FmIndexStruct
+    from nvbio_b200._lib import (StringSetStruct, GotohSchemeStruct, PairParamsStruct, PairOutStruct, SeedExtendParamsStruct, FmIndexStruct,
+                                 BestAlignmentOutStruct)
     L = _lib.lib()
     tb = C.c_size_t(0)
     ss = StringSetStruct(); ss.d_words = 16; ss.bits = 2; ss.big_endian = 1; ss.stride = 160; ss.length = 150
@@ -92,6 +94,35 @@ def test_argument_validation_of_the_widened_api():
     pp.min_frag = 600
     assert L.nvb_seed_extend_paired(C.byref(fm), C.c_void_p(16), C.byref(ss), C.c_uint32(8), C.byref(sp), C.c_uint32(100), C.byref(pp), C.byref(po),
                                     None, None, C.byref(tb), None) == -1
+    pp.min_frag = 0
+    # 8-bit reads are NVB_E_UNSUPPORTED (-4); a failed check of the pair arguments, outputs or parameters wins over it
+    s8 = StringSetStruct(); s8.d_words = 16; s8.bits = 8; s8.big_endian = 1; s8.stride = 152; s8.length = 150
+    r = lambda x: C.byref(x) if x is not None else None      # noqa: E731
+
+    def paired(reads=s8, pp_=pp, po_=po, temp_bytes=tb, n_pairs=8):
+        return L.nvb_seed_extend_paired(C.byref(fm), C.c_void_p(16), r(reads), C.c_uint32(n_pairs), C.byref(sp), C.c_uint32(100), r(pp_), r(po_),
+                                        None, None, r(temp_bytes), None)
+    assert paired() == -4
+    assert paired(pp_=None) == -1 and paired(po_=None) == -1 and paired(temp_bytes=None) == -1 and paired(n_pairs=0x40000000) == -1
+    assert paired(reads=None) == -1 and paired(reads=ss, temp_bytes=None) == -1 and paired(reads=ss, n_pairs=0x40000000) == -1
+    po.d_mate_pos = None
+    assert paired() == -1
+    po.d_mate_pos = 16
+    pp.max_frag = 0
+    assert paired() == -1
+    pp.max_frag = 500
+
+    # single-end traceback: NULL or incomplete best_alignment (-1), also with 8-bit reads
+    def traceback(ba, reads=s8):
+        return L.nvb_seed_extend_traceback(C.byref(fm), C.c_void_p(16), r(reads), C.c_uint32(8), C.byref(sp), C.c_uint32(100), C.c_void_p(16),
+                                           C.c_void_p(16), None, None, None, None, None, r(ba), None, C.byref(tb), None)
+    assert traceback(None) == -1 and traceback(None, reads=ss) == -1
+    for k in ("d_ops", "d_n_ops", "d_begin", "max_ops"):
+        ba = BestAlignmentOutStruct(); ba.d_ops = 16; ba.max_ops = 300; ba.d_n_ops = 16; ba.d_begin = 16
+        setattr(ba, k, None if k != "max_ops" else 0)
+        assert traceback(ba) == -1 and traceback(ba, reads=ss) == -1, k
+    ba = BestAlignmentOutStruct(); ba.d_ops = 16; ba.max_ops = 300; ba.d_n_ops = 16; ba.d_begin = 16
+    assert traceback(ba) == -4 and traceback(ba, reads=None) == -1
 
 
 def test_no_oracle_in_product():

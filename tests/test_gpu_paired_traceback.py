@@ -325,10 +325,10 @@ def test_argument_validation_without_gpu():
     mp = MapqParamsStruct(); mp.d_min_score = 16; mp.max_read_len = 150; mp.match_bonus = 2
     mo = PairMapqOutStruct(); mo.d_second_pair_score = 16; mo.d_mate_mapq = 16
 
-    def call(ba_=ba, mp_=mp, mo_=mo, ss_=ss, sp_=sp, po_=po):
-        return f(C.byref(fm), C.c_void_p(16), C.byref(ss_), C.c_uint32(8), C.byref(sp_), C.c_uint32(100), C.byref(pp), C.byref(po_),
-                 C.byref(ba_) if ba_ is not None else None, C.byref(mp_) if mp_ is not None else None,
-                 C.byref(mo_) if mo_ is not None else None, None, None, C.byref(tb), None)
+    def call(ba_=ba, mp_=mp, mo_=mo, ss_=ss, sp_=sp, po_=po, pp_=pp, fm_=fm, genome=16, tb_=tb, n_pairs=8):
+        r = lambda x: C.byref(x) if x is not None else None      # noqa: E731
+        return f(r(fm_), C.c_void_p(genome), r(ss_), C.c_uint32(n_pairs), r(sp_), C.c_uint32(100), r(pp_), r(po_), r(ba_), r(mp_), r(mo_),
+                 None, None, r(tb_), None)
     assert call(ba_=None) == -1
     for k in ("d_ops", "d_n_ops", "d_begin"):
         b = BestAlignmentOutStruct(); b.d_ops = 16; b.max_ops = 300; b.d_n_ops = 16; b.d_begin = 16
@@ -346,3 +346,35 @@ def test_argument_validation_without_gpu():
     assert call(sp_=sp1) == -1
     long_ = StringSetStruct(); long_.d_words = 16; long_.bits = 2; long_.big_endian = 1; long_.stride = 528; long_.length = 513
     assert call(ss_=long_, mp_=None, mo_=None) == -4
+    assert call(ss_=None) == -1 and call(tb_=None) == -1 and call(pp_=None) == -1 and call(po_=None) == -1 and call(n_pairs=0x40000000) == -1
+    # which code wins when several checks fail: the call's arguments, mate_alignment and the MAPQ inputs / outputs (-1), then reads over
+    # 512 bp (-4), then the pair outputs and parameters and the index, reads and seed parameters (-1 or -4)
+    big = MapqParamsStruct(); big.d_min_score = 16; big.max_read_len = 513; big.match_bonus = 2
+    for k in ("d_ops", "d_n_ops", "d_begin", "max_ops"):
+        b = BestAlignmentOutStruct(); b.d_ops = 16; b.max_ops = 300; b.d_n_ops = 16; b.d_begin = 16
+        setattr(b, k, None if k != "max_ops" else 0)
+        assert call(ss_=long_, ba_=b, mp_=big) == -1, k
+    assert call(ss_=long_, ba_=None) == -1 and call(ss_=long_, tb_=None) == -1 and call(ss_=long_, pp_=None) == -1
+    assert call(ss_=long_, po_=None) == -1 and call(ss_=long_, n_pairs=0x40000000) == -1
+    assert call(ss_=long_, mp_=big, mo_=None) == -1 and call(ss_=long_, mp_=None) == -1
+    assert call(ss_=long_) == -1                                          # the min-score table (150) does not cover 513
+    assert call(ss_=long_, mp_=big) == -4
+    no_min = MapqParamsStruct(); no_min.max_read_len = 513; no_min.match_bonus = 2
+    assert call(ss_=long_, mp_=no_min) == -1
+    no_mapq = PairMapqOutStruct(); no_mapq.d_second_pair_score = 16
+    assert call(ss_=long_, mp_=big, mo_=no_mapq) == -1
+    assert call(ss_=long_, mp_=big, po_=bad_out) == -4 and call(ss_=long_, mp_=big, sp_=sp1) == -4
+    far = PairParamsStruct(); far.min_frag, far.max_frag, far.min_mate_score, far.rescue_capacity = 600, 500, 50, 100
+    assert call(ss_=long_, mp_=big, pp_=far) == -4 and call(pp_=far) == -1
+    bad_fm = FmIndexStruct(); bad_fm.d_bwt_occ = 32; bad_fm.d_ssa = 32; bad_fm.length = 1000; bad_fm.primary = 5; bad_fm.sa_interval = 12
+    assert call(ss_=long_, mp_=big, fm_=bad_fm) == -4 and call(fm_=bad_fm) == -1
+    assert call(ss_=long_, mp_=big, genome=None) == -4 and call(genome=None) == -1
+    assert call(ss_=long_, mp_=big, sp_=None) == -4 and call(sp_=None) == -1
+    long8 = StringSetStruct(); long8.d_words = 16; long8.bits = 8; long8.big_endian = 1; long8.stride = 528; long8.length = 513
+    assert call(ss_=long8, mp_=None, mo_=None) == -4 and call(ss_=long8, mp_=None, mo_=None, po_=bad_out) == -4
+    # 8-bit reads (-4) lose to every failed paired, best-alignment and MAPQ check
+    s8 = StringSetStruct(); s8.d_words = 16; s8.bits = 8; s8.big_endian = 1; s8.stride = 152; s8.length = 150
+    assert call(ss_=s8) == -4
+    no_ops = BestAlignmentOutStruct(); no_ops.d_ops = 16; no_ops.max_ops = 0; no_ops.d_n_ops = 16; no_ops.d_begin = 16
+    assert call(ss_=s8, po_=bad_out) == -1 and call(ss_=s8, sp_=sp1) == -1 and call(ss_=s8, pp_=far) == -1 and call(ss_=s8, ba_=no_ops) == -1
+    assert call(ss_=s8, mp_=short) == -1 and call(ss_=s8, mo_=None) == -1 and call(ss_=s8, mo_=no_mapq) == -1

@@ -105,10 +105,10 @@ def test_fixture_equals_live_reference(G):
 
 def test_argument_validation_without_gpu():
     """nvb_seed_extend_mapq rejects missing MAPQ inputs / outputs and a min-score table shorter than the reads with NVB_E_INVALID (-1)
-    before any CUDA call"""
+    before any CUDA call, also when the reads would be NVB_E_UNSUPPORTED (-4)"""
     from nvbio_b200 import _lib
     from nvbio_b200._lib import (StringSetStruct, GotohSchemeStruct, SeedExtendParamsStruct, FmIndexStruct, MapqParamsStruct,
-                                 MapqOutStruct)
+                                 MapqOutStruct, BestAlignmentOutStruct)
     L = _lib.lib()
     ss = StringSetStruct(); ss.d_words = 16; ss.bits = 2; ss.big_endian = 1; ss.stride = 160; ss.length = 150
     sch = GotohSchemeStruct(); sch.match, sch.mismatch, sch.pattern_gap_open, sch.pattern_gap_ext, sch.text_gap_open, sch.text_gap_ext = 2, -2, -5, -3, -5, -3
@@ -117,11 +117,10 @@ def test_argument_validation_without_gpu():
     fm = FmIndexStruct(); fm.d_bwt_occ = 32; fm.d_ssa = 32; fm.length = 1000; fm.primary = 5; fm.sa_interval = 16
     tb = C.c_size_t(0)
 
-    def call(mp, mo):
-        return L.nvb_seed_extend_mapq(C.byref(fm), C.c_void_p(16), C.byref(ss), C.c_uint32(8), C.byref(sp), C.c_uint32(100),
-                                      C.c_void_p(16), C.c_void_p(16), None, None, None, None, None, None,
-                                      C.byref(mp) if mp is not None else None, C.byref(mo) if mo is not None else None,
-                                      None, C.byref(tb), None)
+    def call(mp, mo, reads=ss, ba=None, params=sp):
+        r = lambda x: C.byref(x) if x is not None else None      # noqa: E731
+        return L.nvb_seed_extend_mapq(C.byref(fm), C.c_void_p(16), r(reads), C.c_uint32(8), C.byref(params), C.c_uint32(100),
+                                      C.c_void_p(16), C.c_void_p(16), None, None, None, None, None, r(ba), r(mp), r(mo), None, C.byref(tb), None)
 
     def good():
         mp = MapqParamsStruct(); mp.d_min_score, mp.max_read_len, mp.match_bonus = 16, 150, 2
@@ -129,10 +128,25 @@ def test_argument_validation_without_gpu():
         return mp, mo
 
     mp, mo = good()
-    assert call(None, mo) == -1 and call(mp, None) == -1
+    assert call(None, mo) == -1 and call(mp, None) == -1 and call(None, None) == -1
     for field in ("d_min_score",):
         mp, mo = good(); setattr(mp, field, None); assert call(mp, mo) == -1
     for field in ("d_second_score", "d_mapq"):
         mp, mo = good(); setattr(mo, field, None); assert call(mp, mo) == -1
     mp, mo = good(); mp.max_read_len = 149
     assert call(mp, mo) == -1
+    mp, mo = good(); assert call(mp, mo, reads=None) == -1
+    # 8-bit reads are NVB_E_UNSUPPORTED (-4), but every failed MAPQ or best-alignment check wins over it
+    s8 = StringSetStruct(); s8.d_words = 16; s8.bits = 8; s8.big_endian = 1; s8.stride = 152; s8.length = 150
+    mp, mo = good(); assert call(mp, mo, reads=s8) == -4
+    mp, mo = good(); mp.max_read_len = 149; assert call(mp, mo, reads=s8) == -1
+    mp, mo = good(); mo.d_mapq = None; assert call(mp, mo, reads=s8) == -1
+    mp, mo = good(); assert call(None, mo, reads=s8) == -1 and call(mp, None, reads=s8) == -1
+    ba = BestAlignmentOutStruct(); ba.d_ops = 16; ba.max_ops = 0; ba.d_n_ops = 16; ba.d_begin = 16
+    mp, mo = good(); assert call(mp, mo, ba=ba) == -1 and call(mp, mo, reads=s8, ba=ba) == -1
+    # the paired traceback's 512 bp limit does not apply to a single-end traceback: reads of 513 bp reach the seed checks
+    s513 = StringSetStruct(); s513.d_words = 16; s513.bits = 2; s513.big_endian = 1; s513.stride = 528; s513.length = 513
+    no_seed = SeedExtendParamsStruct(); no_seed.seed_len, no_seed.seed_interval, no_seed.band_len, no_seed.type = 0, 10, 31, 1
+    no_seed.both_strands, no_seed.max_seed_hits, no_seed.dedup_jobs, no_seed.scheme = 1, 100, 1, sch
+    ba.max_ops = 1100
+    mp, mo = good(); mp.max_read_len = 513; assert call(mp, mo, reads=s513, ba=ba, params=no_seed) == -1

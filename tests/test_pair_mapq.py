@@ -229,7 +229,7 @@ def test_pair_rule_edges(H):
 
 def test_argument_validation_without_gpu():
     """nvb_seed_extend_paired_mapq rejects missing MAPQ inputs / outputs, a min-score table shorter than the reads and what
-    nvb_seed_extend_paired rejects with NVB_E_INVALID (-1) before any CUDA call"""
+    nvb_seed_extend_paired rejects with NVB_E_INVALID (-1) before any CUDA call, also when the reads would be NVB_E_UNSUPPORTED (-4)"""
     from nvbio_b200 import _lib
     from nvbio_b200._lib import (StringSetStruct, GotohSchemeStruct, SeedExtendParamsStruct, FmIndexStruct, MapqParamsStruct,
                                  PairParamsStruct, PairOutStruct, PairMapqOutStruct)
@@ -248,10 +248,10 @@ def test_argument_validation_without_gpu():
         mo = PairMapqOutStruct(); mo.d_second_pair_score, mo.d_mate_mapq = 16, 16
         return pp, po, mp, mo
 
-    def call(pp, po, mp, mo, n_pairs=4):
+    def call(pp, po, mp, mo, n_pairs=4, reads=ss, params=sp, temp_bytes=tb):
         r = lambda x: C.byref(x) if x is not None else None      # noqa: E731
-        return L.nvb_seed_extend_paired_mapq(C.byref(fm), C.c_void_p(16), C.byref(ss), C.c_uint32(n_pairs), C.byref(sp), C.c_uint32(100),
-                                             r(pp), r(po), r(mp), r(mo), None, None, C.byref(tb), None)
+        return L.nvb_seed_extend_paired_mapq(C.byref(fm), C.c_void_p(16), r(reads), C.c_uint32(n_pairs), r(params), C.c_uint32(100),
+                                             r(pp), r(po), r(mp), r(mo), None, None, r(temp_bytes), None)
 
     pp, po, mp, mo = good()
     assert call(None, po, mp, mo) == -1 and call(pp, None, mp, mo) == -1 and call(pp, po, None, mo) == -1 and call(pp, po, mp, None) == -1
@@ -263,3 +263,22 @@ def test_argument_validation_without_gpu():
         pp, po, mp, mo = good(); setattr(po, field, None); assert call(pp, po, mp, mo) == -1
     pp, po, mp, mo = good(); pp.min_frag = 600; assert call(pp, po, mp, mo) == -1
     pp, po, mp, mo = good(); assert call(pp, po, mp, mo, n_pairs=0x40000000) == -1
+    pp, po, mp, mo = good(); assert call(pp, po, mp, mo, reads=None) == -1 and call(pp, po, mp, mo, temp_bytes=None) == -1
+    # 8-bit reads are NVB_E_UNSUPPORTED (-4), but every failed pair or MAPQ check wins over it
+    s8 = StringSetStruct(); s8.d_words = 16; s8.bits = 8; s8.big_endian = 1; s8.stride = 152; s8.length = 150
+    pp, po, mp, mo = good(); assert call(pp, po, mp, mo, reads=s8) == -4
+    pp, po, mp, mo = good(); mp.max_read_len = 149; assert call(pp, po, mp, mo, reads=s8) == -1
+    pp, po, mp, mo = good(); mo.d_mate_mapq = None; assert call(pp, po, mp, mo, reads=s8) == -1
+    pp, po, mp, mo = good(); assert call(pp, po, None, mo, reads=s8) == -1 and call(pp, po, mp, None, reads=s8) == -1
+    pp, po, mp, mo = good(); po.d_mate_strand = None; assert call(pp, po, mp, mo, reads=s8) == -1
+    pp, po, mp, mo = good(); pp.max_frag = 0; assert call(pp, po, mp, mo, reads=s8) == -1
+    pp, po, mp, mo = good(); assert call(pp, po, mp, mo, reads=s8, temp_bytes=None) == -1
+    pp, po, mp, mo = good(); assert call(pp, po, mp, mo, reads=s8, n_pairs=0x40000000) == -1
+    one = SeedExtendParamsStruct(); one.seed_len, one.seed_interval, one.band_len, one.type, one.both_strands, one.max_seed_hits = 20, 10, 31, 1, 0, 100
+    one.scheme = sch
+    pp, po, mp, mo = good(); assert call(pp, po, mp, mo, reads=s8, params=one) == -1 and call(pp, po, mp, mo, params=None) == -1
+    # the paired traceback's 512 bp limit does not apply here: reads of 513 bp reach the seed checks
+    s513 = StringSetStruct(); s513.d_words = 16; s513.bits = 2; s513.big_endian = 1; s513.stride = 528; s513.length = 513
+    no_seed = SeedExtendParamsStruct(); no_seed.seed_len, no_seed.seed_interval, no_seed.band_len, no_seed.type = 0, 10, 31, 1
+    no_seed.both_strands, no_seed.max_seed_hits, no_seed.dedup_jobs, no_seed.scheme = 1, 100, 1, sch
+    pp, po, mp, mo = good(); mp.max_read_len = 513; assert call(pp, po, mp, mo, reads=s513, params=no_seed) == -1
