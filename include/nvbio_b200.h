@@ -753,6 +753,69 @@ typedef struct nvb_bgzf_out {
 int nvb_bgzf_compress(const uint8_t* d_in, uint64_t n_bytes, const nvb_bgzf_out* out, void* d_temp, size_t* temp_bytes, void* stream);
 
 /* -------------------------------------------------------------------------------------------
+ * Coordinate sort of BAM records on the device.  Asynchronous on `stream`, no host round trip; NVB_E_TEMP_SIZE protocol.
+ *
+ * Input: n records laid out as nvb_bam_records lays them out, record i = bytes [d_offsets[i], d_offsets[i + 1]) of d_records, starting
+ * with its block_size; records may start at any byte offset.
+ * Order: key = (refID as uint32, pos as uint32), so unplaced records (refID -1) come last; equal keys keep their input order (a stable
+ * sort), so the unplaced records keep their input order too.  This is a valid SO:coordinate order; it does not break ties on the
+ * strand as samtools sort does.
+ * Output (nvb_bam_sort_out): output record j is input record d_order[j] (d_order may be NULL), at [d_offsets[j], d_offsets[j + 1]) of
+ * d_records (16-byte aligned).  d_offsets[n + 1] is always written whole; a record is stored only if it fits whole within `capacity`
+ * (d_records may be NULL when capacity is 0).
+ * NVB_E_INVALID (before any CUDA call) for a NULL out / temp_bytes / out->d_offsets, a NULL or misaligned out->d_records with capacity
+ * > 0, NULL inputs with n > 0, or n >= 2^31 - 1. */
+typedef struct nvb_bam_sort_out {
+    uint8_t*  d_records;
+    uint64_t  capacity;
+    uint64_t* d_offsets;               /* [n + 1] */
+    uint32_t* d_order;                 /* [n], may be NULL */
+} nvb_bam_sort_out;
+
+int nvb_bam_sort(const uint8_t* d_records, const uint64_t* d_offsets, uint32_t n, const nvb_bam_sort_out* out, void* d_temp,
+                 size_t* temp_bytes, void* stream);
+
+/* -------------------------------------------------------------------------------------------
+ * The BAI index (SAMv1 section 5.2) of a coordinate-sorted, BGZF-compressed BAM file, built on the device.  Asynchronous on `stream`,
+ * no host round trip; NVB_E_TEMP_SIZE protocol.  The rules are those of htslib's indexer (contrib/htslib/sam.c:366-424,
+ * hts.c:473-696), with the two deviations listed at the end.
+ *
+ * The file: the header's BGZF members (header_bytes compressed bytes, ending at a member boundary), then nvb_bgzf_compress of exactly
+ * d_records[0 : d_offsets[n]] (d_block_offsets is its output), then the 28-byte EOF block.  The records are in nvb_bam_sort order.
+ * Virtual offsets are those the reader reports (bgzf_tell), which moves to the next member as soon as it has consumed one: uncompressed
+ * byte u < total of the records is ((header_bytes + d_block_offsets[u / 0xFF00]) << 16) | (u % 0xFF00); a record's start is the map of
+ * d_offsets[i]; F = (header_bytes + d_block_offsets[n_blocks] + 28) << 16, the file size, ends what no later record ends.
+ * Per record: rlen = the sum of the M / D / N / = / X lengths of its CIGAR, 1 when that is 0 (the record's bin field is not read);
+ * [beg, end) = [pos, pos + rlen); bin = reg2bin(beg, end) (14 bits, 5 levels), 4680 for an unplaced record; mapped = FLAG lacks 0x4.
+ * Chunks, per refID: each maximal run of consecutive records with equal bin gives [start of its first record, start of the next record
+ * in the file, or F).  Pseudo-bin 37450 per present refID: (start of its first record, end of its last chunk), (n_mapped, n_unmapped).
+ * Bin compression: for levels 5 down to 1, every bin b at that level, its chunks ordered by start: when (last.end >> 16) -
+ * (first.start >> 16) < 65536 and the parent (b - 1) >> 3 holds chunks, b's chunks move to the parent and b is dropped.  Then in every
+ * real bin a chunk whose start >> 16 <= the previous chunk's end >> 16 joins it.
+ * Linear index per refID: n_intv = 1 + max over MAPPED records of (end - 1) >> 14, 0 without a mapped record; entry w = the start of the
+ * first mapped record covering window w; a window no record covers takes the refID's first-record start before the first covered
+ * window, else the entry before it.
+ * Serialisation: "BAI\1", n_ref, per refID n_bin, its bins in ascending bin number (bin, n_chunk, chunks) with the pseudo-bin last,
+ * n_intv and the entries; then n_no_coor.
+ * Deviations from the htslib of the reference tree (DESIGN.md section 3.15): bins are written in ascending order (htslib: its hash
+ * table's order, which the format leaves open), and n_no_coor is the number of unplaced records (htslib stops counting after the first).
+ *
+ * Output (nvb_bai_out): d_status[0] = 0, or 1 when the records are not in nvb_bam_sort order, 2 when a refID >= n_refs, 3 when a placed
+ * record's span leaves [0, 2^29] (the lowest code that applies); d_size[0] = the index's length (0 with a nonzero status); the index is
+ * stored only if the status is 0 and it fits whole within `capacity` (d_bai may be NULL when capacity is 0).
+ * NVB_E_INVALID (before any CUDA call) for a NULL out / temp_bytes / d_size / d_status / d_offsets / d_block_offsets, a NULL d_bai with
+ * capacity > 0, NULL records with n > 0, or n or n_refs >= 2^31 - 1; NVB_E_UNSUPPORTED when max_ref_len > 2^29, which BAI cannot index. */
+typedef struct nvb_bai_out {
+    uint8_t*  d_bai;
+    uint64_t  capacity;
+    uint64_t* d_size;                  /* [1] */
+    uint32_t* d_status;                /* [1] */
+} nvb_bai_out;
+
+int nvb_bam_index(const uint8_t* d_records, const uint64_t* d_offsets, uint32_t n, const uint64_t* d_block_offsets, uint64_t header_bytes,
+                  uint32_t n_refs, uint32_t max_ref_len, const nvb_bai_out* out, void* d_temp, size_t* temp_bytes, void* stream);
+
+/* -------------------------------------------------------------------------------------------
  * Host-buffer entry point: batches of reads in HOST memory in, per-read results in HOST memory out.
  * Replaces nvBowtie's input thread -> compute thread hand-off and its per-stage cudaDeviceSynchronize
  * (nvBowtie/bowtie2/cuda/compute_thread.cu:213-243, nvBowtie/bowtie2/cuda/defs.h:64, aligner_best_approx.h:219-241):

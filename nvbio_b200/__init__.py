@@ -12,3 +12,4 @@ from .pipeline import SeedExtendParams, seed_extend, StreamingSeedExtend, PairPa
 from .finish import finish_alignments, FinishedAlignments                        # noqa: F401
 from .bam import ContigTable, BamRecords, bam_records, bam_header, write_bam, numbered_names    # noqa: F401
 from .bgzf import BgzfBlocks, BgzfCall, bgzf_compress                           # noqa: F401
+from .bam_sort import SortedBamRecords, sort_bam_records, bam_index, write_sorted_bam    # noqa: F401

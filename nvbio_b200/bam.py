@@ -175,9 +175,11 @@ class BamCall:
         return BamRecords(data=self.data[:self.capacity], offsets=self.offsets, counts=self.counts)
 
 
-def bam_header(contigs: ContigTable, program: str = "nvbio_b200") -> bytes:
-    """BAM header bytes: magic, the SAM header text (@HD, one @SQ per contig, @PG) and the reference list"""
-    text = "@HD\tVN:1.0\tSO:unsorted\n" + "".join("@SQ\tSN:%s\tLN:%d\n" % (nm, ln) for nm, ln in zip(contigs.names, contigs.lengths)) + \
+def bam_header(contigs: ContigTable, program: str = "nvbio_b200", sort_order: str = "unsorted") -> bytes:
+    """BAM header bytes: magic, the SAM header text (@HD with SO:sort_order, one @SQ per contig, @PG) and the reference list"""
+    if sort_order not in ("unknown", "unsorted", "queryname", "coordinate"):
+        raise ValueError("bam_header: sort_order %r is not one of the SAM specification's" % sort_order)
+    text = "@HD\tVN:1.0\tSO:%s\n" % sort_order + "".join("@SQ\tSN:%s\tLN:%d\n" % (nm, ln) for nm, ln in zip(contigs.names, contigs.lengths)) + \
         "@PG\tID:%s\tPN:%s\n" % (program, program)
     t = text.encode()
     out = [b"BAM\1", struct.pack("<i", len(t)), t, struct.pack("<i", len(contigs.names))]
