@@ -496,6 +496,56 @@ int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     const nvb_mapq_params* mapq, const nvb_mapq_out* mapq_out,
                     void* d_temp, size_t* temp_bytes, void* stream);
 
+/* Up to k distinct alignments of every read, each traced (single end; nvBowtie's all-mapping mode, --all / -a, params.cpp:140-142,
+ * aligner_all.h:49-235 and 278-690, with the per-read limit of Bowtie2's -k).  Call with the arguments of nvb_seed_extend_mapq, with
+ * best_alignment == NULL; the best, second-best and MAPQ outputs are exactly those of nvb_seed_extend_mapq for the same inputs.
+ *   Candidates of read r: the alignments nvb_seed_extend_mapq's second-best rule sees (score s, strand t, end p = window begin + sink.x, tie
+ *   index), without the empty jobs and without those with s < d_min_score[len] -- every alignment the reference's all mode reports reaches
+ *   that score (score_all_inl.h:141-150).
+ *   Selection: the candidates in descending (s, -tie) order (make_best_key); a candidate (p, t) is admitted when it is distinct from every
+ *   alignment (a.end, a.strand) admitted before it -- distinct_alignment(p, t, a.end, a.strand, len), t != a.strand or p outside
+ *   [a.end - min(a.end, len/2), a.end + len/2] (io::distinct_alignments, nvbio/io/alignments_inl.h:33-47); the walk stops after
+ *   max_per_read admissions (0: none).  So rank 0 is nvb_seed_extend's best alignment when that reaches the min score (a read whose best
+ *   is below it has no alignment here), and for max_per_read != 1 rank 1 is nvb_seed_extend_mapq's second-best alignment.
+ *   Output: read order, and rank order within a read.  d_first is the exclusive scan of the per-read counts, written whole; read r's
+ *   alignments [d_first[r], d_first[r + 1]) are stored only if d_first[r + 1] <= capacity, so the stored reads are a prefix.  d_count =
+ *   (alignments stored, wanted), as d_n_rescue.  Alignment i: d_read[i], d_score[i], d_pos[i] (its end), and in `alignment` its banded
+ *   traceback as nvb_seed_extend_traceback writes a read's (ops END -> START at d_ops[i * max_ops ..], d_n_ops[i], d_begin[i] = (genome
+ *   coordinate of the first aligned text symbol, first aligned read symbol), d_strand[i]): equal to nvb_banded_gotoh_traceback of its
+ *   (strand, window) job alone.  Entries at or beyond d_count[0] are not written.  No host round trip.
+ *   Deliberate deviations from nvBowtie (DESIGN.md section 3.16): it de-duplicates only identical (read, strand, seed diagonal) hits
+ *   (aligner_all.h:496-553), so one locus reached on two diagonals is reported twice -- here the distinct rule suppresses that; and the
+ *   per-read limit max_per_read.
+ * NVB_E_INVALID (before any CUDA call) for a NULL mapq, all_params or all_out, a NULL d_first / d_read / d_score / d_pos / d_count or
+ * alignment.d_ops / d_n_ops / d_begin / d_strand, best_alignment != NULL, alignment.max_ops == 0, or the checks of nvb_seed_extend_mapq;
+ * NVB_E_UNSUPPORTED for reads->length > 512 (as the paired traceback).  The alignments are traced in ceil(capacity / n_reads) slices of
+ * at most n_reads (each a few kernel launches; one past the stored alignments does no work), so the
+ * temp size grows by the traceback's share of nvb_seed_extend_traceback plus about 24 bytes per unit of hit_capacity, 16 bytes per
+ * alignment slot and 12 bytes per read. */
+typedef struct nvb_all_params {
+    uint32_t max_per_read;             /* k; 0 = every distinct alignment (nvBowtie --all) */
+    uint32_t capacity;                 /* alignment slots of the per-alignment outputs */
+} nvb_all_params;
+typedef struct nvb_all_out {
+    uint32_t* d_first;                 /* [n_reads + 1] read r's alignments are [d_first[r], d_first[r + 1]); always written whole */
+    uint32_t* d_read;                  /* [capacity] the read of alignment i */
+    int32_t*  d_score;                 /* [capacity] */
+    uint32_t* d_pos;                   /* [capacity] end = window begin + sink.x, as d_best_pos */
+    nvb_best_alignment_out alignment;  /* [capacity] ops / n_ops / begin / strand, as nvb_seed_extend_traceback */
+    uint32_t* d_count;                 /* [2] alignments stored, wanted */
+} nvb_all_out;
+
+int nvb_seed_extend_all(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_reads,
+                    const nvb_seed_extend_params* params, uint32_t hit_capacity,
+                    int32_t* d_best_score, uint32_t* d_best_pos,
+                    uint32_t* d_n_hits, uint32_t* d_hit_read, nvb_uint2* d_hit_window,
+                    int32_t* d_hit_score, nvb_uint2* d_hit_sink,
+                    const nvb_best_alignment_out* best_alignment,
+                    const nvb_mapq_params* mapq, const nvb_mapq_out* mapq_out,
+                    const nvb_all_params* all_params, const nvb_all_out* all_out,
+                    void* d_temp, size_t* temp_bytes, void* stream);
+
 /* -------------------------------------------------------------------------------------------
  * Paired-end composition (BASELINE configs[4] shape; nvBowtie best_approx paired: anchor scoring + opposite-mate full DP,
  * nvBowtie/bowtie2/cuda/aligner_best_approx_paired.h, score_opposite_inl.h:90-266, alignment_utils.h:62-95 PE_POLICY_FR).
@@ -723,6 +773,34 @@ typedef struct nvb_bam_out {
 } nvb_bam_out;
 
 int nvb_bam_records(const nvb_bam_in* in, uint32_t n, const nvb_bam_out* out, void* d_temp, size_t* temp_bytes, void* stream);
+
+/* BAM records of nvb_seed_extend_all's alignments: several per read.  Same bam1_t encoding, placement and contig rules as nvb_bam_records,
+ * single end.  Inputs: base.reads = the n_reads reads (with base.d_read_quals and one name per read); base.d_n_ops / d_begin / d_strand /
+ * d_score and base.finish = the per-alignment outputs of nvb_seed_extend_all and of nvb_finish_alignments over its alignment slots (string
+ * i of that call's string set is read d_read[i]); base.d_mapq / base.d_second_score are per READ (may be NULL); base.d_pair_flags must be
+ * NULL.  d_first / capacity as nvb_seed_extend_all wrote them: read r's alignments are [d_first[r], d_first[r + 1]), stored only if
+ * d_first[r + 1] <= capacity.
+ * Records, per read in read order: its alignments that pass the placement rule (mapped, span inside one contig), in rank order.  The
+ * first is the PRIMARY record: MAPQ d_mapq[r] (255 without it) and XS as in nvb_bam_records; every later one is SECONDARY: FLAG 0x100,
+ * MAPQ 255, no XS.  Every mapped record carries NM AS [XS] XM XO XG MD as nvb_bam_records writes them, then NH:i = the read's number of
+ * mapped records, typed by htslib's rule.  A read with no placeable alignment -- also one whose range lies beyond capacity -- gets exactly
+ * one unmapped record, as nvb_bam_records writes it.  SEQ and QUAL are written in full on every record.  So every read yields exactly one
+ * primary or unmapped record.
+ * Deliberate deviation from nvBowtie (DESIGN.md section 3.16): it defines SAM_FLAGS_SECONDARY (nvbio/io/output/output_sam.h:57) but never
+ * sets it, and writes every all-mode alignment as a primary record with MAPQ 255 (aligner_all.h:83); the SAM specification asks for one
+ * primary line per read.
+ * Outputs (nvb_bam_out): d_offsets has room for n_reads + capacity + 1 entries; record k = bytes [d_offsets[k], d_offsets[k + 1]) for
+ * k < d_counts[0], the number of records (the entries after it repeat the total).  d_counts[1] = mapped records, [2] alignments unmapped
+ * by the contig rule, [3] alignments unmapped because finish did not write them whole, plus the reads beyond capacity.  Otherwise the
+ * capacity rules of nvb_bam_out.  No host round trip.  NVB_E_INVALID (before any CUDA call) for the checks of nvb_bam_records, a NULL in /
+ * d_first, d_pair_flags != NULL, or n_reads + capacity >= 2^31 - 1. */
+typedef struct nvb_bam_all_in {
+    nvb_bam_in       base;
+    const uint32_t*  d_first;          /* [n_reads + 1] */
+    uint32_t         capacity;         /* alignment slots of the nvb_seed_extend_all call */
+} nvb_bam_all_in;
+
+int nvb_bam_records_all(const nvb_bam_all_in* in, uint32_t n_reads, const nvb_bam_out* out, void* d_temp, size_t* temp_bytes, void* stream);
 
 /* -------------------------------------------------------------------------------------------
  * BGZF compression on the device (SAMv1 section 4.1; the framing of htslib's writer, contrib/htslib/bgzf.c:59 header and

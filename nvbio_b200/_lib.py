@@ -10,12 +10,12 @@ EXPORTS = [
     "nvb_version", "nvb_error_string",
     "nvb_fm_rank", "nvb_fm_rank4", "nvb_fm_match", "nvb_fm_match_approx", "nvb_fm_locate", "nvb_fm_filter_rank", "nvb_fm_filter_locate",
     "nvb_banded_gotoh_score", "nvb_banded_gotoh_score_indirect", "nvb_banded_gotoh_traceback", "nvb_gotoh_score", "nvb_gotoh_score_indirect", "nvb_banded_gotoh_score_window", "nvb_banded_gotoh_score_best2", "nvb_gotoh_traceback", "nvb_seed_extend_paired",
-    "nvb_fm_build_occ", "nvb_fm_build_bwt", "nvb_fm_build_ktab", "nvb_fm_build_ktab_located", "nvb_fm_build_ktab_context", "nvb_fm_build_ktab_wide", "nvb_fm_build_rows", "nvb_seed_extend", "nvb_seed_extend_traceback", "nvb_seed_extend_mapq", "nvb_seed_extend_paired_mapq", "nvb_seed_extend_paired_traceback",
+    "nvb_fm_build_occ", "nvb_fm_build_bwt", "nvb_fm_build_ktab", "nvb_fm_build_ktab_located", "nvb_fm_build_ktab_context", "nvb_fm_build_ktab_wide", "nvb_fm_build_rows", "nvb_seed_extend", "nvb_seed_extend_traceback", "nvb_seed_extend_mapq", "nvb_seed_extend_all", "nvb_seed_extend_paired_mapq", "nvb_seed_extend_paired_traceback",
     "nvb_seed_extend_stage_ms",
     "nvb_dict_rank", "nvb_dict_rank4", "nvb_dict_build_occ",
     "nvb_map_seeds", "nvb_fm_locate_init", "nvb_fm_locate_lookup", "nvb_fm_locate_sorted",
     "nvb_pipeline_create", "nvb_pipeline_submit", "nvb_pipeline_wait", "nvb_pipeline_traffic", "nvb_pipeline_destroy",
-    "nvb_finish_alignments", "nvb_bam_records", "nvb_bgzf_compress", "nvb_bam_sort", "nvb_bam_index",
+    "nvb_finish_alignments", "nvb_bam_records", "nvb_bam_records_all", "nvb_bgzf_compress", "nvb_bam_sort", "nvb_bam_index",
 ]
 # test / tuning hooks of include/nvbio_b200_debug.h (not part of the drop-in ABI)
 DEBUG_EXPORTS = [
@@ -71,6 +71,10 @@ class BamInStruct(C.Structure):           # nvb_bam_in
                 ("d_names", C.c_void_p), ("d_name_offsets", C.c_void_p)]
 
 
+class BamAllInStruct(C.Structure):        # nvb_bam_all_in
+    _fields_ = [("base", BamInStruct), ("d_first", C.c_void_p), ("capacity", C.c_uint32)]
+
+
 class BamOutStruct(C.Structure):          # nvb_bam_out
     _fields_ = [("d_records", C.c_void_p), ("capacity", C.c_uint64), ("d_offsets", C.c_void_p), ("d_counts", C.c_void_p)]
 
@@ -93,6 +97,15 @@ class MapqParamsStruct(C.Structure):       # nvb_mapq_params
 
 class MapqOutStruct(C.Structure):          # nvb_mapq_out
     _fields_ = [("d_second_score", C.c_void_p), ("d_second_pos", C.c_void_p), ("d_second_strand", C.c_void_p), ("d_mapq", C.c_void_p)]
+
+
+class AllParamsStruct(C.Structure):         # nvb_all_params
+    _fields_ = [("max_per_read", C.c_uint32), ("capacity", C.c_uint32)]
+
+
+class AllOutStruct(C.Structure):            # nvb_all_out
+    _fields_ = [("d_first", C.c_void_p), ("d_read", C.c_void_p), ("d_score", C.c_void_p), ("d_pos", C.c_void_p),
+                ("alignment", BestAlignmentOutStruct), ("d_count", C.c_void_p)]
 
 
 class PairParamsStruct(C.Structure):        # nvb_pair_params

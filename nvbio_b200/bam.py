@@ -9,7 +9,7 @@ from dataclasses import dataclass
 from typing import Iterable, List, Optional, Sequence
 import numpy as np
 import torch
-from ._lib import lib, check, BamInStruct, BamOutStruct
+from ._lib import lib, check, BamInStruct, BamOutStruct, BamAllInStruct
 from .finish import FinishedAlignments
 from .strings import PackedStringSet
 
@@ -173,6 +173,60 @@ class BamCall:
         check(lib().nvb_bam_records(C.byref(self.a), C.c_uint32(self.n), C.byref(self.o), C.c_void_p(self.temp.data_ptr()), C.byref(tb),
                                     C.c_void_p(st.cuda_stream)), "nvb_bam_records")
         return BamRecords(data=self.data[:self.capacity], offsets=self.offsets, counts=self.counts)
+
+
+def bam_records_all(al, finished: FinishedAlignments, reads: PackedStringSet, contigs: ContigTable, names: Sequence,
+                    quals: Optional[torch.Tensor] = None, capacity: Optional[int] = None, stream=None) -> BamRecords:
+    """BAM records of seed_extend_all's alignments (nvb_bam_records_all): per read, its placeable alignments in rank order, the first
+    primary (the read's MAPQ and XS), the others secondary (FLAG 0x100, MAPQ 255), each with NH; one unmapped record for a read without a
+    placeable alignment.  al: an AllAlignments; finished: finish_alignments over al.strings(reads) and al's ops / n_ops / begin / strand;
+    names: one per read; capacity: bytes of the output buffer (by default an upper bound that never truncates).  Waits for the record
+    count, so that the result holds exactly the records."""
+    n = al.n_reads
+    if reads.count != n or len(names) != n:
+        raise ValueError("bam_records_all: %d reads and %d names for %d reads" % (reads.count, len(names), n))
+    if finished.n_cigar.numel() != al.capacity:
+        raise ValueError("bam_records_all: %d finished alignments for %d alignment slots" % (finished.n_cigar.numel(), al.capacity))
+    if quals is not None and (quals.dtype != torch.uint8 or not quals.is_cuda):
+        raise ValueError("bam_records_all: quals must be a uint8 device tensor")
+    dev = al.score.device
+    d_names, d_name_off, name_bytes = _names_tensors(names, dev)
+    max_cigar, max_md = finished.cigar.shape[1], finished.md.shape[1]
+    slots = n + al.capacity
+    if capacity is None:
+        per = 36 + 1 + 4 * max_cigar + (reads.length + 1) // 2 + reads.length + 6 * 7 + 4 + max_md + 7
+        capacity = slots * per + name_bytes * (1 + al.capacity)
+    data = torch.empty(max(int(capacity), 16), dtype=torch.uint8, device=dev)
+    offsets = torch.empty(slots + 1, dtype=torch.int64, device=dev)
+    counts = torch.empty(4, dtype=torch.int32, device=dev)
+
+    def ptr(t):
+        return None if t is None else t.untyped_storage().data_ptr() + t.storage_offset() * t.element_size()
+    cdev = contigs.device(dev)
+    a = BamAllInStruct()
+    b = a.base
+    b.reads = reads.struct()
+    b.d_read_quals = ptr(quals)
+    b.d_n_ops, b.d_begin, b.d_strand = ptr(al.n_ops), ptr(al.begin), ptr(al.strand)
+    f = b.finish
+    f.d_cigar, f.max_cigar, f.d_n_cigar = ptr(finished.cigar), max_cigar, ptr(finished.n_cigar)
+    f.d_md, f.max_md, f.d_md_len, f.d_edits = ptr(finished.md), max_md, ptr(finished.md_len), ptr(finished.edits)
+    b.d_score, b.d_mapq, b.d_second_score, b.d_pair_flags = ptr(al.score), ptr(al.mapq), ptr(al.second_score), None
+    b.d_contig_begin, b.n_contigs = ptr(cdev), len(contigs.names)
+    b.d_names, b.d_name_offsets = ptr(d_names), ptr(d_name_off)
+    a.d_first, a.capacity = ptr(al.first), al.capacity
+    o = BamOutStruct()
+    o.d_records, o.capacity, o.d_offsets, o.d_counts = data.data_ptr(), int(capacity), offsets.data_ptr(), counts.data_ptr()
+    st = (stream if stream is not None else torch.cuda.current_stream(dev)).cuda_stream
+    tb = C.c_size_t(0)
+    err = lib().nvb_bam_records_all(C.byref(a), C.c_uint32(n), C.byref(o), None, C.byref(tb), C.c_void_p(st))
+    if err not in (0, NVB_E_TEMP_SIZE):
+        check(err, "nvb_bam_records_all")
+    temp = torch.empty(max(tb.value, 1), dtype=torch.uint8, device=dev)
+    check(lib().nvb_bam_records_all(C.byref(a), C.c_uint32(n), C.byref(o), C.c_void_p(temp.data_ptr()), C.byref(tb), C.c_void_p(st)),
+          "nvb_bam_records_all")
+    n_rec = int(counts[0])                                                 # (synchronises)
+    return BamRecords(data=data[:int(capacity)], offsets=offsets[:n_rec + 1], counts=counts)
 
 
 def bam_header(contigs: ContigTable, program: str = "nvbio_b200", sort_order: str = "unsorted") -> bytes:

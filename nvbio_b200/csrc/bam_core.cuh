@@ -49,12 +49,27 @@ struct BamIn {
     const uint32_t* pair_flags;
     const uint32_t* contig_begin; uint32_t n_contigs;
     const char*     names;  const uint32_t* name_off;
-    uint32_t        n;                              // alignments (= records)
+    uint32_t        n;                              // alignments (= records); nvb_bam_records_all: record slots
+    const uint4*    rec = nullptr;                  // nvb_bam_records_all: record k = (alignment or BAM_NO_ALN, read, NH, primary); else NULL
 };
 
-// alignment of record k (paired: record 2p + m is mate m of pair p, alignment m * n / 2 + p) and the index of its name
-__host__ __device__ __forceinline__ uint32_t bam_alignment(const BamIn& in, uint32_t k) { return in.pair_flags ? (k & 1u) * (in.n >> 1) + (k >> 1) : k; }
-__host__ __device__ __forceinline__ uint32_t bam_name(const BamIn& in, uint32_t k) { return in.pair_flags ? k >> 1 : k; }
+constexpr uint32_t BAM_NO_ALN = 0xFFFFFFFFu;        // the unmapped record of a read without a placeable alignment
+
+// alignment of record k (paired: record 2p + m is mate m of pair p, alignment m * n / 2 + p), the index of its name and of its read in
+// `reads`; mapq / second score are per alignment in nvb_bam_records and per read in nvb_bam_records_all
+__host__ __device__ __forceinline__ uint32_t bam_alignment(const BamIn& in, uint32_t k)
+{
+    return in.rec ? in.rec[k].x : (in.pair_flags ? (k & 1u) * (in.n >> 1) + (k >> 1) : k);
+}
+__host__ __device__ __forceinline__ uint32_t bam_name(const BamIn& in, uint32_t k) { return in.rec ? in.rec[k].y : (in.pair_flags ? k >> 1 : k); }
+__host__ __device__ __forceinline__ uint32_t bam_seq(const BamIn& in, uint32_t k) { return in.rec ? in.rec[k].y : bam_alignment(in, k); }
+// XS of mapped record k (alignment a): INT32_MIN = none.  nvb_bam_records_all: the read's second score, on its primary record only
+__host__ __device__ __forceinline__ int32_t bam_xs(const BamIn& in, uint32_t k, uint32_t a)
+{
+    if (!in.second) return INT32_MIN;
+    if (in.rec) return in.rec[k].w ? in.second[in.rec[k].y] : INT32_MIN;
+    return in.second[a];
+}
 
 // the largest r < n_contigs with contig_begin[r] <= x (upper_bound - 1; contig_begin[0] = 0)
 __host__ __device__ __forceinline__ uint32_t contig_of(const uint32_t* __restrict__ cb, uint32_t n_contigs, uint32_t x)
@@ -103,12 +118,13 @@ __host__ __device__ __forceinline__ uint32_t bam_name_len(const BamIn& in, uint3
     return l < BAM_MAX_NAME ? l : BAM_MAX_NAME;
 }
 
-// tag bytes of mapped alignment a: NM, AS, [XS], XM, XO, XG as integer tags (md0 = their size), then MD:Z when not empty
-__host__ __device__ __forceinline__ uint32_t bam_int_tags_bytes(const BamIn& in, uint32_t a)
+// tag bytes of mapped alignment a with second score xs (bam_xs): NM, AS, [XS], XM, XO, XG as integer tags; MD:Z (when not empty) and,
+// in nvb_bam_records_all, NH follow them
+__host__ __device__ __forceinline__ uint32_t bam_int_tags_bytes(const BamIn& in, uint32_t a, int32_t xs)
 {
     const uint32_t* e = in.edits + 4u * (size_t)a;
     uint32_t b = 15u + tag_int_bytes(e[0]) + tag_int_bytes(in.score[a]) + tag_int_bytes(e[1]) + tag_int_bytes(e[2]) + tag_int_bytes(e[3]);
-    if (in.second && in.second[a] != INT32_MIN) b += 3u + tag_int_bytes(in.second[a]);
+    if (xs != INT32_MIN) b += 3u + tag_int_bytes(xs);
     return b;
 }
 
@@ -148,9 +164,13 @@ __host__ __device__ inline uint64_t bam_plan_record(const BamIn& in, uint32_t k,
     }
     const uint32_t nc = mapped ? in.n_cigar[a] : 0u;
     if (mapped) bin = bam_reg2bin(pos, (int64_t)pos + me.rlen);
-    const uint32_t mapq = mapped ? (in.mapq ? in.mapq[a] : 255u) : 0u;
+    uint32_t mapq = mapped ? (in.mapq ? in.mapq[a] : 255u) : 0u;
+    if (in.rec && mapped) {                         // nvb_bam_records_all: the read's MAPQ on its primary record, 255 and 0x100 on the others
+        mapq = in.rec[k].w && in.mapq ? in.mapq[in.rec[k].y] : 255u;
+        if (!in.rec[k].w) flag |= 0x100u;
+    }
     const uint32_t l_name = bam_name_len(in, bam_name(in, k)) + 1u;
-    const uint32_t l_seq = str_len(in.reads, a);
+    const uint32_t l_seq = str_len(in.reads, bam_seq(in, k));
     w[0] = (uint32_t)ref; w[1] = (uint32_t)pos;
     w[2] = bin << 16 | mapq << 8 | l_name;
     w[3] = flag << 16 | nc;
@@ -158,8 +178,9 @@ __host__ __device__ inline uint64_t bam_plan_record(const BamIn& in, uint32_t k,
     w[5] = (uint32_t)nref; w[6] = (uint32_t)npos; w[7] = (uint32_t)tlen;
     uint64_t size = BAM_FIXED + l_name + 4u * nc + ((l_seq + 1u) >> 1) + l_seq;
     if (mapped) {
-        size += bam_int_tags_bytes(in, a);
+        size += bam_int_tags_bytes(in, a, bam_xs(in, k, a));
         if (in.md_len[a]) size += 4u + in.md_len[a];
+        if (in.rec) size += 3u + tag_int_bytes(in.rec[k].z);
     }
     return size;
 }
@@ -180,6 +201,39 @@ __host__ __device__ inline void bam_plan_unit(const BamIn& in, uint32_t u, uint3
     cnt[0] += (p0.state == BAM_MAPPED) + (p1.state == BAM_MAPPED);
     cnt[1] += (p0.state == BAM_OFF_CONTIG) + (p1.state == BAM_OFF_CONTIG);
     cnt[2] += (p0.state == BAM_UNFINISHED) + (p1.state == BAM_UNFINISHED);
+}
+
+// nvb_bam_records_all, read r (alignments [first[r], first[r + 1]), stored when first[r + 1] <= capacity): its mapped alignments in rank
+// order, or one unmapped record.  rec_first == NULL: only count -- returns the records, adds (mapped, off-contig, unfinished or beyond the
+// capacity) to cnt.  Else writes records rec_first[r] .. : rec (as BamIn.rec, which must point at it), cores and sizes
+__host__ __device__ inline uint32_t bam_plan_read_all(const BamIn& in, uint32_t r, const uint32_t* first, uint32_t capacity, const uint32_t* rec_first,
+                                                      uint4* rec, uint32_t* __restrict__ cores, uint64_t* __restrict__ sizes, uint32_t cnt[3])
+{
+    const uint32_t b = first[r], e = first[r + 1];
+    const bool stored = e <= capacity;
+    uint32_t m = 0;
+    if (stored)
+        for (uint32_t a = b; a < e; ++a) {
+            const uint32_t st = bam_place(in, a).state;
+            m += st == BAM_MAPPED;
+            if (!rec_first) { cnt[1] += st == BAM_OFF_CONTIG; cnt[2] += st == BAM_UNFINISHED; }
+        }
+    if (!rec_first) { cnt[0] += m; cnt[2] += !stored; return m ? m : 1u; }
+    uint32_t k = rec_first[r];
+    if (!m) {
+        BamPlace p; p.state = BAM_UNALIGNED; p.ref = -1; p.pos = -1; p.rlen = 0u; p.strand = 0u;
+        rec[k] = make_uint4(BAM_NO_ALN, r, 0u, 1u);
+        sizes[k] = bam_plan_record(in, k, p, nullptr, cores + 8u * (size_t)k);
+        return 1u;
+    }
+    for (uint32_t a = b; a < e; ++a) {
+        const BamPlace p = bam_place(in, a);
+        if (p.state != BAM_MAPPED) continue;
+        rec[k] = make_uint4(a, r, m, k == rec_first[r] ? 1u : 0u);
+        sizes[k] = bam_plan_record(in, k, p, nullptr, cores + 8u * (size_t)k);
+        ++k;
+    }
+    return m;
 }
 
 __host__ __device__ __forceinline__ void put32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }
@@ -213,7 +267,7 @@ __host__ __device__ __forceinline__ void bam_compose(const BamIn& in, uint32_t k
     const uint32_t* cg = in.cigar + (size_t)a * in.max_cigar;
     for (uint32_t i = lane; i < nc; i += nl) put32(p + 4u * i, cg[i]);
     p += 4u * nc;
-    const uint32_t off = str_off(in.reads, a);
+    const uint32_t off = str_off(in.reads, bam_seq(in, k));
     for (uint32_t y = lane * CHUNK; y < l; y += nl * CHUNK) {
         const uint32_t cnt = l - y < CHUNK ? l - y : CHUNK;
         uint32_t codes, nflags;
@@ -236,20 +290,24 @@ __host__ __device__ __forceinline__ void bam_compose(const BamIn& in, uint32_t k
     p += l;
     if (!mapped) return;
     const uint32_t* e = in.edits + 4u * (size_t)a;
+    const int32_t xs = bam_xs(in, k, a);
     if (lane == 0u) {
         uint8_t* t = put_int_tag(p, 'N', 'M', e[0]);
         t = put_int_tag(t, 'A', 'S', in.score[a]);
-        if (in.second && in.second[a] != INT32_MIN) t = put_int_tag(t, 'X', 'S', in.second[a]);
+        if (xs != INT32_MIN) t = put_int_tag(t, 'X', 'S', xs);
         t = put_int_tag(t, 'X', 'M', e[1]);
         t = put_int_tag(t, 'X', 'O', e[2]);
         put_int_tag(t, 'X', 'G', e[3]);
     }
     const uint32_t ml = in.md_len[a];
-    if (ml == 0u) return;
-    p += bam_int_tags_bytes(in, a);
-    const char* md = in.md + (size_t)a * in.max_md;
-    if (lane == 0u) { p[0] = 'M'; p[1] = 'D'; p[2] = 'Z'; p[3u + ml] = 0u; }
-    for (uint32_t i = lane; i < ml; i += nl) p[3u + i] = (uint8_t)md[i];
+    p += bam_int_tags_bytes(in, a, xs);
+    if (ml) {
+        const char* md = in.md + (size_t)a * in.max_md;
+        if (lane == 0u) { p[0] = 'M'; p[1] = 'D'; p[2] = 'Z'; p[3u + ml] = 0u; }
+        for (uint32_t i = lane; i < ml; i += nl) p[3u + i] = (uint8_t)md[i];
+        p += 4u + ml;
+    }
+    if (in.rec && lane == 0u) put_int_tag(p, 'N', 'H', in.rec[k].z);
 }
 
 } // namespace nvb

@@ -267,6 +267,11 @@ constexpr uint32_t FULL_TB_MAX_M = 512u;               // 16 pattern columns per
 // gotoh_kernels.cu: with a == NULL only *pool_bytes (the slot pool, bounded by the resident warps and max_n, not by the item count);
 // else the launch.  NVB_E_UNSUPPORTED unless 1 <= max_m <= FULL_TB_MAX_M and max_n <= 65535
 int full_warp_traceback(int type, uint32_t max_m, uint32_t max_n, const FullTbArgs* a, size_t* pool_bytes, cudaStream_t s);
+// gotoh_kernels.cu: nvb_banded_gotoh_traceback over the first min(*d_n, n) alignments, the count on the device (d_n == NULL: all n); the
+// temp size is that of n alignments
+int banded_traceback(int band_len, int type, const nvb_gotoh_scheme* scheme, const nvb_string_set* patterns, const uint8_t* d_quals,
+                     const nvb_string_set* texts, const uint32_t* d_n, uint32_t n, int32_t* d_score, nvb_uint2* d_sink, nvb_uint2* d_source,
+                     uint8_t* d_ops, uint32_t max_ops, uint32_t* d_n_ops, void* d_temp, size_t* temp_bytes, void* stream);
 
 // left boundary (H, E) of text row r (0-based) in the first column, as gotoh_full_impl2 starts its first stripe
 template <int TYPE>

@@ -598,7 +598,7 @@ __global__ void __launch_bounds__(256)
 gotoh_traceback_gapless_kernel(const GotohScheme S, const GotohBatch b, const TracebackOut o, uint32_t* __restrict__ todo, uint32_t* __restrict__ todo_count)
 {
     const uint32_t a = blockIdx.x * 256 + threadIdx.x;
-    const bool in_range = a < b.n_max;
+    const bool in_range = a < batch_count(b);
     uint32_t len = 0u;
     bool done = false;
     if (in_range) {
@@ -950,11 +950,12 @@ int nvb_gotoh_score_indirect(int type, const nvb_gotoh_scheme* scheme, const nvb
     return gotoh_full_impl(type, scheme, patterns, d_quals, texts, d_n, n_max, d_score, d_sink, d_temp, temp_bytes, stream);
 }
 
-int nvb_banded_gotoh_traceback(int band_len, int type, const nvb_gotoh_scheme* scheme,
-                               const nvb_string_set* patterns, const uint8_t* d_quals, const nvb_string_set* texts, uint32_t n,
-                               int32_t* d_score, nvb_uint2* d_sink, nvb_uint2* d_source,
-                               uint8_t* d_ops, uint32_t max_ops, uint32_t* d_n_ops,
-                               void* d_temp, size_t* temp_bytes, void* stream)
+} // extern "C"
+
+namespace nvb {
+int banded_traceback(int band_len, int type, const nvb_gotoh_scheme* scheme, const nvb_string_set* patterns, const uint8_t* d_quals,
+                     const nvb_string_set* texts, const uint32_t* d_n, uint32_t n, int32_t* d_score, nvb_uint2* d_sink, nvb_uint2* d_source,
+                     uint8_t* d_ops, uint32_t max_ops, uint32_t* d_n_ops, void* d_temp, size_t* temp_bytes, void* stream)
 {
     if (!scheme || !temp_bytes || !valid_strset(patterns) || !valid_strset(texts)) return NVB_E_INVALID;
     if (!(band_len == 3 || band_len == 5 || band_len == 7 || band_len == 15 || band_len == 31)) return NVB_E_INVALID;
@@ -977,7 +978,7 @@ int nvb_banded_gotoh_traceback(int band_len, int type, const nvb_gotoh_scheme* s
     cudaStream_t s = as_stream(stream);
     GotohBatch b;
     b.pat = make_strset(patterns); b.txt = make_strset(texts); b.quals = d_quals;
-    b.d_n = nullptr; b.n_max = n; b.score = d_score; b.sink = (uint2*)d_sink;
+    b.d_n = d_n; b.n_max = n; b.score = d_score; b.sink = (uint2*)d_sink;
     TracebackOut o;
     o.source = (uint2*)d_source; o.ops = d_ops; o.n_ops = d_n_ops; o.max_ops = max_ops; o.dirs = dirs; o.dir_rows = max_m;
     const GotohScheme S = make_scheme(scheme);
@@ -989,7 +990,7 @@ int nvb_banded_gotoh_traceback(int band_len, int type, const nvb_gotoh_scheme* s
     // has no gap (most reads) from the sink alone; 3. the rest goes through the direction-matrix traceback
     {
         size_t sb = score_bytes + 256;
-        const int r = banded_impl(band_len, type, scheme, patterns, d_quals, texts, nullptr, n, d_score, d_sink, score_tmp, &sb, stream);
+        const int r = banded_impl(band_len, type, scheme, patterns, d_quals, texts, d_n, n, d_score, d_sink, score_tmp, &sb, stream);
         if (r != NVB_OK) return r;
     }
     NVB_CUDA_TRY(cudaMemsetAsync(todo_count, 0, sizeof(uint32_t), s));
@@ -997,6 +998,19 @@ int nvb_banded_gotoh_traceback(int band_len, int type, const nvb_gotoh_scheme* s
     else                   gotoh_traceback_gapless_kernel<NVB_SEMI_GLOBAL><<<(n + 255u) / 256u, 256, 0, s>>>(S, b, o, todo, todo_count);
     NVB_LAUNCH_CHECK();
     return dispatch_traceback(band_len, type, S, b, o, todo, todo_count, s);
+}
+} // namespace nvb
+
+extern "C" {
+
+int nvb_banded_gotoh_traceback(int band_len, int type, const nvb_gotoh_scheme* scheme,
+                               const nvb_string_set* patterns, const uint8_t* d_quals, const nvb_string_set* texts, uint32_t n,
+                               int32_t* d_score, nvb_uint2* d_sink, nvb_uint2* d_source,
+                               uint8_t* d_ops, uint32_t max_ops, uint32_t* d_n_ops,
+                               void* d_temp, size_t* temp_bytes, void* stream)
+{
+    return banded_traceback(band_len, type, scheme, patterns, d_quals, texts, nullptr, n, d_score, d_sink, d_source, d_ops, max_ops, d_n_ops,
+                            d_temp, temp_bytes, stream);
 }
 
 int nvb_banded_gotoh_score_window(int band_len, int type, const nvb_gotoh_scheme* scheme,

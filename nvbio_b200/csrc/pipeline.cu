@@ -136,18 +136,6 @@ __device__ __forceinline__ uint2 hit_window(uint32_t pos, uint32_t seed_begin, u
     return make_uint2(gb, ge64 < g.genome_len ? (uint32_t)ge64 : g.genome_len);
 }
 
-// best-per-read key (64-bit atomicMax; 0 = none): higher score, then smaller hit index -- both paths' tie rule
-__device__ __forceinline__ unsigned long long make_best_key(int32_t score, uint32_t index)
-{
-    return ((unsigned long long)((uint32_t)score ^ 0x80000000u) << 32) | (unsigned long long)(0xFFFFFFFFu - index);
-}
-__device__ __forceinline__ int32_t  best_key_score(unsigned long long key) { return (int32_t)((uint32_t)(key >> 32) ^ 0x80000000u); }
-__device__ __forceinline__ uint32_t best_key_index(unsigned long long key) { return 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull); }
-
-// a scored job is an alignment unless the DP reported it empty (window shorter than the read: NVB_SINK_MIN, sink 0xFFFFFFFF) -- a read
-// running more than band/2 symbols past the genome's end gets such a window; it never becomes a best, second-best or pair candidate
-__device__ __forceinline__ bool job_aligned(uint2 sink) { return sink.x != 0xFFFFFFFFu; }
-
 // one thread per (string, seed slot): SA range of the seed, and its clamped size (sizes == NULL on the per-read path, which sums the
 // sizes of a read's ranges itself).
 // genome != NULL (the per-read path on an index with the full suffix array): single-row ranges are located on the spot --
@@ -709,6 +697,71 @@ debug_mapq_eval_kernel(const int32_t* __restrict__ best, const uint8_t* __restri
 }
 
 // ---------------------------------------------------------------------------------------------
+// up to k distinct alignments per read (nvb_seed_extend_all).  pair_cand_scatter_kernel gathers every read's reportable candidates into a
+// segment of their own (best_order), a segmented sort orders each by make_best_key, descending; all_select_kernel walks the segments
+// (select_distinct), the exclusive scan of its counts is d_first, and all_emit_kernel writes the stored alignments and their traceback
+// jobs, which are traced in slices of n_reads.
+// ---------------------------------------------------------------------------------------------
+
+// one thread per read: its sorted segment as end_strand (es, over the sorted keys), then select_distinct in place; cnt[r] = the read's
+// alignments, their candidate indices at idx[seg[r] ..]
+__global__ void __launch_bounds__(256)
+all_select_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict__ str_len, const uint32_t* __restrict__ seg,
+                  unsigned long long* __restrict__ es, uint32_t* __restrict__ idx, const uint32_t k, uint32_t* __restrict__ cnt)
+{
+    const uint32_t r = blockIdx.x * 256 + threadIdx.x;
+    if (r >= g.n_reads) return;
+    const uint32_t b = seg[r], n = seg[r + 1] - b;
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t j = idx[b + i];
+        es[b + i] = end_strand(c.end(j), c.string[j] % g.strands);
+    }
+    cnt[r] = select_distinct(es + b, idx + b, n, str_len[r * g.strands], k);
+}
+
+// count = (alignments stored, wanted): the stored reads are the prefix with first[r + 1] <= capacity.  slice_n[t] = the stored alignments
+// of traceback slice t, [t * n_reads, (t + 1) * n_reads)
+__global__ void __launch_bounds__(256)
+all_count_kernel(const uint32_t n_reads, const uint32_t* __restrict__ first, const uint32_t capacity, const uint32_t n_slices,
+                 uint32_t* __restrict__ count, uint32_t* __restrict__ slice_n)
+{
+    const uint32_t stored = first[upper_bound_u32(first, n_reads + 1u, capacity) - 1u];   // first[0] = 0 <= capacity
+    const uint32_t t = blockIdx.x * 256 + threadIdx.x;
+    if (t == 0) { count[0] = stored; count[1] = first[n_reads]; }
+    if (t >= n_slices) return;
+    const uint64_t b = (uint64_t)t * n_reads;
+    slice_n[t] = stored > b ? (uint32_t)(stored - b < n_reads ? stored - b : n_reads) : 0u;
+}
+
+// one thread per read whose alignments fit: alignment first[r] + i is its candidate idx[seg[r] + i]; its traceback job into `jobs`
+__global__ void __launch_bounds__(256)
+all_emit_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict__ first, const uint32_t* __restrict__ seg,
+                const uint32_t* __restrict__ idx, const uint32_t capacity, uint32_t* __restrict__ out_read, int32_t* __restrict__ out_score,
+                uint32_t* __restrict__ out_pos, uint8_t* __restrict__ out_strand, const Jobs jobs)
+{
+    const uint32_t r = blockIdx.x * 256 + threadIdx.x;
+    if (r >= g.n_reads) return;
+    const uint32_t o = first[r], e = first[r + 1];
+    if (e > capacity) return;
+    const uint32_t* sel = idx + seg[r];
+    for (uint32_t a = o; a < e; ++a) {
+        const uint32_t j = sel[a - o], s = c.string[j];
+        out_read[a] = r; out_score[a] = c.score[j]; out_pos[a] = c.end(j); out_strand[a] = (uint8_t)(s % g.strands);
+        jobs.p_off[a] = c.jobs.p_off[j]; jobs.p_len[a] = c.jobs.p_len[j]; jobs.t_off[a] = c.jobs.t_off[j]; jobs.t_len[a] = c.jobs.t_len[j];
+    }
+}
+
+// source cell (window-relative text start, read start) -> begin of the first *n alignments of a traceback slice
+__global__ void __launch_bounds__(256)
+all_begin_kernel(const uint32_t* __restrict__ n, const uint32_t* __restrict__ t_off, const uint2* __restrict__ source, uint2* __restrict__ begin)
+{
+    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= *n) return;
+    const uint2 sc = source[i];
+    begin[i] = make_uint2(t_off[i] + sc.x, sc.y);
+}
+
+// ---------------------------------------------------------------------------------------------
 // paired-end stage (see nvb_seed_extend_paired in the header for the rules)
 // ---------------------------------------------------------------------------------------------
 struct MateBest { bool has; int32_t score; uint32_t strand, beg, end, len; };
@@ -872,19 +925,20 @@ pair_rescue_items_kernel(const uint32_t n_pairs, const uint32_t* __restrict__ pa
 // (strand, end); pair_second_kernel pairs them up (pair_combinations, pipeline_core.cuh) and adds the pair's rescues.
 // ---------------------------------------------------------------------------------------------
 
-// candidates per read (counts) or their place in the read's segment (seg != NULL: cursor = counts zeroed, key = (strand << 32) | end)
+// reportable candidates per read (counts) or their place in the read's segment (seg != NULL: cursor = counts zeroed, key = (strand << 32)
+// | end, or make_best_key when best_order: nvb_seed_extend_all)
 __global__ void __launch_bounds__(256)
 pair_cand_scatter_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict__ str_len, const int32_t* __restrict__ min_score,
                          const uint32_t* __restrict__ seg, uint32_t* __restrict__ cursor, unsigned long long* __restrict__ key,
-                         uint32_t* __restrict__ val)
+                         uint32_t* __restrict__ val, const bool best_order)
 {
     const uint32_t n = *c.count;
     for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
         const uint32_t s = c.string[j], read = s / g.strands;
-        if (!job_aligned(c.sink[j]) || c.score[j] < min_score[str_len[s]]) continue;
+        if (!reportable(c.score[j], c.sink[j], min_score[str_len[s]])) continue;
         const uint32_t slot = atomicAdd(cursor + read, 1u);
         if (!seg) continue;
-        key[seg[read] + slot] = ((unsigned long long)(s % g.strands) << 32) | c.end(j);
+        key[seg[read] + slot] = best_order ? make_best_key(c.score[j], c.tie(j)) : ((unsigned long long)(s % g.strands) << 32) | c.end(j);
         val[seg[read] + slot] = j;
     }
 }
@@ -1049,6 +1103,9 @@ struct PipeCall {
     unsigned long long* second_key;                                        // second-best alignment of every read (MO)
     uint32_t *pc_cnt, *pc_seg, *pc_fw, *pc_n, *pc_val[2], *pc_end, *pc_tie, *se_pos;     // paired MAPQ (PMO): candidate segments per read
     unsigned long long* pc_key[2]; int32_t* pc_score; char *pc_scan_tmp, *pc_sort_tmp; size_t pc_scan_bytes, pc_sort_bytes;
+    const nvb_all_params* AP; const nvb_all_out* AO;                        // nvb_seed_extend_all: candidate segments, their sort, jobs
+    uint32_t *al_cnt, *al_seg, *al_val[2], *al_slice_n, n_slices; unsigned long long* al_key[2]; Jobs al_jobs;
+    char *al_scan_tmp, *al_sort_tmp; size_t al_scan_bytes, al_sort_bytes;
 
     int stage(int i) const { return (int)cudaEventRecord(SE->ev[i], s); }    // boundary i of nvb_seed_extend_stage_ms
 
@@ -1108,11 +1165,11 @@ struct PipeCall {
         }
         scan_tmp  = tc.take<char>(scan_bytes);
         gotoh_tmp = tc.take<char>(gotoh_bytes);
-        if (BA) {
-            best = take_jobs(tc, n_reads);
+        if (BA || AO) {                                              // nvb_seed_extend_all: one slice of n_reads alignments at a time
+            if (BA) best = take_jobs(tc, n_reads);
             b_score = tc.take<int32_t>(n_reads); b_sink = tc.take<uint2>(n_reads); b_source = tc.take<uint2>(n_reads);
-            NVB_TRY(size_only(nvb_banded_gotoh_traceback(g.band, P->type, &P->scheme, &sv.pats, nullptr, &sv.txts, n_reads,
-                                                         nullptr, nullptr, nullptr, nullptr, BA->max_ops, nullptr, nullptr, &tb_bytes, s)));
+            NVB_TRY(size_only(nvb_banded_gotoh_traceback(g.band, P->type, &P->scheme, &sv.pats, nullptr, &sv.txts, n_reads, nullptr, nullptr,
+                                                         nullptr, nullptr, BA ? BA->max_ops : AO->alignment.max_ops, nullptr, nullptr, &tb_bytes, s)));
             tb_tmp = tc.take<char>(tb_bytes);
         }
         if (PP) {
@@ -1144,6 +1201,19 @@ struct PipeCall {
             if (cap) NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairs(nullptr, pc_sort_bytes, pc_key[0], pc_key[1], pc_val[0], pc_val[1], (int)cap,
                                                                      (int)n_reads, pc_seg, pc_seg + 1, s));
             pc_sort_tmp = tc.take<char>(pc_sort_bytes);
+        }
+        if (AO) {
+            const uint32_t acap = AP->capacity;
+            n_slices = n_reads ? (uint32_t)(((uint64_t)acap + n_reads - 1u) / n_reads) : 0u;
+            al_cnt = tc.take<uint32_t>((size_t)n_reads + 1); al_seg = tc.take<uint32_t>((size_t)n_reads + 1);
+            for (int k = 0; k < 2; ++k) { al_key[k] = tc.take<unsigned long long>(cap); al_val[k] = tc.take<uint32_t>(cap); }
+            al_jobs = take_jobs(tc, acap); al_slice_n = tc.take<uint32_t>((size_t)n_slices + 1);
+            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, al_scan_bytes, al_cnt, al_seg, (int)n_reads + 1, s));
+            al_scan_tmp = tc.take<char>(al_scan_bytes);
+            al_sort_bytes = 0;
+            if (cap) NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairsDescending(nullptr, al_sort_bytes, al_key[0], al_key[1], al_val[0], al_val[1],
+                                                                               (int)cap, (int)n_reads, al_seg, al_seg + 1, s));
+            al_sort_tmp = tc.take<char>(al_sort_bytes);
         }
         need = tc.total();
         return NVB_OK;
@@ -1321,12 +1391,12 @@ struct PipeCall {
         NVB_CUDA_TRY(cudaMemsetAsync(pc_cnt, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
         if (cap) {
             const uint32_t grid = resident_grid(cap);
-            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, nullptr, pc_cnt, nullptr, nullptr);
+            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, nullptr, pc_cnt, nullptr, nullptr, false);
             NVB_LAUNCH_CHECK();
             size_t bytes = pc_scan_bytes;
             NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(pc_scan_tmp, bytes, pc_cnt, pc_seg, (int)n_reads + 1, s));
             NVB_CUDA_TRY(cudaMemsetAsync(pc_cnt, 0, sizeof(uint32_t) * n_reads, s));
-            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, pc_seg, pc_cnt, pc_key[0], pc_val[0]);
+            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, pc_seg, pc_cnt, pc_key[0], pc_val[0], false);
             NVB_LAUNCH_CHECK();
             bytes = pc_sort_bytes;
             NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairs(pc_sort_tmp, bytes, pc_key[0], pc_key[1], pc_val[0], pc_val[1], (int)cap, (int)n_reads,
@@ -1335,6 +1405,54 @@ struct PipeCall {
             NVB_CUDA_TRY(cudaMemsetAsync(pc_seg, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
         pair_cand_merge_kernel<<<(n_reads + 255) / 256, 256, 0, s>>>(n_reads, pc_seg, pc_cnt, pc_key[1], pc_val[1], scored(), pc_end, pc_score,
                                                                       pc_tie, pc_fw, pc_n);
+        return launched();
+    }
+
+    // up to k distinct alignments of every read (after second_best: the same candidates), each traced; no host round trip
+    int all_alignments() const
+    {
+        const uint32_t cap = hit_capacity, n_reads = g.n_reads, acap = AP->capacity, rgrid = (n_reads + 255) / 256;
+        const nvb_all_out& O = *AO;
+        NVB_CUDA_TRY(cudaMemsetAsync(al_cnt, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
+        if (cap) {
+            const uint32_t grid = resident_grid(cap);
+            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, nullptr, al_cnt, nullptr, nullptr, true);
+            NVB_LAUNCH_CHECK();
+            size_t bytes = al_scan_bytes;
+            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(al_scan_tmp, bytes, al_cnt, al_seg, (int)n_reads + 1, s));
+            NVB_CUDA_TRY(cudaMemsetAsync(al_cnt, 0, sizeof(uint32_t) * n_reads, s));
+            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, al_seg, al_cnt, al_key[0], al_val[0], true);
+            NVB_LAUNCH_CHECK();
+            bytes = al_sort_bytes;
+            NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairsDescending(al_sort_tmp, bytes, al_key[0], al_key[1], al_val[0], al_val[1], (int)cap,
+                                                                       (int)n_reads, al_seg, al_seg + 1, s));
+        } else
+            NVB_CUDA_TRY(cudaMemsetAsync(al_seg, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
+        // al_cnt[n_reads] stays 0: the scan's extra element makes d_first[n_reads] the total
+        all_select_kernel<<<rgrid, 256, 0, s>>>(g, scored(), str_len, al_seg, al_key[1], al_val[1], AP->max_per_read, al_cnt);
+        NVB_LAUNCH_CHECK();
+        size_t bytes = al_scan_bytes;
+        NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(al_scan_tmp, bytes, al_cnt, O.d_first, (int)n_reads + 1, s));
+        all_count_kernel<<<(n_slices + 256) / 256, 256, 0, s>>>(n_reads, O.d_first, acap, n_slices, O.d_count, al_slice_n);
+        NVB_LAUNCH_CHECK();
+        if (!acap) return launched();
+        all_emit_kernel<<<rgrid, 256, 0, s>>>(g, scored(), O.d_first, al_seg, al_val[1], acap, O.d_read, O.d_score, O.d_pos, O.alignment.d_strand,
+                                              al_jobs);
+        NVB_LAUNCH_CHECK();
+        // slice t: alignments [t * n_reads, + n) traced like the best alignments of nvb_seed_extend_traceback (its direction matrices, sized
+        // for n_reads); the count of each slice lives on the device, a slice past the stored alignments launches only empty CTAs
+        const nvb_best_alignment_out& A = O.alignment;
+        for (uint32_t t = 0; t < n_slices; ++t) {
+            const size_t b = (size_t)t * n_reads;
+            const uint32_t n = (uint32_t)(acap - b < n_reads ? acap - b : n_reads);
+            const Jobs j{al_jobs.p_off + b, al_jobs.p_len + b, al_jobs.t_off + b, al_jobs.t_len + b};
+            const JobViews v = job_views(j, rd.length + g.band);
+            size_t tb = tb_bytes;
+            NVB_TRY(banded_traceback(g.band, P->type, &P->scheme, &v.pats, str_quals, &v.txts, al_slice_n + t, n, b_score, (nvb_uint2*)b_sink,
+                                     (nvb_uint2*)b_source, A.d_ops + b * A.max_ops, A.max_ops, A.d_n_ops + b, tb_tmp, &tb, s));
+            all_begin_kernel<<<(n + 255) / 256, 256, 0, s>>>(al_slice_n + t, j.t_off, b_source, (uint2*)A.d_begin + b);
+            NVB_LAUNCH_CHECK();
+        }
         return launched();
     }
 
@@ -1406,7 +1524,7 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     const nvb_best_alignment_out* BA,
                     const nvb_pair_params* PP, const nvb_pair_out* PO,
                     const nvb_mapq_params* MP, const nvb_mapq_out* MO, const nvb_pair_mapq_out* PMO,
-                    void* d_temp, size_t* temp_bytes, void* stream)
+                    void* d_temp, size_t* temp_bytes, void* stream, const nvb_all_params* AP = nullptr, const nvb_all_out* AO = nullptr)
 {
     // The entry points check only what cannot be seen here: that the structs they require are there, and the pair count before
     // 2 * n_pairs is formed.  The order below decides which code a call with several faults gets: the paired traceback's read length
@@ -1418,6 +1536,7 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     if (MO && (!MO->d_second_score || !MO->d_mapq)) return NVB_E_INVALID;
     if (PMO && (!PMO->d_second_pair_score || !PMO->d_mate_mapq)) return NVB_E_INVALID;
     if (PP && BA && reads->length > FULL_TB_MAX_M) return NVB_E_UNSUPPORTED;                 // nvBowtie's MAXIMUM_READ_LENGTH
+    if (AO && reads->length > FULL_TB_MAX_M) return NVB_E_UNSUPPORTED;
     if (PP) {
         if (!PO->d_pair_score || !PO->d_pair_flags || !PO->d_mate_score || !PO->d_mate_pos || !PO->d_mate_strand) return NVB_E_INVALID;
         if (!P || !P->both_strands || (n_reads & 1u) || PP->max_frag == 0 || PP->min_frag > PP->max_frag) return NVB_E_INVALID;
@@ -1447,6 +1566,7 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     const cudaStream_t s = c.s = as_stream(stream);
     c.P = P; c.f = make_fmindex(fmi); c.rd = make_strset(reads); c.genome = d_genome; c.nq = (uint32_t)nq64; c.hit_capacity = hit_capacity;
     c.best_score = d_best_score; c.best_pos = d_best_pos; c.hit_score = d_hit_score; c.hit_sink = d_hit_sink; c.BA = BA; c.PP = PP; c.PO = PO; c.MP = MP; c.MO = MO;
+    c.AP = AP; c.AO = AO;
     if (PMO) {                                 // the single-end second best and MAPQ of every mate (mate_mapq: overwritten for paired pairs)
         c.PMO = PMO;
         c.se_mo.d_second_score = PMO->d_mate_second_score; c.se_mo.d_mapq = PMO->d_mate_mapq;
@@ -1462,7 +1582,13 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     size_t need = 0;
     NVB_TRY(c.carve(d_temp, need));
     if (!d_temp || *temp_bytes < need) { *temp_bytes = need; return NVB_E_TEMP_SIZE; }
-    if (n_reads == 0) return NVB_OK;
+    if (n_reads == 0) {
+        if (AO) {
+            NVB_CUDA_TRY(cudaMemsetAsync(AO->d_first, 0, sizeof(uint32_t), s));
+            NVB_CUDA_TRY(cudaMemsetAsync(AO->d_count, 0, 2 * sizeof(uint32_t), s));
+        }
+        return NVB_OK;
+    }
 
     NVB_TRY(default_stage_events(&c.SE));
     NVB_TRY(c.stage(0));
@@ -1483,6 +1609,7 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     }
     if (BA && !PP) NVB_TRY(c.best_traceback());
     if (c.MO) NVB_TRY(c.second_best());
+    if (AO) NVB_TRY(c.all_alignments());
     if (PMO) NVB_TRY(c.pair_candidates());
     if (PP) NVB_TRY(c.paired_rescue());
     if (BA && PP) { NVB_TRY(c.best_traceback()); NVB_TRY(c.rescue_traceback()); }
@@ -1556,6 +1683,27 @@ extern "C" int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_g
     if (!mapq || !mapq_out) return NVB_E_INVALID;
     return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
                             d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, mapq, mapq_out, nullptr, d_temp, temp_bytes, stream);
+}
+
+extern "C" int nvb_seed_extend_all(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_reads,
+                    const nvb_seed_extend_params* P, uint32_t hit_capacity,
+                    int32_t* d_best_score, uint32_t* d_best_pos,
+                    uint32_t* d_n_hits, uint32_t* d_hit_read, nvb_uint2* d_hit_window,
+                    int32_t* d_hit_score, nvb_uint2* d_hit_sink,
+                    const nvb_best_alignment_out* best_alignment,
+                    const nvb_mapq_params* mapq, const nvb_mapq_out* mapq_out,
+                    const nvb_all_params* all_params, const nvb_all_out* all_out,
+                    void* d_temp, size_t* temp_bytes, void* stream)
+{
+    if (!mapq || !mapq_out || !all_params || !all_out || best_alignment) return NVB_E_INVALID;
+    const nvb_all_out& O = *all_out;
+    const nvb_best_alignment_out& A = O.alignment;
+    if (!O.d_first || !O.d_read || !O.d_score || !O.d_pos || !O.d_count || !A.d_ops || !A.d_n_ops || !A.d_begin || !A.d_strand || A.max_ops == 0)
+        return NVB_E_INVALID;
+    return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
+                            d_hit_score, d_hit_sink, nullptr, nullptr, nullptr, mapq, mapq_out, nullptr, d_temp, temp_bytes, stream,
+                            all_params, all_out);
 }
 
 extern "C" int nvb_seed_extend_paired_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,

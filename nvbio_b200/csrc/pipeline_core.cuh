@@ -173,6 +173,44 @@ __host__ __device__ __forceinline__ bool distinct_alignment(uint32_t p, uint32_t
     return t != bt || p < bp - (bp < d ? bp : d) || p > bp + d;
 }
 
+// best-per-read key (64-bit atomicMax; 0 = none): higher score, then smaller tie index -- both paths' tie rule
+__host__ __device__ __forceinline__ unsigned long long make_best_key(int32_t score, uint32_t index)
+{
+    return ((unsigned long long)((uint32_t)score ^ 0x80000000u) << 32) | (unsigned long long)(0xFFFFFFFFu - index);
+}
+__host__ __device__ __forceinline__ int32_t  best_key_score(unsigned long long key) { return (int32_t)((uint32_t)(key >> 32) ^ 0x80000000u); }
+__host__ __device__ __forceinline__ uint32_t best_key_index(unsigned long long key) { return 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull); }
+
+// a scored job is an alignment unless the DP reported it empty (window shorter than the read: NVB_SINK_MIN, sink 0xFFFFFFFF) -- a read
+// running more than band/2 symbols past the genome's end gets such a window; it never becomes a best, second-best or pair candidate
+__host__ __device__ __forceinline__ bool job_aligned(uint2 sink) { return sink.x != 0xFFFFFFFFu; }
+
+// a scored job that may be reported beside the best alignment: aligned and reaching the read's min score (the candidates of the paired
+// MAPQ and of nvb_seed_extend_all)
+__host__ __device__ __forceinline__ bool reportable(int32_t score, uint2 sink, int32_t min_score) { return job_aligned(sink) && score >= min_score; }
+
+// (end, strand) of a candidate packed for select_distinct
+__host__ __device__ __forceinline__ unsigned long long end_strand(uint32_t end, uint32_t strand) { return ((unsigned long long)end << 1) | (strand & 1u); }
+
+// Selection rule of nvb_seed_extend_all for one read of length len: es / idx hold its reportable candidates in descending make_best_key
+// order as end_strand / candidate index.  Walk them in that order and admit a candidate when it is distinct_alignment (candidate first,
+// admitted alignment second) from every one admitted before; stop after k admissions (k = 0: none).  The admitted ones are compacted in
+// place to the front of es / idx (entry m is written only after entry i >= m was read); returns their number.
+__host__ __device__ inline uint32_t select_distinct(unsigned long long* es, uint32_t* idx, uint32_t n, uint32_t len, uint32_t k)
+{
+    uint32_t m = 0;
+    for (uint32_t i = 0; i < n && (k == 0u || m < k); ++i) {
+        const unsigned long long c = es[i];
+        const uint32_t p = (uint32_t)(c >> 1), t = (uint32_t)(c & 1u);
+        bool ok = true;
+        for (uint32_t a = 0; a < m && ok; ++a) ok = distinct_alignment(p, t, (uint32_t)(es[a] >> 1), (uint32_t)(es[a] & 1u), len);
+        if (!ok) continue;
+        const uint32_t j = idx[i];
+        es[m] = c; idx[m] = j; ++m;
+    }
+    return m;
+}
+
 // begin of an alignment ending at `end` of a read of length len: end - len, clamped at 0 (no traceback: soft clips and indels ignored)
 __host__ __device__ __forceinline__ uint32_t aln_begin(uint32_t end, uint32_t len) { return end > len ? end - len : 0u; }
 

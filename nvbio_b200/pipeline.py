@@ -6,7 +6,7 @@ from typing import Optional
 import torch
 import numpy as np
 from ._lib import (lib, check, SeedExtendParamsStruct, BestAlignmentOutStruct, PairParamsStruct, PairOutStruct, MapqParamsStruct, MapqOutStruct,
-                   PairMapqOutStruct)
+                   PairMapqOutStruct, AllParamsStruct, AllOutStruct)
 from .strings import PackedStringSet
 from .fmindex import FMIndexDevice
 from . import aln
@@ -194,6 +194,113 @@ def seed_extend(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStringSet
     tb = C.c_size_t(workspace.temp_bytes)
     check(_call(fmi, genome, reads, params, workspace, workspace.temp, tb), "nvb_seed_extend")
     return workspace
+
+
+def _storage_ptr(t):
+    """the address of t's first element, also for an empty view of a non-empty allocation (whose data_ptr() is 0)"""
+    return t.untyped_storage().data_ptr() + t.storage_offset() * t.element_size()
+
+
+class AllAlignments:
+    """Up to max_per_read distinct alignments of every read (nvb_seed_extend_all), each traced.  Per read (n): .best_score, .best_pos,
+    .second_score, .second_pos, .second_strand, .mapq (those of seed_extend(mapq=...)), .first[n + 1] (read r's alignments are
+    [first[r], first[r + 1])) and .n_hits[3]; per alignment slot (capacity): .read, .score, .pos (end), .ops[., max_ops] (END->START),
+    .n_ops, .begin = (genome start, read start), .strand; .count = (stored, wanted).  Only the first count[0] slots are written."""
+
+    def __init__(self, fmi, genome, reads: PackedStringSet, params: SeedExtendParams, mapq: MapqParams, max_per_read: int, capacity: int,
+                 hit_capacity: int):
+        dev = fmi.device
+        n = reads.count
+        self.n_reads, self.max_per_read, self.capacity, self.hit_capacity = n, int(max_per_read), int(capacity), int(hit_capacity)
+        self.mapq_params = mapq
+        per_read = lambda dt: torch.empty(max(n, 1), dtype=dt, device=dev)[:n]     # noqa: E731  (never a NULL pointer)
+        self.best_score, self.best_pos = per_read(torch.int32), per_read(torch.int32)
+        self.n_hits = torch.zeros(3, dtype=torch.int32, device=dev)
+        self.second_score, self.second_pos = per_read(torch.int32), per_read(torch.int32)
+        self.second_strand, self.mapq = per_read(torch.uint8), per_read(torch.uint8)
+        self.max_ops = 2 * reads.length + params.band_len             # (as SeedExtendWorkspace)
+        c = self.capacity
+        self.first = torch.empty(n + 1, dtype=torch.int32, device=dev)
+        self.read = torch.empty(c, dtype=torch.int32, device=dev)
+        self.score = torch.empty(c, dtype=torch.int32, device=dev)
+        self.pos = torch.empty(c, dtype=torch.int32, device=dev)
+        self.ops = torch.zeros((c, self.max_ops), dtype=torch.uint8, device=dev)
+        self.n_ops = torch.zeros(c, dtype=torch.int32, device=dev)
+        self.begin = torch.empty((c, 2), dtype=torch.int32, device=dev)
+        self.strand = torch.empty(c, dtype=torch.uint8, device=dev)
+        self.count = torch.zeros(2, dtype=torch.int32, device=dev)
+        tb = C.c_size_t(0)
+        r = self._call(fmi, genome, reads, params, None, tb)
+        if r != -2:
+            check(r, "nvb_seed_extend_all(size query)")
+        self.temp = torch.empty(tb.value, dtype=torch.uint8, device=dev)
+        self.temp_bytes = tb.value
+
+    def _call(self, fmi, genome, reads, params, temp, tb):
+        s, rd, ps, mp = fmi.struct(), reads.struct(), params.struct(), self.mapq_params.struct()
+        mo = MapqOutStruct()
+        mo.d_second_score, mo.d_second_pos = _storage_ptr(self.second_score), _storage_ptr(self.second_pos)
+        mo.d_second_strand, mo.d_mapq = _storage_ptr(self.second_strand), _storage_ptr(self.mapq)
+        ap = AllParamsStruct()
+        ap.max_per_read, ap.capacity = self.max_per_read, self.capacity
+        ao = AllOutStruct()
+        ao.d_first, ao.d_read, ao.d_score, ao.d_pos = self.first.data_ptr(), self.read.data_ptr(), self.score.data_ptr(), self.pos.data_ptr()
+        ao.alignment.d_ops, ao.alignment.max_ops, ao.alignment.d_n_ops = self.ops.data_ptr(), self.max_ops, self.n_ops.data_ptr()
+        ao.alignment.d_begin, ao.alignment.d_strand = self.begin.data_ptr(), self.strand.data_ptr()
+        ao.d_count = self.count.data_ptr()
+        return lib().nvb_seed_extend_all(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(reads.count), C.byref(ps), C.c_uint32(self.hit_capacity),
+                                         C.c_void_p(_storage_ptr(self.best_score)), C.c_void_p(_storage_ptr(self.best_pos)), _p(self.n_hits),
+                                         None, None, None, None, None,
+                                         C.byref(mp), C.byref(mo), C.byref(ap), C.byref(ao), _p(temp), C.byref(tb),
+                                         C.c_void_p(torch.cuda.current_stream().cuda_stream))
+
+    def run(self, fmi, genome, reads, params):
+        tb = C.c_size_t(self.temp_bytes)
+        check(self._call(fmi, genome, reads, params, self.temp, tb), "nvb_seed_extend_all")
+        return self
+
+    def strings(self, reads: PackedStringSet) -> PackedStringSet:
+        """the reads of the capacity alignment slots as a string set over the reads' own words (string i = read read[i]; slots past
+        count[0] point at read 0): the `reads` of finish_alignments over these alignments"""
+        n = reads.count
+        idx = self.read.long().clamp(0, max(n - 1, 0))
+        if int(self.count[0]) < self.capacity:
+            idx = torch.where(torch.arange(self.capacity, device=idx.device) < self.count[0], idx, torch.zeros_like(idx))
+        if reads.offsets is not None:
+            offsets = reads.offsets[idx] if n else torch.zeros(self.capacity, dtype=torch.int32, device=idx.device)
+        else:
+            offsets = (idx * reads.stride).to(torch.int32)
+        lengths = reads.lengths[idx] if reads.lengths is not None and n else torch.full((self.capacity,), reads.length, dtype=torch.int32,
+                                                                                          device=idx.device)
+        return PackedStringSet(words=reads.words, bits=reads.bits, big_endian=reads.big_endian, offsets=offsets.contiguous(),
+                               lengths=lengths.contiguous(), stride=0, length=reads.length, count=self.capacity)
+
+
+    def bam_records(self, genome: torch.Tensor, genome_len: int, reads: PackedStringSet, contigs, names, quals: Optional[torch.Tensor] = None,
+                    capacity: Optional[int] = None):
+        """finish_alignments over the alignment slots, then their BAM records (bam_records_all: primary, secondary and unmapped records,
+        NH); the returned BamRecords is what write_sorted_bam / bgzf_compress take"""
+        from .finish import finish_alignments
+        from .bam import bam_records_all
+        f = finish_alignments(genome, self.strings(reads), self.ops, self.n_ops, self.begin, self.strand, genome_len=genome_len)
+        return bam_records_all(self, f, reads, contigs, names, quals=quals, capacity=capacity)
+
+
+def seed_extend_all(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStringSet, params: SeedExtendParams, mapq: MapqParams,
+                    max_per_read: int, capacity: Optional[int] = None, hit_capacity: Optional[int] = None,
+                    workspace: Optional[AllAlignments] = None) -> AllAlignments:
+    """up to max_per_read distinct alignments of every read (0 = every distinct alignment: nvBowtie's --all), traced, with the
+    best / second-best / MAPQ outputs of seed_extend(mapq=...).  capacity: alignment slots, by default max_per_read * n_reads + 1024
+    (16 per read for max_per_read = 0), at most hit_capacity; .count[1] > .count[0] tells that reads were left out.  The call traces in
+    ceil(capacity / n_reads) slices of n_reads, each a few kernel launches even when empty, so a capacity far above the alignments
+    expected costs launches.  A workspace of an equally-shaped earlier call is reused as it is"""
+    if workspace is None:
+        if hit_capacity is None:
+            hit_capacity = 32 * reads.count + 1024
+        if capacity is None:
+            capacity = min((int(max_per_read) or 16) * reads.count + 1024, hit_capacity)
+        workspace = AllAlignments(fmi, genome, reads, params, mapq, max_per_read, capacity, hit_capacity)
+    return workspace.run(fmi, genome, reads, params)
 
 
 PAIR_UNPAIRED, PAIR_CONCORDANT, PAIR_RESCUED_MATE1, PAIR_RESCUED_MATE2 = 0, 1, 2, 4
