@@ -616,16 +616,17 @@ pipe_winner_kernel(const PipeGeom g, const Scored c, const unsigned long long* _
     }
 }
 
-// source cell (window-relative text start, read start) -> (genome coordinate, read start); reads without a hit: n_ops 0
+// source cell (window-relative text start, read start) -> (genome coordinate, read start) of the first n traced jobs (d_n != NULL:
+// *d_n).  best_key != NULL: job r is read r's best, and a read without a hit gets n_ops 0
 __global__ void __launch_bounds__(256)
-pipe_best_begin_kernel(const PipeGeom g, const unsigned long long* __restrict__ best_key, const uint32_t* __restrict__ bt_off,
-                       const uint2* __restrict__ source, uint32_t* __restrict__ n_ops, uint2* __restrict__ begin)
+traceback_begin_kernel(const uint32_t* __restrict__ d_n, const uint32_t n, const unsigned long long* __restrict__ best_key,
+                       const uint32_t* __restrict__ t_off, const uint2* __restrict__ source, uint32_t* __restrict__ n_ops, uint2* __restrict__ begin)
 {
-    const uint32_t r = blockIdx.x * 256 + threadIdx.x;
-    if (r >= g.n_reads) return;
-    if (best_key[r] == 0ull) { n_ops[r] = 0; begin[r] = make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu); return; }
-    const uint2 sc = source[r];
-    begin[r] = make_uint2(bt_off[r] + sc.x, sc.y);
+    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= (d_n ? *d_n : n)) return;
+    if (best_key && best_key[i] == 0ull) { n_ops[i] = 0; begin[i] = make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu); return; }
+    const uint2 sc = source[i];
+    begin[i] = make_uint2(t_off[i] + sc.x, sc.y);
 }
 
 __global__ void __launch_bounds__(256)
@@ -696,11 +697,29 @@ debug_mapq_eval_kernel(const int32_t* __restrict__ best, const uint8_t* __restri
     mapq[i] = (uint8_t)bowtie_mapq2(best[i], has_second[i] != 0, second[i], (int32_t)len[i] * match_bonus[i], min_score[i], match_bonus[i] == 0);
 }
 
+// candidate segments of the paired MAPQ and of nvb_seed_extend_all (PipeCall::cand_segments): reportable candidates per read (counts) or
+// their place in the read's segment (seg != NULL: cursor = counts zeroed, key = (strand << 32) | end, or ~make_best_key when by_best:
+// ascending keys are then nvb_seed_extend_all's rank order)
+__global__ void __launch_bounds__(256)
+cand_scatter_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict__ str_len, const int32_t* __restrict__ min_score,
+                    const uint32_t* __restrict__ seg, uint32_t* __restrict__ cursor, unsigned long long* __restrict__ key,
+                    uint32_t* __restrict__ val, const bool by_best)
+{
+    const uint32_t n = *c.count;
+    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
+        const uint32_t s = c.string[j], read = s / g.strands;
+        if (!reportable(c.score[j], c.sink[j], min_score[str_len[s]])) continue;
+        const uint32_t slot = atomicAdd(cursor + read, 1u);
+        if (!seg) continue;
+        key[seg[read] + slot] = by_best ? ~make_best_key(c.score[j], c.tie(j)) : ((unsigned long long)(s % g.strands) << 32) | c.end(j);
+        val[seg[read] + slot] = j;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
-// up to k distinct alignments per read (nvb_seed_extend_all).  pair_cand_scatter_kernel gathers every read's reportable candidates into a
-// segment of their own (best_order), a segmented sort orders each by make_best_key, descending; all_select_kernel walks the segments
-// (select_distinct), the exclusive scan of its counts is d_first, and all_emit_kernel writes the stored alignments and their traceback
-// jobs, which are traced in slices of n_reads.
+// up to k distinct alignments per read (nvb_seed_extend_all).  The candidate segments in rank order (descending make_best_key);
+// all_select_kernel walks them (select_distinct), the exclusive scan of its counts is d_first, and all_emit_kernel writes the stored
+// alignments and their traceback jobs, which are traced in slices of n_reads.
 // ---------------------------------------------------------------------------------------------
 
 // one thread per read: its sorted segment as end_strand (es, over the sorted keys), then select_distinct in place; cnt[r] = the read's
@@ -749,16 +768,6 @@ all_emit_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict__ f
         out_read[a] = r; out_score[a] = c.score[j]; out_pos[a] = c.end(j); out_strand[a] = (uint8_t)(s % g.strands);
         jobs.p_off[a] = c.jobs.p_off[j]; jobs.p_len[a] = c.jobs.p_len[j]; jobs.t_off[a] = c.jobs.t_off[j]; jobs.t_len[a] = c.jobs.t_len[j];
     }
-}
-
-// source cell (window-relative text start, read start) -> begin of the first *n alignments of a traceback slice
-__global__ void __launch_bounds__(256)
-all_begin_kernel(const uint32_t* __restrict__ n, const uint32_t* __restrict__ t_off, const uint2* __restrict__ source, uint2* __restrict__ begin)
-{
-    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
-    if (i >= *n) return;
-    const uint2 sc = source[i];
-    begin[i] = make_uint2(t_off[i] + sc.x, sc.y);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -925,24 +934,6 @@ pair_rescue_items_kernel(const uint32_t n_pairs, const uint32_t* __restrict__ pa
 // (strand, end); pair_second_kernel pairs them up (pair_combinations, pipeline_core.cuh) and adds the pair's rescues.
 // ---------------------------------------------------------------------------------------------
 
-// reportable candidates per read (counts) or their place in the read's segment (seg != NULL: cursor = counts zeroed, key = (strand << 32)
-// | end, or make_best_key when best_order: nvb_seed_extend_all)
-__global__ void __launch_bounds__(256)
-pair_cand_scatter_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict__ str_len, const int32_t* __restrict__ min_score,
-                         const uint32_t* __restrict__ seg, uint32_t* __restrict__ cursor, unsigned long long* __restrict__ key,
-                         uint32_t* __restrict__ val, const bool best_order)
-{
-    const uint32_t n = *c.count;
-    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
-        const uint32_t s = c.string[j], read = s / g.strands;
-        if (!reportable(c.score[j], c.sink[j], min_score[str_len[s]])) continue;
-        const uint32_t slot = atomicAdd(cursor + read, 1u);
-        if (!seg) continue;
-        key[seg[read] + slot] = best_order ? make_best_key(c.score[j], c.tie(j)) : ((unsigned long long)(s % g.strands) << 32) | c.end(j);
-        val[seg[read] + slot] = j;
-    }
-}
-
 // one thread per read: its sorted segment merged per (strand, end) into the one with the highest (score, -tie), written to m_end / m_score
 // / m_tie from the segment's start; n_fw / n_merged = forward / all merged candidates
 __global__ void __launch_bounds__(256)
@@ -1075,15 +1066,22 @@ static uint32_t resident_grid(uint32_t n) { const uint32_t grid = (n + 255) / 25
 static Jobs take_jobs(TempCarver& tc, size_t n) { return Jobs{tc.take<uint32_t>(n), tc.take<uint32_t>(n), tc.take<uint32_t>(n), tc.take<uint32_t>(n)}; }
 struct JobViews { nvb_string_set pats, txts; };
 
-// one call: its inputs, the path it takes, its temp buffers (NULL in the size query and where the path does not use them), its stages
-struct PipeCall {
-    PipeGeom g; cudaStream_t s; const nvb_seed_extend_params* P; FmIndex f; StrSet rd; const uint32_t* genome;
-    uint32_t nq, hit_capacity;
-    bool dedup, per_read, eligible;                                         // eligible: the exact shortcut applies (gapless_job_shortcut)
-    bool seed_split;                                                        // the located seed match in two passes (match_seeds)
-    int32_t* best_score; uint32_t* best_pos; int32_t* hit_score; nvb_uint2* hit_sink;   // the caller's outputs (per-hit ones may be NULL)
+// one seed + extend call as an entry point states it: inputs, per-read and per-hit outputs (the per-hit ones may be NULL) and the
+// optional groups, NULL when not asked for: BA best-alignment traceback, PP / PO pairs, MP / MO MAPQ, PMO paired MAPQ, AP / AO k alignments
+struct SeedExtendReq {
+    const nvb_fm_index* fmi; const uint32_t* genome; const nvb_string_set* reads; uint32_t n_reads; const nvb_seed_extend_params* P; uint32_t hit_capacity;
+    int32_t* best_score; uint32_t* best_pos; uint32_t* n_hits; uint32_t* hit_read; nvb_uint2* hit_window; int32_t* hit_score; nvb_uint2* hit_sink;
     const nvb_best_alignment_out* BA; const nvb_pair_params* PP; const nvb_pair_out* PO;
     const nvb_mapq_params* MP; const nvb_mapq_out* MO; const nvb_pair_mapq_out* PMO;
+    const nvb_all_params* AP; const nvb_all_out* AO;
+};
+
+// one call: its request, the path it takes, its temp buffers (NULL in the size query and where the path does not use them), its stages
+struct PipeCall : SeedExtendReq {
+    PipeGeom g; cudaStream_t s; FmIndex f; StrSet rd;
+    uint32_t nq;
+    bool dedup, per_read, eligible;                                         // eligible: the exact shortcut applies (gapless_job_shortcut)
+    bool seed_split;                                                        // the located seed match in two passes (match_seeds)
     nvb_mapq_out se_mo;                                                     // paired MAPQ: the single-end stage's outputs (MO = &se_mo)
     StageEvents* SE;
     uint32_t *str_words, *str_len; uint8_t* str_quals;                      // [fw, rc] strings
@@ -1101,11 +1099,10 @@ struct PipeCall {
     Jobs rescue; int32_t* rs_score; uint2* rs_sink; char *pscan_tmp, *full_tmp; size_t pscan_bytes, full_bytes;
     uint2* rt_items; uint32_t* rt_count; char* rt_pool; size_t rt_pool_bytes;   // paired traceback (PP and BA): rescued mates, warp slot pool
     unsigned long long* second_key;                                        // second-best alignment of every read (MO)
-    uint32_t *pc_cnt, *pc_seg, *pc_fw, *pc_n, *pc_val[2], *pc_end, *pc_tie, *se_pos;     // paired MAPQ (PMO): candidate segments per read
-    unsigned long long* pc_key[2]; int32_t* pc_score; char *pc_scan_tmp, *pc_sort_tmp; size_t pc_scan_bytes, pc_sort_bytes;
-    const nvb_all_params* AP; const nvb_all_out* AO;                        // nvb_seed_extend_all: candidate segments, their sort, jobs
-    uint32_t *al_cnt, *al_seg, *al_val[2], *al_slice_n, n_slices; unsigned long long* al_key[2]; Jobs al_jobs;
-    char *al_scan_tmp, *al_sort_tmp; size_t al_scan_bytes, al_sort_bytes;
+    uint32_t *cs_cnt, *cs_seg, *cs_val[2]; unsigned long long* cs_key[2];  // candidate segments (PMO or AO), their scan and sort
+    char *cs_scan_tmp, *cs_sort_tmp; size_t cs_scan_bytes, cs_sort_bytes;
+    uint32_t *pc_fw, *pc_n, *pc_end, *pc_tie, *se_pos; int32_t* pc_score;   // paired MAPQ (PMO): merged candidates per read
+    uint32_t *al_slice_n, n_slices; Jobs al_jobs;                           // nvb_seed_extend_all: traceback slices, jobs
 
     int stage(int i) const { return (int)cudaEventRecord(SE->ev[i], s); }    // boundary i of nvb_seed_extend_stage_ms
 
@@ -1189,31 +1186,25 @@ struct PipeCall {
             }
         }
         if (MO) second_key = tc.take<unsigned long long>(n_reads);
+        if (PMO || AO) {
+            cs_cnt = tc.take<uint32_t>((size_t)n_reads + 1); cs_seg = tc.take<uint32_t>((size_t)n_reads + 1);
+            for (int k = 0; k < 2; ++k) { cs_key[k] = tc.take<unsigned long long>(cap); cs_val[k] = tc.take<uint32_t>(cap); }
+            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, cs_scan_bytes, cs_cnt, cs_seg, (int)n_reads + 1, s));
+            cs_scan_tmp = tc.take<char>(cs_scan_bytes);
+            cs_sort_bytes = 0;
+            if (cap) NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairs(nullptr, cs_sort_bytes, cs_key[0], cs_key[1], cs_val[0], cs_val[1], (int)cap,
+                                                                     (int)n_reads, cs_seg, cs_seg + 1, s));
+            cs_sort_tmp = tc.take<char>(cs_sort_bytes);
+        }
         if (PMO) {
             if (!PMO->d_mate_second_score) se_mo.d_second_score = tc.take<int32_t>(n_reads);
-            pc_cnt = tc.take<uint32_t>((size_t)n_reads + 1); pc_seg = tc.take<uint32_t>((size_t)n_reads + 1);
             pc_fw = tc.take<uint32_t>(n_reads); pc_n = tc.take<uint32_t>(n_reads); se_pos = tc.take<uint32_t>(n_reads);
-            for (int k = 0; k < 2; ++k) { pc_key[k] = tc.take<unsigned long long>(cap); pc_val[k] = tc.take<uint32_t>(cap); }
             pc_end = tc.take<uint32_t>(cap); pc_score = tc.take<int32_t>(cap); pc_tie = tc.take<uint32_t>(cap);
-            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, pc_scan_bytes, pc_cnt, pc_seg, (int)n_reads + 1, s));
-            pc_scan_tmp = tc.take<char>(pc_scan_bytes);
-            pc_sort_bytes = 0;
-            if (cap) NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairs(nullptr, pc_sort_bytes, pc_key[0], pc_key[1], pc_val[0], pc_val[1], (int)cap,
-                                                                     (int)n_reads, pc_seg, pc_seg + 1, s));
-            pc_sort_tmp = tc.take<char>(pc_sort_bytes);
         }
         if (AO) {
             const uint32_t acap = AP->capacity;
             n_slices = n_reads ? (uint32_t)(((uint64_t)acap + n_reads - 1u) / n_reads) : 0u;
-            al_cnt = tc.take<uint32_t>((size_t)n_reads + 1); al_seg = tc.take<uint32_t>((size_t)n_reads + 1);
-            for (int k = 0; k < 2; ++k) { al_key[k] = tc.take<unsigned long long>(cap); al_val[k] = tc.take<uint32_t>(cap); }
             al_jobs = take_jobs(tc, acap); al_slice_n = tc.take<uint32_t>((size_t)n_slices + 1);
-            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, al_scan_bytes, al_cnt, al_seg, (int)n_reads + 1, s));
-            al_scan_tmp = tc.take<char>(al_scan_bytes);
-            al_sort_bytes = 0;
-            if (cap) NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairsDescending(nullptr, al_sort_bytes, al_key[0], al_key[1], al_val[0], al_val[1],
-                                                                               (int)cap, (int)n_reads, al_seg, al_seg + 1, s));
-            al_sort_tmp = tc.take<char>(al_sort_bytes);
         }
         need = tc.total();
         return NVB_OK;
@@ -1350,11 +1341,18 @@ struct PipeCall {
             pair_empty_rescued_jobs_kernel<<<(n_pairs + 255) / 256, 256, 0, s>>>(n_pairs, PO->d_pair_flags, best.p_len, best.t_len);
             NVB_LAUNCH_CHECK();
         }
-        const JobViews v = job_views(best, rd.length + g.band);
+        return trace_jobs(best, nullptr, g.n_reads, *BA, 0, best_key);
+    }
+
+    // banded traceback of the first n jobs of a list (d_n != NULL: *d_n <= n of them) into alignments [off, off + n) of A, in the
+    // best-alignment traceback's temp buffers; best_key != NULL: job r is read r's best (see traceback_begin_kernel)
+    int trace_jobs(const Jobs& j, const uint32_t* d_n, uint32_t n, const nvb_best_alignment_out& A, size_t off, const unsigned long long* key) const
+    {
+        const JobViews v = job_views(j, rd.length + g.band);
         size_t bytes = tb_bytes;
-        NVB_TRY(nvb_banded_gotoh_traceback(g.band, P->type, &P->scheme, &v.pats, str_quals, &v.txts, g.n_reads, b_score, (nvb_uint2*)b_sink,
-                                           (nvb_uint2*)b_source, BA->d_ops, BA->max_ops, BA->d_n_ops, tb_tmp, &bytes, s));
-        pipe_best_begin_kernel<<<rgrid, 256, 0, s>>>(g, best_key, best.t_off, b_source, BA->d_n_ops, (uint2*)BA->d_begin);
+        NVB_TRY(banded_traceback(g.band, P->type, &P->scheme, &v.pats, str_quals, &v.txts, d_n, n, b_score, (nvb_uint2*)b_sink,
+                                 (nvb_uint2*)b_source, A.d_ops + off * A.max_ops, A.max_ops, A.d_n_ops + off, tb_tmp, &bytes, s));
+        traceback_begin_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_n, n, key, j.t_off, b_source, A.d_n_ops + off, (uint2*)A.d_begin + off);
         return launched();
     }
 
@@ -1382,76 +1380,64 @@ struct PipeCall {
         return launched();
     }
 
-    // paired MAPQ, before the rescue overwrites the mate arrays: every read's candidates (those second_best() sees that reach its min
-    // score) in a segment of their own, sorted by (strand, end) and merged per (strand, end); the single-end best ends (rescue anchors)
-    int pair_candidates() const
+    // every read's candidates (those second_best() sees that reach its min score) in a segment of their own, [cs_seg[r], + cs_cnt[r]),
+    // sorted by (strand, end) or, by_best, in rank order (descending make_best_key): keys in cs_key[1], candidates in cs_val[1];
+    // cs_cnt[n_reads] = 0
+    int cand_segments(bool by_best) const
     {
         const uint32_t cap = hit_capacity, n_reads = g.n_reads;
-        NVB_CUDA_TRY(cudaMemcpyAsync(se_pos, best_pos, sizeof(uint32_t) * n_reads, cudaMemcpyDeviceToDevice, s));
-        NVB_CUDA_TRY(cudaMemsetAsync(pc_cnt, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
+        NVB_CUDA_TRY(cudaMemsetAsync(cs_cnt, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
         if (cap) {
             const uint32_t grid = resident_grid(cap);
-            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, nullptr, pc_cnt, nullptr, nullptr, false);
+            cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, nullptr, cs_cnt, nullptr, nullptr, by_best);
             NVB_LAUNCH_CHECK();
-            size_t bytes = pc_scan_bytes;
-            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(pc_scan_tmp, bytes, pc_cnt, pc_seg, (int)n_reads + 1, s));
-            NVB_CUDA_TRY(cudaMemsetAsync(pc_cnt, 0, sizeof(uint32_t) * n_reads, s));
-            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, pc_seg, pc_cnt, pc_key[0], pc_val[0], false);
+            size_t bytes = cs_scan_bytes;
+            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(cs_scan_tmp, bytes, cs_cnt, cs_seg, (int)n_reads + 1, s));
+            NVB_CUDA_TRY(cudaMemsetAsync(cs_cnt, 0, sizeof(uint32_t) * n_reads, s));
+            cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, cs_seg, cs_cnt, cs_key[0], cs_val[0], by_best);
             NVB_LAUNCH_CHECK();
-            bytes = pc_sort_bytes;
-            NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairs(pc_sort_tmp, bytes, pc_key[0], pc_key[1], pc_val[0], pc_val[1], (int)cap, (int)n_reads,
-                                                             pc_seg, pc_seg + 1, s));
+            bytes = cs_sort_bytes;
+            NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairs(cs_sort_tmp, bytes, cs_key[0], cs_key[1], cs_val[0], cs_val[1], (int)cap, (int)n_reads,
+                                                             cs_seg, cs_seg + 1, s));
         } else
-            NVB_CUDA_TRY(cudaMemsetAsync(pc_seg, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
-        pair_cand_merge_kernel<<<(n_reads + 255) / 256, 256, 0, s>>>(n_reads, pc_seg, pc_cnt, pc_key[1], pc_val[1], scored(), pc_end, pc_score,
-                                                                      pc_tie, pc_fw, pc_n);
+            NVB_CUDA_TRY(cudaMemsetAsync(cs_seg, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
+        return NVB_OK;
+    }
+
+    // paired MAPQ, before the rescue overwrites the mate arrays: the candidate segments merged per (strand, end); the single-end best ends
+    // (rescue anchors)
+    int pair_candidates() const
+    {
+        NVB_CUDA_TRY(cudaMemcpyAsync(se_pos, best_pos, sizeof(uint32_t) * g.n_reads, cudaMemcpyDeviceToDevice, s));
+        NVB_TRY(cand_segments(false));
+        pair_cand_merge_kernel<<<(g.n_reads + 255) / 256, 256, 0, s>>>(g.n_reads, cs_seg, cs_cnt, cs_key[1], cs_val[1], scored(), pc_end, pc_score,
+                                                                        pc_tie, pc_fw, pc_n);
         return launched();
     }
 
     // up to k distinct alignments of every read (after second_best: the same candidates), each traced; no host round trip
     int all_alignments() const
     {
-        const uint32_t cap = hit_capacity, n_reads = g.n_reads, acap = AP->capacity, rgrid = (n_reads + 255) / 256;
+        const uint32_t n_reads = g.n_reads, acap = AP->capacity, rgrid = (n_reads + 255) / 256;
         const nvb_all_out& O = *AO;
-        NVB_CUDA_TRY(cudaMemsetAsync(al_cnt, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
-        if (cap) {
-            const uint32_t grid = resident_grid(cap);
-            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, nullptr, al_cnt, nullptr, nullptr, true);
-            NVB_LAUNCH_CHECK();
-            size_t bytes = al_scan_bytes;
-            NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(al_scan_tmp, bytes, al_cnt, al_seg, (int)n_reads + 1, s));
-            NVB_CUDA_TRY(cudaMemsetAsync(al_cnt, 0, sizeof(uint32_t) * n_reads, s));
-            pair_cand_scatter_kernel<<<grid, 256, 0, s>>>(g, scored(), str_len, MP->d_min_score, al_seg, al_cnt, al_key[0], al_val[0], true);
-            NVB_LAUNCH_CHECK();
-            bytes = al_sort_bytes;
-            NVB_CUDA_TRY(cub::DeviceSegmentedSort::SortPairsDescending(al_sort_tmp, bytes, al_key[0], al_key[1], al_val[0], al_val[1], (int)cap,
-                                                                       (int)n_reads, al_seg, al_seg + 1, s));
-        } else
-            NVB_CUDA_TRY(cudaMemsetAsync(al_seg, 0, sizeof(uint32_t) * ((size_t)n_reads + 1), s));
-        // al_cnt[n_reads] stays 0: the scan's extra element makes d_first[n_reads] the total
-        all_select_kernel<<<rgrid, 256, 0, s>>>(g, scored(), str_len, al_seg, al_key[1], al_val[1], AP->max_per_read, al_cnt);
+        NVB_TRY(cand_segments(true));
+        // cs_cnt[n_reads] stays 0: the scan's extra element makes d_first[n_reads] the total
+        all_select_kernel<<<rgrid, 256, 0, s>>>(g, scored(), str_len, cs_seg, cs_key[1], cs_val[1], AP->max_per_read, cs_cnt);
         NVB_LAUNCH_CHECK();
-        size_t bytes = al_scan_bytes;
-        NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(al_scan_tmp, bytes, al_cnt, O.d_first, (int)n_reads + 1, s));
+        size_t bytes = cs_scan_bytes;
+        NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(cs_scan_tmp, bytes, cs_cnt, O.d_first, (int)n_reads + 1, s));
         all_count_kernel<<<(n_slices + 256) / 256, 256, 0, s>>>(n_reads, O.d_first, acap, n_slices, O.d_count, al_slice_n);
         NVB_LAUNCH_CHECK();
         if (!acap) return launched();
-        all_emit_kernel<<<rgrid, 256, 0, s>>>(g, scored(), O.d_first, al_seg, al_val[1], acap, O.d_read, O.d_score, O.d_pos, O.alignment.d_strand,
+        all_emit_kernel<<<rgrid, 256, 0, s>>>(g, scored(), O.d_first, cs_seg, cs_val[1], acap, O.d_read, O.d_score, O.d_pos, O.alignment.d_strand,
                                               al_jobs);
         NVB_LAUNCH_CHECK();
         // slice t: alignments [t * n_reads, + n) traced like the best alignments of nvb_seed_extend_traceback (its direction matrices, sized
         // for n_reads); the count of each slice lives on the device, a slice past the stored alignments launches only empty CTAs
-        const nvb_best_alignment_out& A = O.alignment;
         for (uint32_t t = 0; t < n_slices; ++t) {
             const size_t b = (size_t)t * n_reads;
-            const uint32_t n = (uint32_t)(acap - b < n_reads ? acap - b : n_reads);
             const Jobs j{al_jobs.p_off + b, al_jobs.p_len + b, al_jobs.t_off + b, al_jobs.t_len + b};
-            const JobViews v = job_views(j, rd.length + g.band);
-            size_t tb = tb_bytes;
-            NVB_TRY(banded_traceback(g.band, P->type, &P->scheme, &v.pats, str_quals, &v.txts, al_slice_n + t, n, b_score, (nvb_uint2*)b_sink,
-                                     (nvb_uint2*)b_source, A.d_ops + b * A.max_ops, A.max_ops, A.d_n_ops + b, tb_tmp, &tb, s));
-            all_begin_kernel<<<(n + 255) / 256, 256, 0, s>>>(al_slice_n + t, j.t_off, b_source, (uint2*)A.d_begin + b);
-            NVB_LAUNCH_CHECK();
+            NVB_TRY(trace_jobs(j, al_slice_n + t, (uint32_t)(acap - b < n_reads ? acap - b : n_reads), O.alignment, b, nullptr));
         }
         return launched();
     }
@@ -1460,7 +1446,7 @@ struct PipeCall {
     int pair_second() const
     {
         const uint32_t n_pairs = g.n_reads / 2u;
-        pair_second_kernel<<<(n_pairs + 255) / 256, 256, 0, s>>>(n_pairs, *PP, *MP, str_len, pc_seg, pc_fw, pc_n, pc_end, pc_score, pc_tie,
+        pair_second_kernel<<<(n_pairs + 255) / 256, 256, 0, s>>>(n_pairs, *PP, *MP, str_len, cs_seg, pc_fw, pc_n, pc_end, pc_score, pc_tie,
                                                                   se_pos, rb_strand, best_key, pw_want, pw_idx, pw_toff, rs_score, rs_sink,
                                                                   PO->d_pair_score, PO->d_pair_flags, PO->d_mate_pos, PO->d_mate_strand,
                                                                   PMO->d_second_pair_score, PMO->d_second_mate_pos, PMO->d_second_mate_strand,
@@ -1515,48 +1501,40 @@ struct PipeCall {
     }
 };
 
-static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
-                    const nvb_string_set* reads, uint32_t n_reads,
-                    const nvb_seed_extend_params* P, uint32_t hit_capacity,
-                    int32_t* d_best_score, uint32_t* d_best_pos,
-                    uint32_t* d_n_hits, uint32_t* d_hit_read, nvb_uint2* d_hit_window,
-                    int32_t* d_hit_score, nvb_uint2* d_hit_sink,
-                    const nvb_best_alignment_out* BA,
-                    const nvb_pair_params* PP, const nvb_pair_out* PO,
-                    const nvb_mapq_params* MP, const nvb_mapq_out* MO, const nvb_pair_mapq_out* PMO,
-                    void* d_temp, size_t* temp_bytes, void* stream, const nvb_all_params* AP = nullptr, const nvb_all_out* AO = nullptr)
+static int seed_extend_impl(const SeedExtendReq& R, void* d_temp, size_t* temp_bytes, void* stream)
 {
     // The entry points check only what cannot be seen here: that the structs they require are there, and the pair count before
     // 2 * n_pairs is formed.  The order below decides which code a call with several faults gets: the paired traceback's read length
     // limit comes after the outputs and MAPQ inputs and before everything else.
-    if (!reads || !temp_bytes) return NVB_E_INVALID;
-    if (BA && (!BA->d_ops || !BA->d_n_ops || !BA->d_begin || BA->max_ops == 0)) return NVB_E_INVALID;
-    if ((MP == nullptr) != (MO == nullptr && PMO == nullptr)) return NVB_E_INVALID;
-    if (MP && (!MP->d_min_score || MP->max_read_len < reads->length)) return NVB_E_INVALID;   // the min-score table must cover every read length
-    if (MO && (!MO->d_second_score || !MO->d_mapq)) return NVB_E_INVALID;
-    if (PMO && (!PMO->d_second_pair_score || !PMO->d_mate_mapq)) return NVB_E_INVALID;
-    if (PP && BA && reads->length > FULL_TB_MAX_M) return NVB_E_UNSUPPORTED;                 // nvBowtie's MAXIMUM_READ_LENGTH
-    if (AO && reads->length > FULL_TB_MAX_M) return NVB_E_UNSUPPORTED;
-    if (PP) {
-        if (!PO->d_pair_score || !PO->d_pair_flags || !PO->d_mate_score || !PO->d_mate_pos || !PO->d_mate_strand) return NVB_E_INVALID;
-        if (!P || !P->both_strands || (n_reads & 1u) || PP->max_frag == 0 || PP->min_frag > PP->max_frag) return NVB_E_INVALID;
+    if (!R.reads || !temp_bytes) return NVB_E_INVALID;
+    if (R.BA && (!R.BA->d_ops || !R.BA->d_n_ops || !R.BA->d_begin || R.BA->max_ops == 0)) return NVB_E_INVALID;
+    if ((R.MP == nullptr) != (R.MO == nullptr && R.PMO == nullptr)) return NVB_E_INVALID;
+    if (R.MP && (!R.MP->d_min_score || R.MP->max_read_len < R.reads->length)) return NVB_E_INVALID;   // the min-score table must cover every read length
+    if (R.MO && (!R.MO->d_second_score || !R.MO->d_mapq)) return NVB_E_INVALID;
+    if (R.PMO && (!R.PMO->d_second_pair_score || !R.PMO->d_mate_mapq)) return NVB_E_INVALID;
+    if (R.PP && R.BA && R.reads->length > FULL_TB_MAX_M) return NVB_E_UNSUPPORTED;                 // nvBowtie's MAXIMUM_READ_LENGTH
+    if (R.AO && R.reads->length > FULL_TB_MAX_M) return NVB_E_UNSUPPORTED;
+    const nvb_seed_extend_params* P = R.P;
+    if (R.PP) {
+        if (!R.PO->d_pair_score || !R.PO->d_pair_flags || !R.PO->d_mate_score || !R.PO->d_mate_pos || !R.PO->d_mate_strand) return NVB_E_INVALID;
+        if (!P || !P->both_strands || (R.n_reads & 1u) || R.PP->max_frag == 0 || R.PP->min_frag > R.PP->max_frag) return NVB_E_INVALID;
     }
-    if (!valid_fmindex(fmi) || !fmi->d_ssa || !d_genome || !valid_strset(reads) || !P) return NVB_E_INVALID;
-    if (reads->bits == 8) return NVB_E_UNSUPPORTED;
+    if (!valid_fmindex(R.fmi) || !R.fmi->d_ssa || !R.genome || !valid_strset(R.reads) || !P) return NVB_E_INVALID;
+    if (R.reads->bits == 8) return NVB_E_UNSUPPORTED;
     if (P->seed_len == 0 || P->seed_interval == 0 || P->max_seed_hits == 0) return NVB_E_INVALID;
-    if (n_reads && (!d_best_score || !d_best_pos)) return NVB_E_INVALID;
-    const uint32_t max_len = reads->length;                 // maximum read length (== length for fixed-length sets)
+    if (R.n_reads && (!R.best_score || !R.best_pos)) return NVB_E_INVALID;
+    const uint32_t max_len = R.reads->length;               // maximum read length (== length for fixed-length sets)
     if (max_len < P->seed_len) return NVB_E_INVALID;
 
-    PipeCall c = {};
+    PipeCall c{R};                                          // the request; everything else starts zeroed
     PipeGeom& g = c.g;
-    g.n_reads = n_reads; g.strands = P->both_strands ? 2u : 1u; g.n_strings = n_reads * g.strands;
-    g.bits = reads->bits;
+    g.n_reads = R.n_reads; g.strands = P->both_strands ? 2u : 1u; g.n_strings = R.n_reads * g.strands;
+    g.bits = R.reads->bits;
     const uint32_t spw = 32u / g.bits;
     g.stride = (max_len + spw - 1u) / spw * spw;
     g.seeds_per_string = (max_len - P->seed_len) / P->seed_interval + 1u;
     g.seed_len = P->seed_len; g.seed_interval = P->seed_interval; g.band = P->band_len;
-    g.max_seed_hits = P->max_seed_hits; g.genome_len = fmi->length;
+    g.max_seed_hits = P->max_seed_hits; g.genome_len = R.fmi->length;
     if ((uint64_t)g.n_strings * g.stride > 0xFFFFFFFFull) return NVB_E_UNSUPPORTED;
     const uint64_t nq64 = (uint64_t)g.n_strings * g.seeds_per_string;
     if (nq64 > 0x7FFFFFFFull) return NVB_E_UNSUPPORTED;
@@ -1564,17 +1542,14 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     if (nq64 * (uint64_t)P->max_seed_hits > 0xFFFFFFFFull) return NVB_E_UNSUPPORTED;
 
     const cudaStream_t s = c.s = as_stream(stream);
-    c.P = P; c.f = make_fmindex(fmi); c.rd = make_strset(reads); c.genome = d_genome; c.nq = (uint32_t)nq64; c.hit_capacity = hit_capacity;
-    c.best_score = d_best_score; c.best_pos = d_best_pos; c.hit_score = d_hit_score; c.hit_sink = d_hit_sink; c.BA = BA; c.PP = PP; c.PO = PO; c.MP = MP; c.MO = MO;
-    c.AP = AP; c.AO = AO;
-    if (PMO) {                                 // the single-end second best and MAPQ of every mate (mate_mapq: overwritten for paired pairs)
-        c.PMO = PMO;
-        c.se_mo.d_second_score = PMO->d_mate_second_score; c.se_mo.d_mapq = PMO->d_mate_mapq;
+    c.f = make_fmindex(R.fmi); c.rd = make_strset(R.reads); c.nq = (uint32_t)nq64;
+    if (R.PMO) {                               // the single-end second best and MAPQ of every mate (mate_mapq: overwritten for paired pairs)
+        c.se_mo.d_second_score = R.PMO->d_mate_second_score; c.se_mo.d_mapq = R.PMO->d_mate_mapq;
         c.MO = &c.se_mo;
     }
     c.dedup = P->dedup_jobs != 0;
     // per-read path: nobody asked for per-hit outputs, so no per-hit array needs to exist (the traceback takes the best of the distinct jobs)
-    c.per_read = c.dedup && g_pipe_path != 1 && !d_hit_read && !d_hit_window && !d_hit_score && !d_hit_sink;
+    c.per_read = c.dedup && g_pipe_path != 1 && !R.hit_read && !R.hit_window && !R.hit_score && !R.hit_sink;
     const nvb_gotoh_scheme& SC = P->scheme;
     c.eligible = c.per_read && P->type == NVB_LOCAL && g.bits == 2 && P->band_len <= 32 && !SC.d_qual_table && SC.match > 0 && SC.mismatch < 0 &&
                  SC.pattern_gap_open < 0 && SC.pattern_gap_ext <= 0 && SC.text_gap_open < 0 && SC.text_gap_ext <= 0;
@@ -1582,10 +1557,10 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     size_t need = 0;
     NVB_TRY(c.carve(d_temp, need));
     if (!d_temp || *temp_bytes < need) { *temp_bytes = need; return NVB_E_TEMP_SIZE; }
-    if (n_reads == 0) {
-        if (AO) {
-            NVB_CUDA_TRY(cudaMemsetAsync(AO->d_first, 0, sizeof(uint32_t), s));
-            NVB_CUDA_TRY(cudaMemsetAsync(AO->d_count, 0, 2 * sizeof(uint32_t), s));
+    if (R.n_reads == 0) {
+        if (R.AO) {
+            NVB_CUDA_TRY(cudaMemsetAsync(R.AO->d_first, 0, sizeof(uint32_t), s));
+            NVB_CUDA_TRY(cudaMemsetAsync(R.AO->d_count, 0, 2 * sizeof(uint32_t), s));
         }
         return NVB_OK;
     }
@@ -1598,24 +1573,25 @@ static int seed_extend_impl(const nvb_fm_index* fmi, const uint32_t* d_genome,
     if (!c.per_read) {
         size_t scan_bytes = c.scan_bytes;
         NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c.scan_tmp, scan_bytes, c.sizes, c.excl, (int)c.nq, s));
-        pipe_count_kernel<<<1, 32, 0, s>>>(c.excl, c.sizes, c.nq, hit_capacity, c.counts);
+        pipe_count_kernel<<<1, 32, 0, s>>>(c.excl, c.sizes, c.nq, R.hit_capacity, c.counts);
         NVB_LAUNCH_CHECK();
     }
     NVB_TRY(c.stage(3));
     NVB_TRY(c.per_read ? c.extend_per_read() : c.extend_per_hit());       // records stages 4 to 6
-    if (hit_capacity && (d_hit_read || d_hit_window)) {
-        pipe_export_hits_kernel<<<(hit_capacity + 255) / 256, 256, 0, s>>>(g, c.counts, c.hit_string, c.hits.t_off, c.hits.t_len, d_hit_read, (uint2*)d_hit_window);
+    if (R.hit_capacity && (R.hit_read || R.hit_window)) {
+        pipe_export_hits_kernel<<<(R.hit_capacity + 255) / 256, 256, 0, s>>>(g, c.counts, c.hit_string, c.hits.t_off, c.hits.t_len, R.hit_read,
+                                                                             (uint2*)R.hit_window);
         NVB_LAUNCH_CHECK();
     }
-    if (BA && !PP) NVB_TRY(c.best_traceback());
+    if (R.BA && !R.PP) NVB_TRY(c.best_traceback());
     if (c.MO) NVB_TRY(c.second_best());
-    if (AO) NVB_TRY(c.all_alignments());
-    if (PMO) NVB_TRY(c.pair_candidates());
-    if (PP) NVB_TRY(c.paired_rescue());
-    if (BA && PP) { NVB_TRY(c.best_traceback()); NVB_TRY(c.rescue_traceback()); }
-    if (PMO) NVB_TRY(c.pair_second());
+    if (R.AO) NVB_TRY(c.all_alignments());
+    if (R.PMO) NVB_TRY(c.pair_candidates());
+    if (R.PP) NVB_TRY(c.paired_rescue());
+    if (R.BA && R.PP) { NVB_TRY(c.best_traceback()); NVB_TRY(c.rescue_traceback()); }
+    if (R.PMO) NVB_TRY(c.pair_second());
     if (!c.dedup) NVB_CUDA_TRY(cudaMemcpyAsync(c.counts + 2, c.counts, sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
-    if (d_n_hits) NVB_CUDA_TRY(cudaMemcpyAsync(d_n_hits, c.counts, 3 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+    if (R.n_hits) NVB_CUDA_TRY(cudaMemcpyAsync(R.n_hits, c.counts, 3 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
     NVB_TRY(c.stage(7));
     c.SE->valid = true;
     return NVB_OK;
@@ -1640,8 +1616,11 @@ extern "C" int nvb_seed_extend(const nvb_fm_index* fmi, const uint32_t* d_genome
                     int32_t* d_hit_score, nvb_uint2* d_hit_sink,
                     void* d_temp, size_t* temp_bytes, void* stream)
 {
-    return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
-                            d_hit_score, d_hit_sink, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
+    SeedExtendReq R = {};
+    R.fmi = fmi; R.genome = d_genome; R.reads = reads; R.n_reads = n_reads; R.P = P; R.hit_capacity = hit_capacity;
+    R.best_score = d_best_score; R.best_pos = d_best_pos; R.n_hits = d_n_hits; R.hit_read = d_hit_read; R.hit_window = d_hit_window;
+    R.hit_score = d_hit_score; R.hit_sink = d_hit_sink;
+    return seed_extend_impl(R, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_traceback(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1654,8 +1633,11 @@ extern "C" int nvb_seed_extend_traceback(const nvb_fm_index* fmi, const uint32_t
                     void* d_temp, size_t* temp_bytes, void* stream)
 {
     if (!best_alignment) return NVB_E_INVALID;
-    return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
-                            d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
+    SeedExtendReq R = {};
+    R.fmi = fmi; R.genome = d_genome; R.reads = reads; R.n_reads = n_reads; R.P = P; R.hit_capacity = hit_capacity;
+    R.best_score = d_best_score; R.best_pos = d_best_pos; R.n_hits = d_n_hits; R.hit_read = d_hit_read; R.hit_window = d_hit_window;
+    R.hit_score = d_hit_score; R.hit_sink = d_hit_sink; R.BA = best_alignment;
+    return seed_extend_impl(R, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1665,9 +1647,11 @@ extern "C" int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream)
 {
     if (!pair_params || !out || n_pairs > 0x3FFFFFFFu) return NVB_E_INVALID;
+    SeedExtendReq R = {};
+    R.fmi = fmi; R.genome = d_genome; R.reads = reads; R.n_reads = 2u * n_pairs; R.P = P; R.hit_capacity = hit_capacity;
     // the per-read best (score, end) of the single-end stage lands in the mate arrays first and is then refined per pair
-    return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
-                            nullptr, nullptr, nullptr, pair_params, out, nullptr, nullptr, nullptr, d_temp, temp_bytes, stream);
+    R.best_score = out->d_mate_score; R.best_pos = out->d_mate_pos; R.n_hits = d_n_hits; R.PP = pair_params; R.PO = out;
+    return seed_extend_impl(R, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1681,8 +1665,11 @@ extern "C" int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_g
                     void* d_temp, size_t* temp_bytes, void* stream)
 {
     if (!mapq || !mapq_out) return NVB_E_INVALID;
-    return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
-                            d_hit_score, d_hit_sink, best_alignment, nullptr, nullptr, mapq, mapq_out, nullptr, d_temp, temp_bytes, stream);
+    SeedExtendReq R = {};
+    R.fmi = fmi; R.genome = d_genome; R.reads = reads; R.n_reads = n_reads; R.P = P; R.hit_capacity = hit_capacity;
+    R.best_score = d_best_score; R.best_pos = d_best_pos; R.n_hits = d_n_hits; R.hit_read = d_hit_read; R.hit_window = d_hit_window;
+    R.hit_score = d_hit_score; R.hit_sink = d_hit_sink; R.BA = best_alignment; R.MP = mapq; R.MO = mapq_out;
+    return seed_extend_impl(R, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_all(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1701,9 +1688,11 @@ extern "C" int nvb_seed_extend_all(const nvb_fm_index* fmi, const uint32_t* d_ge
     const nvb_best_alignment_out& A = O.alignment;
     if (!O.d_first || !O.d_read || !O.d_score || !O.d_pos || !O.d_count || !A.d_ops || !A.d_n_ops || !A.d_begin || !A.d_strand || A.max_ops == 0)
         return NVB_E_INVALID;
-    return seed_extend_impl(fmi, d_genome, reads, n_reads, P, hit_capacity, d_best_score, d_best_pos, d_n_hits, d_hit_read, d_hit_window,
-                            d_hit_score, d_hit_sink, nullptr, nullptr, nullptr, mapq, mapq_out, nullptr, d_temp, temp_bytes, stream,
-                            all_params, all_out);
+    SeedExtendReq R = {};
+    R.fmi = fmi; R.genome = d_genome; R.reads = reads; R.n_reads = n_reads; R.P = P; R.hit_capacity = hit_capacity;
+    R.best_score = d_best_score; R.best_pos = d_best_pos; R.n_hits = d_n_hits; R.hit_read = d_hit_read; R.hit_window = d_hit_window;
+    R.hit_score = d_hit_score; R.hit_sink = d_hit_sink; R.MP = mapq; R.MO = mapq_out; R.AP = all_params; R.AO = all_out;
+    return seed_extend_impl(R, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_paired_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1714,8 +1703,10 @@ extern "C" int nvb_seed_extend_paired_mapq(const nvb_fm_index* fmi, const uint32
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream)
 {
     if (!pair_params || !out || !mapq || !mapq_out || n_pairs > 0x3FFFFFFFu) return NVB_E_INVALID;
-    return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
-                            nullptr, nullptr, nullptr, pair_params, out, mapq, nullptr, mapq_out, d_temp, temp_bytes, stream);
+    SeedExtendReq R = {};
+    R.fmi = fmi; R.genome = d_genome; R.reads = reads; R.n_reads = 2u * n_pairs; R.P = P; R.hit_capacity = hit_capacity;
+    R.best_score = out->d_mate_score; R.best_pos = out->d_mate_pos; R.n_hits = d_n_hits; R.PP = pair_params; R.PO = out; R.MP = mapq; R.PMO = mapq_out;
+    return seed_extend_impl(R, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_seed_extend_paired_traceback(const nvb_fm_index* fmi, const uint32_t* d_genome,
@@ -1727,8 +1718,11 @@ extern "C" int nvb_seed_extend_paired_traceback(const nvb_fm_index* fmi, const u
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream)
 {
     if (!pair_params || !out || !mate_alignment || n_pairs > 0x3FFFFFFFu) return NVB_E_INVALID;
-    return seed_extend_impl(fmi, d_genome, reads, 2u * n_pairs, P, hit_capacity, out->d_mate_score, out->d_mate_pos, d_n_hits, nullptr, nullptr,
-                            nullptr, nullptr, mate_alignment, pair_params, out, mapq, nullptr, mapq_out, d_temp, temp_bytes, stream);
+    SeedExtendReq R = {};
+    R.fmi = fmi; R.genome = d_genome; R.reads = reads; R.n_reads = 2u * n_pairs; R.P = P; R.hit_capacity = hit_capacity;
+    R.best_score = out->d_mate_score; R.best_pos = out->d_mate_pos; R.n_hits = d_n_hits; R.PP = pair_params; R.PO = out;
+    R.BA = mate_alignment; R.MP = mapq; R.PMO = mapq_out;
+    return seed_extend_impl(R, d_temp, temp_bytes, stream);
 }
 
 extern "C" int nvb_debug_mapq_eval(const int32_t* d_best, const uint8_t* d_has_second, const int32_t* d_second, const uint32_t* d_len,

@@ -1,6 +1,6 @@
 // tests/host/all_harness.cu -- TEST INFRASTRUCTURE.
 // The selection rule of nvb_seed_extend_all run serially on the CPU with the routines the kernels use (reportable, make_best_key,
-// end_strand, select_distinct in pipeline_core.cuh): pair_cand_scatter_kernel's filter, the segmented sort's order and
+// end_strand, select_distinct in pipeline_core.cuh): cand_scatter_kernel's filter, the segmented sort's order and
 // all_select_kernel's walk over one read's candidates.  Built by tests/test_all_host.py.
 #include "../../nvbio_b200/csrc/pipeline_core.cuh"
 #include <algorithm>

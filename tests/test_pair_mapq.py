@@ -138,7 +138,7 @@ def run_host(H, cases, min_frag, max_frag):
 
 
 def check(H, cases, min_frag, max_frag, min_score=None):
-    """min_score: drop the candidates below it first, as pair_cand_scatter_kernel does"""
+    """min_score: drop the candidates below it first, as cand_scatter_kernel does"""
     if min_score is not None:
         cases = [([c for c in c1 if c[0] >= min_score], [c for c in c2 if c[0] >= min_score]) + tuple(rest) for c1, c2, *rest in cases]
     got = run_host(H, cases, min_frag, max_frag)

@@ -22,7 +22,7 @@ if ROOT not in sys.path:
 import bench  # noqa: E402
 from tools.bench_mapq import power_limit_w  # noqa: E402
 
-SELECT = ("all_select", "all_count", "all_emit", "all_begin", "pair_cand_scatter", "DeviceSegmentedSort", "DeviceScan", "SegmentedSort")
+SELECT = ("all_select", "all_count", "all_emit", "cand_scatter", "DeviceSegmentedSort", "DeviceScan", "SegmentedSort")
 TRACE = ("traceback", "gotoh", "banded", "pair_")
 
 
