@@ -81,8 +81,105 @@ __device__ __forceinline__ uint32_t swap_2bit_order(uint32_t x) {
     return ((r >> 1) & 0x55555555u) | ((r & 0x55555555u) << 1);
 }
 
-// ROWS2: two pattern rows in flight per thread (gotoh_pair)
+// one pair of alignments (2 pair, 2 pair + 1) of gotoh_pair_kernel, n = the batch size; my_sel = the thread's selector column
 template <int B, int TYPE, int PFMT, bool ROWS2>
+__device__ __forceinline__ void gotoh_pair_job(const GotohScheme& S, const GotohBatch& b, const uint32_t sel_rows, uint32_t* __restrict__ todo,
+                                               uint32_t* __restrict__ todo_count, const uint32_t pair, const uint32_t n, uint16_t* my_sel,
+                                               const uint32_t* prof_tab)
+{
+    const uint32_t a0 = 2u * pair;
+    const bool has1 = (a0 + 1u < n);
+    const uint32_t a1 = has1 ? a0 + 1u : a0;          // an odd tail computes the same alignment in both halves
+
+    const uint32_t M0 = str_len(b.pat, a0), M1 = str_len(b.pat, a1);
+    const uint32_t N0 = str_len(b.txt, a0), N1 = str_len(b.txt, a1);
+    const uint32_t Mmax = M0 > M1 ? M0 : M1;
+    const uint32_t L = Mmax + (uint32_t)B - 1u;       // text columns touched
+
+    const bool ok = (M0 >= 1u) && (M1 >= 1u) && (N0 >= M0 + (uint32_t)B - 1u) && (N1 >= M1 + (uint32_t)B - 1u) &&
+                    (L <= sel_rows) && (TYPE == NVB_LOCAL || M0 == M1);
+    if (!ok) {
+        const uint32_t cnt = has1 ? 2u : 1u;
+        const uint32_t slot = atomicAdd(todo_count, cnt);
+        todo[slot] = a0;
+        if (has1) todo[slot + 1u] = a1;
+        return;
+    }
+
+    // stage the PRMT selectors of this thread's two text windows (own shared-memory column: no barrier needed).
+    // Word-wise: the 16 symbols starting at any offset are a funnel shift of two consecutive words, and the loads
+    // of successive words are independent, so they overlap instead of forming a chain of dependent round trips.
+    {
+        const uint32_t t0 = str_off(b.txt, a0), t1 = str_off(b.txt, a1);
+        const uint32_t* __restrict__ w = b.txt.words;
+        const bool be = b.txt.big_endian != 0;
+        const uint32_t w0 = t0 >> 4, w1 = t1 >> 4;                         // first stream word of each window
+        const uint32_t sh0 = 2u * (t0 & 15u), sh1 = 2u * (t1 & 15u);
+        const uint32_t last0 = (t0 + N0 - 1u) >> 4, last1 = (t1 + N1 - 1u) >> 4;   // last word holding a window symbol
+        const uint32_t nw = (L + 15u) >> 4;
+        // the window words are fetched eight (+1) per alignment at a time, all loads of a batch independent of each other: a
+        // thread pays two or three DRAM round trips for its two windows instead of one per word (the windows sit at random
+        // genome positions, and at 16 warps per SM nobody else hides that latency)
+        // (the shared array is sized for whole words of 16 columns, so no per-column bound checks: symbols past a window's end
+        // are masked to 0 per word, columns past L are written and never read)
+        for (uint32_t kb = 0; kb < nw; kb += 8u) {
+            uint32_t a0[9], a1[9];
+#pragma unroll
+            for (uint32_t q = 0; q < 9u; ++q) {
+                // never touch a word beyond the window's last one
+                a0[q] = (w0 + kb + q <= last0) ? w[w0 + kb + q] : 0u;
+                a1[q] = (w1 + kb + q <= last1) ? w[w1 + kb + q] : 0u;
+            }
+#pragma unroll
+            for (uint32_t q = 0; q < 8u; ++q) {
+                const uint32_t k = kb + q;
+                if (k < nw) {
+                    uint32_t c0, c1;
+                    if (be) {
+                        c0 = sh0 ? ((a0[q] << sh0) | (a0[q + 1] >> (32u - sh0))) : a0[q];
+                        c1 = sh1 ? ((a1[q] << sh1) | (a1[q + 1] >> (32u - sh1))) : a1[q];
+                    } else {
+                        c0 = sh0 ? ((a0[q] >> sh0) | (a0[q + 1] << (32u - sh0))) : a0[q];
+                        c1 = sh1 ? ((a1[q] >> sh1) | (a1[q + 1] << (32u - sh1))) : a1[q];
+                    }
+                    const uint32_t first = k << 4;
+                    // symbols of this word inside the window: v0, v1 in [0, 16]; the rest read as symbol 0
+                    const uint32_t v0 = N0 > first ? (N0 - first < 16u ? N0 - first : 16u) : 0u;
+                    const uint32_t v1 = N1 > first ? (N1 - first < 16u ? N1 - first : 16u) : 0u;
+                    const uint32_t m0 = v0 >= 16u ? 0xFFFFFFFFu : (be ? ~(0xFFFFFFFFu >> (2u * v0)) : ((1u << (2u * v0)) - 1u));
+                    const uint32_t m1 = v1 >= 16u ? 0xFFFFFFFFu : (be ? ~(0xFFFFFFFFu >> (2u * v1)) : ((1u << (2u * v1)) - 1u));
+                    c0 &= m0; c1 &= m1;
+                    if (!be) { c0 = swap_2bit_order(c0); c1 = swap_2bit_order(c1); }        // first symbol in the top bits from here on
+                    // four columns at a time: one byte of each window side by side, then per column a shift, a mask and an IMAD
+                    //   x = g0 | g1 << 8;  pair_selector(g0, g1) = 0xC480 + x * 0x11
+#pragma unroll
+                    for (uint32_t by = 0; by < 4u; ++by) {
+                        const uint32_t W = prmt(c0, c1, (3u - by) | ((7u - by) << 4) | 0x3200u);      // byte `by` (from the top) of c0 | of c1 << 8
+#pragma unroll
+                        for (uint32_t m = 0; m < 4u; ++m) {
+                            const uint32_t x = (W >> (6u - 2u * m)) & 0x0303u;
+                            my_sel[(first + 4u * by + m) * PAIR_BLOCKDIM] = (uint16_t)(x * 0x11u + 0xC480u);
+                        }
+                    }
+                }
+            }
+        }
+    }
+
+    SinkResult r0, r1;
+    gotoh_pair<B, TYPE, PFMT, ROWS2>(S, b.pat.words, b.pat.bits, b.pat.big_endian,
+                        str_off(b.pat, a0), M0, str_off(b.pat, a1), M1, N0, N1,
+                        my_sel, PAIR_BLOCKDIM, r0, r1, b.quals, prof_tab);
+    b.score[a0] = r0.score; b.sink[a0] = make_uint2(r0.x, r0.y);
+    if (has1) { b.score[a1] = r1.score; b.sink[a1] = make_uint2(r1.x, r1.y); }
+}
+
+// ROWS2: two pattern rows in flight per thread (gotoh_pair)
+// TICKET (only with a device-side count, b.d_n): a resident grid whose warps claim 32 pairs at a time from the ticket todo_count[1]
+// (zeroed with todo_count[0]), so the launch costs what the batch holds and not what its capacity could.  Sized from the capacity
+// (one pair per thread, the exact-count path), most of a pipeline batch's CTAs would start only to find no work: each still reserves
+// its selector shared memory, fills prof_tab and reads *d_n before it leaves.
+template <int B, int TYPE, int PFMT, bool ROWS2, bool TICKET>
 __global__ void __launch_bounds__(PAIR_BLOCKDIM, 4)
 gotoh_pair_kernel(const GotohScheme S, const GotohBatch b, uint32_t sel_rows, uint32_t* __restrict__ todo, uint32_t* __restrict__ todo_count)
 {
@@ -94,96 +191,21 @@ gotoh_pair_kernel(const GotohScheme S, const GotohBatch b, uint32_t sel_rows, ui
     const uint32_t n = batch_count(b);
     const uint32_t n_pairs = (n + 1u) / 2u;
     uint16_t* my_sel = sel_smem + threadIdx.x;
-    // one pair per thread (a grid-stride loop over a resident grid measured 5% slower: 108 vs 118 registers cost
-    // more than the empty CTAs of a device-side count save)
-    {
+    if (!TICKET) {
+        // one pair per thread (a grid-stride loop over a resident grid measured 5% slower: 108 vs 118 registers cost
+        // more than the empty CTAs of a device-side count save)
         const uint32_t pair = blockIdx.x * PAIR_BLOCKDIM + threadIdx.x;
         if (pair >= n_pairs) return;
-        const uint32_t a0 = 2u * pair;
-        const bool has1 = (a0 + 1u < n);
-        const uint32_t a1 = has1 ? a0 + 1u : a0;          // an odd tail computes the same alignment in both halves
-
-        const uint32_t M0 = str_len(b.pat, a0), M1 = str_len(b.pat, a1);
-        const uint32_t N0 = str_len(b.txt, a0), N1 = str_len(b.txt, a1);
-        const uint32_t Mmax = M0 > M1 ? M0 : M1;
-        const uint32_t L = Mmax + (uint32_t)B - 1u;       // text columns touched
-
-        const bool ok = (M0 >= 1u) && (M1 >= 1u) && (N0 >= M0 + (uint32_t)B - 1u) && (N1 >= M1 + (uint32_t)B - 1u) &&
-                        (L <= sel_rows) && (TYPE == NVB_LOCAL || M0 == M1);
-        if (!ok) {
-            const uint32_t cnt = has1 ? 2u : 1u;
-            const uint32_t slot = atomicAdd(todo_count, cnt);
-            todo[slot] = a0;
-            if (has1) todo[slot + 1u] = a1;
-            return;
+        gotoh_pair_job<B, TYPE, PFMT, ROWS2>(S, b, sel_rows, todo, todo_count, pair, n, my_sel, prof_tab);
+    } else {
+        const uint32_t lane = threadIdx.x & 31u;
+        for (;;) {
+            uint32_t first = 0;
+            if (lane == 0u) first = atomicAdd(todo_count + 1, 32u);
+            first = __shfl_sync(0xFFFFFFFFu, first, 0);
+            if (first >= n_pairs) return;
+            if (first + lane < n_pairs) gotoh_pair_job<B, TYPE, PFMT, ROWS2>(S, b, sel_rows, todo, todo_count, first + lane, n, my_sel, prof_tab);
         }
-
-        // stage the PRMT selectors of this thread's two text windows (own shared-memory column: no barrier needed).
-        // Word-wise: the 16 symbols starting at any offset are a funnel shift of two consecutive words, and the loads
-        // of successive words are independent, so they overlap instead of forming a chain of dependent round trips.
-        {
-            const uint32_t t0 = str_off(b.txt, a0), t1 = str_off(b.txt, a1);
-            const uint32_t* __restrict__ w = b.txt.words;
-            const bool be = b.txt.big_endian != 0;
-            const uint32_t w0 = t0 >> 4, w1 = t1 >> 4;                         // first stream word of each window
-            const uint32_t sh0 = 2u * (t0 & 15u), sh1 = 2u * (t1 & 15u);
-            const uint32_t last0 = (t0 + N0 - 1u) >> 4, last1 = (t1 + N1 - 1u) >> 4;   // last word holding a window symbol
-            const uint32_t nw = (L + 15u) >> 4;
-            // the window words are fetched eight (+1) per alignment at a time, all loads of a batch independent of each other: a
-            // thread pays two or three DRAM round trips for its two windows instead of one per word (the windows sit at random
-            // genome positions, and at 16 warps per SM nobody else hides that latency)
-            // (the shared array is sized for whole words of 16 columns, so no per-column bound checks: symbols past a window's end
-            // are masked to 0 per word, columns past L are written and never read)
-            for (uint32_t kb = 0; kb < nw; kb += 8u) {
-                uint32_t a0[9], a1[9];
-#pragma unroll
-                for (uint32_t q = 0; q < 9u; ++q) {
-                    // never touch a word beyond the window's last one
-                    a0[q] = (w0 + kb + q <= last0) ? w[w0 + kb + q] : 0u;
-                    a1[q] = (w1 + kb + q <= last1) ? w[w1 + kb + q] : 0u;
-                }
-#pragma unroll
-                for (uint32_t q = 0; q < 8u; ++q) {
-                    const uint32_t k = kb + q;
-                    if (k < nw) {
-                        uint32_t c0, c1;
-                        if (be) {
-                            c0 = sh0 ? ((a0[q] << sh0) | (a0[q + 1] >> (32u - sh0))) : a0[q];
-                            c1 = sh1 ? ((a1[q] << sh1) | (a1[q + 1] >> (32u - sh1))) : a1[q];
-                        } else {
-                            c0 = sh0 ? ((a0[q] >> sh0) | (a0[q + 1] << (32u - sh0))) : a0[q];
-                            c1 = sh1 ? ((a1[q] >> sh1) | (a1[q + 1] << (32u - sh1))) : a1[q];
-                        }
-                        const uint32_t first = k << 4;
-                        // symbols of this word inside the window: v0, v1 in [0, 16]; the rest read as symbol 0
-                        const uint32_t v0 = N0 > first ? (N0 - first < 16u ? N0 - first : 16u) : 0u;
-                        const uint32_t v1 = N1 > first ? (N1 - first < 16u ? N1 - first : 16u) : 0u;
-                        const uint32_t m0 = v0 >= 16u ? 0xFFFFFFFFu : (be ? ~(0xFFFFFFFFu >> (2u * v0)) : ((1u << (2u * v0)) - 1u));
-                        const uint32_t m1 = v1 >= 16u ? 0xFFFFFFFFu : (be ? ~(0xFFFFFFFFu >> (2u * v1)) : ((1u << (2u * v1)) - 1u));
-                        c0 &= m0; c1 &= m1;
-                        if (!be) { c0 = swap_2bit_order(c0); c1 = swap_2bit_order(c1); }        // first symbol in the top bits from here on
-                        // four columns at a time: one byte of each window side by side, then per column a shift, a mask and an IMAD
-                        //   x = g0 | g1 << 8;  pair_selector(g0, g1) = 0xC480 + x * 0x11
-#pragma unroll
-                        for (uint32_t by = 0; by < 4u; ++by) {
-                            const uint32_t W = prmt(c0, c1, (3u - by) | ((7u - by) << 4) | 0x3200u);      // byte `by` (from the top) of c0 | of c1 << 8
-#pragma unroll
-                            for (uint32_t m = 0; m < 4u; ++m) {
-                                const uint32_t x = (W >> (6u - 2u * m)) & 0x0303u;
-                                my_sel[(first + 4u * by + m) * PAIR_BLOCKDIM] = (uint16_t)(x * 0x11u + 0xC480u);
-                            }
-                        }
-                    }
-                }
-            }
-        }
-
-        SinkResult r0, r1;
-        gotoh_pair<B, TYPE, PFMT, ROWS2>(S, b.pat.words, b.pat.bits, b.pat.big_endian,
-                            str_off(b.pat, a0), M0, str_off(b.pat, a1), M1, N0, N1,
-                            my_sel, PAIR_BLOCKDIM, r0, r1, b.quals, prof_tab);
-        b.score[a0] = r0.score; b.sink[a0] = make_uint2(r0.x, r0.y);
-        if (has1) { b.score[a1] = r1.score; b.sink[a1] = make_uint2(r1.x, r1.y); }
     }
 }
 
@@ -648,8 +670,8 @@ static int launch_generic(const GotohScheme& S, const GotohBatch& b, const uint3
     return NVB_OK;
 }
 
-template <int B, int TYPE, int PFMT, bool ROWS2>
-static int launch_pair_fmt(const GotohScheme& S, const GotohBatch& b, uint32_t sel_rows, uint32_t* todo, uint32_t* todo_count, cudaStream_t s)
+template <int B, int TYPE, int PFMT, bool ROWS2, bool TICKET>
+static int launch_pair_grid(const GotohScheme& S, const GotohBatch& b, uint32_t sel_rows, uint32_t* todo, uint32_t* todo_count, cudaStream_t s)
 {
     const size_t smem = (size_t)((sel_rows + 15u) & ~15u) * PAIR_BLOCKDIM * sizeof(uint16_t) + (size_t)g_pair_extra_smem;   // whole words of 16 columns
     // the attribute is per DEVICE: a host that drives several GPUs from one process (nvBowtie's one compute thread per
@@ -659,14 +681,26 @@ static int launch_pair_fmt(const GotohScheme& S, const GotohBatch& b, uint32_t s
     NVB_CUDA_TRY(cudaGetDevice(&dev));
     if (dev < 0 || dev >= NVB_MAX_DEVICES) return NVB_E_UNSUPPORTED;
     if (!attr_done[dev].load(std::memory_order_acquire)) {
-        NVB_CUDA_TRY(cudaFuncSetAttribute(gotoh_pair_kernel<B, TYPE, PFMT, ROWS2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        NVB_CUDA_TRY(cudaFuncSetAttribute(gotoh_pair_kernel<B, TYPE, PFMT, ROWS2, TICKET>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         attr_done[dev].store(true, std::memory_order_release);
     }
     const uint32_t pairs = (b.n_max + 1u) / 2u;
-    const uint32_t grid = (pairs + PAIR_BLOCKDIM - 1) / PAIR_BLOCKDIM;
-    gotoh_pair_kernel<B, TYPE, PFMT, ROWS2><<<grid, PAIR_BLOCKDIM, smem, s>>>(S, b, sel_rows, todo, todo_count);
+    uint32_t grid = (pairs + PAIR_BLOCKDIM - 1) / PAIR_BLOCKDIM;
+    if (TICKET) {                                                  // resident: what the SMs hold at once
+        int per_sm = 0;
+        NVB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gotoh_pair_kernel<B, TYPE, PFMT, ROWS2, TICKET>, PAIR_BLOCKDIM, smem));
+        const uint32_t resident = sm_count() * (uint32_t)(per_sm > 0 ? per_sm : 1);
+        grid = grid < resident ? grid : resident;
+    }
+    gotoh_pair_kernel<B, TYPE, PFMT, ROWS2, TICKET><<<grid, PAIR_BLOCKDIM, smem, s>>>(S, b, sel_rows, todo, todo_count);
     NVB_LAUNCH_CHECK();
     return NVB_OK;
+}
+template <int B, int TYPE, int PFMT, bool ROWS2>
+static int launch_pair_fmt(const GotohScheme& S, const GotohBatch& b, uint32_t sel_rows, uint32_t* todo, uint32_t* todo_count, cudaStream_t s)
+{
+    if (b.d_n) return launch_pair_grid<B, TYPE, PFMT, ROWS2, true>(S, b, sel_rows, todo, todo_count, s);
+    return launch_pair_grid<B, TYPE, PFMT, ROWS2, false>(S, b, sel_rows, todo, todo_count, s);
 }
 template <int B, int TYPE, int PFMT>
 static int launch_pair_rows(const GotohScheme& S, const GotohBatch& b, uint32_t sel_rows, uint32_t* todo, uint32_t* todo_count, cudaStream_t s)
@@ -769,7 +803,7 @@ static int banded_impl(int band, int type, const nvb_gotoh_scheme* scheme,
     if (!fast) { set_route(0, nullptr); return dispatch_generic(band, type, S, b, nullptr, nullptr, n_max, s); }
 
     set_route(1, todo_count);
-    NVB_CUDA_TRY(cudaMemsetAsync(todo_count, 0, sizeof(uint32_t), s));
+    NVB_CUDA_TRY(cudaMemsetAsync(todo_count, 0, 2 * sizeof(uint32_t), s));     // [0] the todo list's length, [1] the pair ticket
     int r = dispatch_pair(band, type, S, b, sel_rows, todo, todo_count, s);
     if (r != NVB_OK) return r;
     return dispatch_generic(band, type, S, b, todo, todo_count, n_max, s);

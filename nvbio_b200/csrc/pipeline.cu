@@ -278,9 +278,38 @@ struct Jobs { uint32_t *p_off, *p_len, *t_off, *t_len; };   // alignment jobs: a
 constexpr uint32_t RJ_BLOCK = 128;          // reads per tile (one CTA, one thread per read in phase A)
 constexpr uint32_t RJ_STAGE = 640;          // staged jobs per CTA (average: ~1.2 per read); more go straight to the global lists
 constexpr int      RJ_LOCAL = 6;            // distinct windows remembered per read (more are still scored, just not de-duplicated)
+constexpr uint32_t RJ_BATCH = 4;            // ranges whose loads phase A issues together
 constexpr uint32_t RJ_CLAIMED = 0xFFFFFFFFu, RJ_CLAIMED_EMPTY = 0xFFFFFFFEu;   // st_slot of a job the shortcut resolved (else: DP slot)
 using RjTileState = cub::ScanTileState<uint32_t>;
 using RjPrefixOp  = cub::TilePrefixCallbackOp<uint32_t, ::cuda::std::plus<uint32_t>, RjTileState>;
+
+// ranges [q0, q0 + RB) of a read's n ranges rr: their clamped hit counts are added to `hits`; returns the non-empty ones as bits.  Every
+// load of the batch is issued before the first is used (16-byte loads when vec: rr + q0 16-byte aligned and n even), so a thread pays
+// one memory round trip per batch instead of one per range.
+template <uint32_t RB>
+__device__ __forceinline__ uint32_t range_batch(const uint2* __restrict__ rr, const uint32_t q0, const uint32_t n, const bool vec,
+                                                const uint32_t max_seed_hits, uint32_t& hits)
+{
+    uint2 v[RB];
+    if (vec) {
+#pragma unroll
+        for (uint32_t j = 0; j < RB; j += 2u) {
+            const uint4 w = q0 + j < n ? *reinterpret_cast<const uint4*>(rr + q0 + j) : make_uint4(1u, 0u, 1u, 0u);
+            v[j] = make_uint2(w.x, w.y); v[j + 1] = make_uint2(w.z, w.w);
+        }
+    } else {
+#pragma unroll
+        for (uint32_t j = 0; j < RB; ++j) v[j] = q0 + j < n ? rr[q0 + j] : make_uint2(1u, 0u);       // (1, 0): an empty range
+    }
+    uint32_t m = 0;
+#pragma unroll
+    for (uint32_t j = 0; j < RB; ++j) {
+        const uint32_t sz = seed_range_hits(v[j], max_seed_hits);
+        hits += sz;
+        m |= (sz != 0u ? 1u : 0u) << j;
+    }
+    return m;
+}
 
 // the tile states of the hit-slot look-back and the counters of one call, reset in stream order: counts[2] = jobs, counts[3] = tile ticket
 __global__ void __launch_bounds__(256)
@@ -291,12 +320,13 @@ pipe_resolve_init_kernel(RjTileState tiles, const uint32_t n_tiles, uint32_t* __
 }
 
 // One tile of RJ_BLOCK reads per CTA.
-//  * Hit slots: each read sums its clamped range sizes (its ranges are read from global memory: staging the tile's 28 KB of ranges in
-//    shared memory measured 0.71 ms against 0.53 on the headline step: it cut the CTAs per SM from 7 to 5); a block scan plus a single-pass decoupled look-back over the tiles gives its first
+//  * Hit slots: each read sums its clamped range sizes and notes which of its first 32 ranges are non-empty (its ranges are read from
+//    global memory in batches of independent 16-byte loads, range_batch: staging the tile's 28 KB of ranges in shared memory measured
+//    0.71 ms against 0.53 on the headline step: it cut the CTAs per SM from 7 to 5); a block scan plus a single-pass decoupled look-back over the tiles gives its first
 //    slot (the per-hit path's exclusive scan at the read's first seed).  The tile index comes from a ticket, so every tile a CTA waits
 //    on belongs to a CTA that is already running.  The last tile writes counts[0] = min(total, capacity), counts[1] = total.
-//  * Phase A, one thread per read: locate, window and the RJ_LOCAL-window de-duplication (strands shared) of every kept hit
-//    (slot < hit_capacity); jobs are staged in shared memory, a job that does not fit goes straight to the job list and the DP list.
+//  * Phase A, one thread per read, over its non-empty ranges only (reloaded RJ_BATCH at a time): locate, window and the RJ_LOCAL-window
+//    de-duplication (strands shared) of every kept hit (slot < hit_capacity); jobs are staged in shared memory, a job that does not fit goes straight to the job list and the DP list.
 //  * Phase B, the whole CTA over the staged jobs: append them to the job list (one atomic), run the exact shortcut (shortcut: 0 = off,
 //    1 = with its one-gap check, 2 = without), compact the others into the DP list (one atomic) and reduce the claimed results per read
 //    (64-bit make_best_key in shared memory).  Every read's best_key / score / end / strand is written here (none: 0 / INT_MIN /
@@ -328,10 +358,14 @@ pipe_resolve_reads_kernel(const FmIndex f, const PipeGeom g, const uint2* __rest
     const bool live = r < g.n_reads;
     const uint2* rr = ranges + (size_t)r * per_read;            // this read's ranges: q = (r * strands + strand) * seeds + k
 
-    // hit slots
-    uint32_t hits = 0, run = 0;
+    // hit slots, and which of the read's first 32 ranges are non-empty: phase A visits only those
+    const bool vec = ((per_read | (uint32_t)((size_t)ranges >> 3)) & 1u) == 0u;
+    uint32_t hits = 0, run = 0, nonempty = 0;
     if (live)
-        for (uint32_t q = 0; q < per_read; ++q) hits += seed_range_hits(rr[q], g.max_seed_hits);
+        for (uint32_t q0 = 0; q0 < per_read; q0 += 16u) {
+            const uint32_t m = range_batch<16>(rr, q0, per_read, vec, g.max_seed_hits, hits);
+            if (q0 < 32u) nonempty |= m << q0;
+        }
     if (tile == 0) {
         uint32_t aggregate;
         BlockScan(s_tmp.scan).ExclusiveSum(hits, run, aggregate);
@@ -346,38 +380,52 @@ pipe_resolve_reads_kernel(const FmIndex f, const PipeGeom g, const uint2* __rest
         counts[0] = total < hit_capacity ? total : hit_capacity;
     }
 
-    // phase A
+    // phase A: the non-empty ranges in seed order, RJ_BATCH at a time (their loads issued together, then walked one by one)
     if (live) {
         uint32_t lk_s[RJ_LOCAL], lk_b[RJ_LOCAL], lk_e[RJ_LOCAL];
         int n_local = 0;
-        for (uint32_t strand = 0; strand < g.strands; ++strand) {
-            const uint32_t s = r * g.strands + strand;
-            const uint32_t len = slen[s];
-            for (uint32_t k = 0; k < g.seeds_per_string; ++k) {
-                const uint2 rq = rr[strand * g.seeds_per_string + k];
-                const bool located = rq.y == 0xFFFFFFFFu;                              // already a text position (fm_match_locate_one)
-                const uint32_t sz = seed_range_hits(rq, g.max_seed_hits);
-                if (sz == 0u) continue;
-                const uint32_t base = run, x = rq.x, seed_begin = k * g.seed_interval;
-                run += sz;
-                for (uint32_t j = 0; j < sz; ++j) {
-                    const uint32_t h = base + j;
-                    if (h >= hit_capacity) break;                                      // beyond the caller's capacity
-                    const uint2 w = hit_window(located ? x : fm_locate_one(f, x + j), seed_begin, len, g);
-                    bool seen = false;
+        const uint32_t len0 = slen[r * g.strands], len1 = g.strands > 1u ? slen[r * g.strands + 1u] : 0u;
+        for (uint32_t q0 = 0; q0 < per_read; q0 += 32u) {
+            uint32_t m = q0 ? 0u : nonempty, unused = 0;
+            if (q0)                                                                    // reads of more than 32 ranges
+                for (uint32_t b = 0; b < 32u; b += 8u) m |= range_batch<8>(rr, q0 + b, per_read, vec, g.max_seed_hits, unused) << b;
+            while (m) {
+                uint32_t bq[RJ_BATCH], nb = 0;
+                uint2 brq[RJ_BATCH];
 #pragma unroll
-                    for (int e = 0; e < RJ_LOCAL; ++e) seen |= (e < n_local) && lk_s[e] == s && lk_b[e] == w.x && lk_e[e] == w.y;
-                    if (seen) continue;
+                for (uint32_t e = 0; e < RJ_BATCH; ++e) { bq[e] = m ? q0 + (uint32_t)__ffs(m) - 1u : 0u; nb += m ? 1u : 0u; m &= m - 1u; }
 #pragma unroll
-                    for (int e = 0; e < RJ_LOCAL; ++e) if (e == n_local) { lk_s[e] = s; lk_b[e] = w.x; lk_e[e] = w.y; }
-                    if (n_local < RJ_LOCAL) ++n_local;
-                    const uint32_t slot = atomicAdd(&s_cnt, 1u);
-                    if (slot < RJ_STAGE) { st_string[slot] = s; st_first[slot] = h; st_toff[slot] = w.x; st_tlen[slot] = w.y - w.x; }
-                    else {                                                             // staging full: straight to both global lists
-                        const uint32_t o = atomicAdd(counts + 2, 1u), d = atomicAdd(dp_count, 1u);
-                        j_string[o] = s; j_first[o] = h;
-                        jobs.p_off[o] = s * g.stride; jobs.p_len[o] = len; jobs.t_off[o] = w.x; jobs.t_len[o] = w.y - w.x;
-                        dp.p_off[d] = s * g.stride; dp.p_len[d] = len; dp.t_off[d] = w.x; dp.t_len[d] = w.y - w.x; dp_job[d] = o;
+                for (uint32_t e = 0; e < RJ_BATCH; ++e) brq[e] = e < nb ? rr[bq[e]] : make_uint2(1u, 0u);
+                for (uint32_t e = 0; e < nb; ++e) {
+                    const uint32_t q = bq[0];
+                    const uint2 rq = brq[0];
+#pragma unroll
+                    for (uint32_t c = 0; c + 1u < RJ_BATCH; ++c) { bq[c] = bq[c + 1]; brq[c] = brq[c + 1]; }   // (registers, not an indexed array)
+                    const uint32_t strand = q < g.seeds_per_string ? 0u : 1u, k = q - strand * g.seeds_per_string;
+                    const uint32_t s = r * g.strands + strand, len = strand ? len1 : len0;
+                    const bool located = rq.y == 0xFFFFFFFFu;                          // already a text position (fm_match_locate_one)
+                    const uint32_t sz = seed_range_hits(rq, g.max_seed_hits);
+                    const uint32_t base = run, x = rq.x, seed_begin = k * g.seed_interval;
+                    run += sz;
+                    for (uint32_t j = 0; j < sz; ++j) {
+                        const uint32_t h = base + j;
+                        if (h >= hit_capacity) break;                                  // beyond the caller's capacity
+                        const uint2 w = hit_window(located ? x : fm_locate_one(f, x + j), seed_begin, len, g);
+                        bool seen = false;
+#pragma unroll
+                        for (int e = 0; e < RJ_LOCAL; ++e) seen |= (e < n_local) && lk_s[e] == s && lk_b[e] == w.x && lk_e[e] == w.y;
+                        if (seen) continue;
+#pragma unroll
+                        for (int e = 0; e < RJ_LOCAL; ++e) if (e == n_local) { lk_s[e] = s; lk_b[e] = w.x; lk_e[e] = w.y; }
+                        if (n_local < RJ_LOCAL) ++n_local;
+                        const uint32_t slot = atomicAdd(&s_cnt, 1u);
+                        if (slot < RJ_STAGE) { st_string[slot] = s; st_first[slot] = h; st_toff[slot] = w.x; st_tlen[slot] = w.y - w.x; }
+                        else {                                                         // staging full: straight to both global lists
+                            const uint32_t o = atomicAdd(counts + 2, 1u), d = atomicAdd(dp_count, 1u);
+                            j_string[o] = s; j_first[o] = h;
+                            jobs.p_off[o] = s * g.stride; jobs.p_len[o] = len; jobs.t_off[o] = w.x; jobs.t_len[o] = w.y - w.x;
+                            dp.p_off[d] = s * g.stride; dp.p_len[d] = len; dp.t_off[d] = w.x; dp.t_len[d] = w.y - w.x; dp_job[d] = o;
+                        }
                     }
                 }
             }

@@ -57,6 +57,8 @@ __host__ __device__ __forceinline__ uint32_t text_window16(const uint32_t g0, co
     return sh ? ((hi << sh) | (lo >> (32u - sh))) : hi;
 }
 
+constexpr uint32_t SHORTCUT_WORDS = 10;     // read words per load batch of gapless_job_shortcut's diagonal pass (a 150 bp read: one batch)
+
 // Exact shortcut of the LOCAL banded extension for a read that lies on its seed's diagonal with few differences -- most reads of a real
 // run.  With m = match > 0 > s = mismatch, gap-open penalties < 0 and gap-extension penalties <= 0, every gap costs at least
 // o = -max(pattern_gap_open, text_gap_open) > 0.  Let T be the best segment of the seed's diagonal j0 and delta = m * M - T:
@@ -90,20 +92,35 @@ __host__ __device__ inline bool gapless_job_shortcut(const uint32_t* __restrict_
     // one pass over the seed's diagonal: its differences (at most mm_max, else the DP), its first two and last two differing rows, and,
     // from the runs of equal symbols between them, the maximum-sum segment with the LAST end among equals.  (mismatch < 0, so h peaks at
     // the ends of runs; a symbol-by-symbol version of this loop cost 1,500 warp instructions per job)
+    // The read and diagonal words are loaded SHORTCUT_WORDS (+1) at a time, every load of a batch issued before the first comparison, so
+    // a job pays one memory round trip per batch instead of one per 16 symbols (job_diff_bits on the same words: the read starts on a
+    // word, the diagonal is a funnel shift of two consecutive text words, and no word past the window's last one is touched).
     int32_t h = 0, best = 0, f1 = (int32_t)M, f2 = (int32_t)M, l1 = -1, l2 = -1; uint32_t end = 0, prev = 0, mm0 = 0;
-    for (uint32_t i = 0; i < M && mm0 <= mm_max; i += 16u) {
-        const uint32_t cnt = M - i < 16u ? M - i : 16u;
-        uint32_t d = job_diff_bits(str_words, genome, po, to + j0, i, cnt);
-        while (d && mm0 <= mm_max) {
-            const uint32_t bit = 31u - nvb_clz(d);                          // highest set bit = first differing symbol of the word
-            const uint32_t p = i + (cnt - 1u - (bit >> 1));
-            d &= ~(1u << bit);
-            h += match * (int32_t)(p - prev);
-            if (h >= best) { best = h; end = p; }
-            h += mismatch; h = h > 0 ? h : 0;
-            if (mm0 == 0u) f1 = (int32_t)p; else if (mm0 == 1u) f2 = (int32_t)p;
-            l2 = l1; l1 = (int32_t)p;
-            prev = p + 1u; ++mm0;
+    const uint32_t wr = po >> 4, wt = (to + j0) >> 4, sht = 2u * ((to + j0) & 15u), wlast = (to + N - 1u) >> 4;
+    for (uint32_t kb = 0; kb * 16u < M && mm0 <= mm_max; kb += SHORTCUT_WORDS) {
+        uint32_t rw[SHORTCUT_WORDS], tw[SHORTCUT_WORDS + 1];
+#pragma unroll
+        for (uint32_t q = 0; q < SHORTCUT_WORDS; ++q) rw[q] = (kb + q) * 16u < M ? str_words[wr + kb + q] : 0u;
+#pragma unroll
+        for (uint32_t q = 0; q <= SHORTCUT_WORDS; ++q) tw[q] = wt + kb + q <= wlast ? genome[wt + kb + q] : 0u;
+#pragma unroll
+        for (uint32_t q = 0; q < SHORTCUT_WORDS; ++q) {
+            const uint32_t i = (kb + q) * 16u;
+            if (i >= M || mm0 > mm_max) break;
+            const uint32_t cnt = M - i < 16u ? M - i : 16u;
+            const uint32_t x = (rw[q] ^ (sht ? (tw[q] << sht) | (tw[q + 1] >> (32u - sht)) : tw[q])) >> (32u - 2u * cnt);
+            uint32_t d = (x | (x >> 1)) & 0x55555555u;
+            while (d && mm0 <= mm_max) {
+                const uint32_t bit = 31u - nvb_clz(d);                      // highest set bit = first differing symbol of the word
+                const uint32_t p = i + (cnt - 1u - (bit >> 1));
+                d &= ~(1u << bit);
+                h += match * (int32_t)(p - prev);
+                if (h >= best) { best = h; end = p; }
+                h += mismatch; h = h > 0 ? h : 0;
+                if (mm0 == 0u) f1 = (int32_t)p; else if (mm0 == 1u) f2 = (int32_t)p;
+                l2 = l1; l1 = (int32_t)p;
+                prev = p + 1u; ++mm0;
+            }
         }
     }
     if (mm0 > mm_max) return false;
