@@ -894,6 +894,41 @@ int nvb_bam_index(const uint8_t* d_records, const uint64_t* d_offsets, uint32_t 
                   uint32_t n_refs, uint32_t max_ref_len, const nvb_bai_out* out, void* d_temp, size_t* temp_bytes, void* stream);
 
 /* -------------------------------------------------------------------------------------------
+ * SAM text of BAM records on the device, byte-identical to htslib's sam_format1 (contrib/htslib/sam.c:879-997; nvBowtie's SAM writer,
+ * nvbio/io/output/output_sam.cpp).  Asynchronous on `stream`, no host round trip; NVB_E_TEMP_SIZE protocol.
+ *
+ * Input: n records laid out as nvb_bam_sort accepts them (the outputs of nvb_bam_records, nvb_bam_records_all and nvb_bam_sort as they
+ * are): record i = bytes [d_offsets[i], d_offsets[i + 1]) of d_records, starting with its block_size, at any byte offset.  Reference
+ * names: bytes d_ref_names, name j = [d_ref_name_offsets[j], d_ref_name_offsets[j + 1]), in the order of the BAM header's reference list.
+ * Line i is record i formatted as sam_format1 formats it, then '\n':
+ *   QNAME (l_read_name - 1 bytes), FLAG;  RNAME, '*' for refID -1;  POS + 1 (an unplaced record prints 0);  MAPQ;
+ *   CIGAR as <len><op> over "MIDNSHP=X", '*' without ops;  RNEXT: '*' for next_refID -1, '=' when it equals refID, else the name;
+ *   PNEXT + 1;  TLEN signed;  SEQ in "=ACMGRSVTWYHKDBN" and QUAL + 33 ('*' when the first QUAL byte is 0xFF), "*\t*" when l_seq is 0;
+ *   the tags in record order, "\tXX:i:<v>" for types c C s S i I (I unsigned) and "\tXX:Z:<s>" for Z.
+ * Integers are printed in decimal as 32-bit values (POS + 1 and PNEXT + 1 wrap as htslib's int arithmetic does), fields separated by one
+ * TAB.  A record is REJECTED and gets a line of 0 bytes when: block_size + 4 is not its extent; its fixed fields, name, CIGAR, SEQ, QUAL or
+ * a tag run past its end; its name is empty (l_read_name < 2) or not NUL-terminated; refID or next_refID lies outside [-1, n_refs); a CIGAR
+ * op is above 8; a tag type is not one of c C s S i I Z, or a Z value has no NUL; or 1-3 bytes are left after its last tag.
+ * (Tag types A f d H B are never written by this library's record writers and are not formatted.)
+ *
+ * Output (nvb_sam_out): line i occupies bytes [d_offsets[i], d_offsets[i + 1]) of d_text, '\n' included; d_offsets[n] is the total.
+ * d_offsets is always written whole; a line is stored only if it fits whole within `capacity`, so the stored lines are a prefix (d_text
+ * may be NULL when capacity is 0: a sizing call).  d_rejected[0] = rejected records, d_rejected[1] = the index of the first, 0xFFFFFFFF
+ * when none.  n = 0 writes d_offsets[0] = 0 and d_rejected = (0, 0xFFFFFFFF).
+ * NVB_E_INVALID (before any CUDA call) for a NULL out / temp_bytes / d_offsets / d_rejected, a NULL d_text with capacity > 0, NULL records
+ * with n > 0, NULL names with n_refs > 0, or n >= 2^31 - 1. */
+typedef struct nvb_sam_out {
+    char*     d_text;
+    uint64_t  capacity;
+    uint64_t* d_offsets;               /* [n + 1] */
+    uint32_t* d_rejected;              /* [2] */
+} nvb_sam_out;
+
+int nvb_sam_format(const uint8_t* d_records, const uint64_t* d_offsets, uint32_t n,
+                   const char* d_ref_names, const uint32_t* d_ref_name_offsets, uint32_t n_refs,
+                   const nvb_sam_out* out, void* d_temp, size_t* temp_bytes, void* stream);
+
+/* -------------------------------------------------------------------------------------------
  * Host-buffer entry point: batches of reads in HOST memory in, per-read results in HOST memory out.
  * Replaces nvBowtie's input thread -> compute thread hand-off and its per-stage cudaDeviceSynchronize
  * (nvBowtie/bowtie2/cuda/compute_thread.cu:213-243, nvBowtie/bowtie2/cuda/defs.h:64, aligner_best_approx.h:219-241):

@@ -13,3 +13,4 @@ from .finish import finish_alignments, FinishedAlignments                       
 from .bam import ContigTable, BamRecords, bam_records, bam_records_all, bam_header, write_bam, numbered_names    # noqa: F401
 from .bgzf import BgzfBlocks, BgzfCall, bgzf_compress                           # noqa: F401
 from .bam_sort import SortedBamRecords, sort_bam_records, bam_index, write_sorted_bam    # noqa: F401
+from .sam import SamText, SamCall, sam_header, sam_text, write_sam                  # noqa: F401

@@ -15,7 +15,7 @@ EXPORTS = [
     "nvb_dict_rank", "nvb_dict_rank4", "nvb_dict_build_occ",
     "nvb_map_seeds", "nvb_fm_locate_init", "nvb_fm_locate_lookup", "nvb_fm_locate_sorted",
     "nvb_pipeline_create", "nvb_pipeline_submit", "nvb_pipeline_wait", "nvb_pipeline_traffic", "nvb_pipeline_destroy",
-    "nvb_finish_alignments", "nvb_bam_records", "nvb_bam_records_all", "nvb_bgzf_compress", "nvb_bam_sort", "nvb_bam_index",
+    "nvb_finish_alignments", "nvb_bam_records", "nvb_bam_records_all", "nvb_bgzf_compress", "nvb_bam_sort", "nvb_bam_index", "nvb_sam_format",
 ]
 # test / tuning hooks of include/nvbio_b200_debug.h (not part of the drop-in ABI)
 DEBUG_EXPORTS = [
@@ -89,6 +89,10 @@ class BamSortOutStruct(C.Structure):      # nvb_bam_sort_out
 
 class BaiOutStruct(C.Structure):          # nvb_bai_out
     _fields_ = [("d_bai", C.c_void_p), ("capacity", C.c_uint64), ("d_size", C.c_void_p), ("d_status", C.c_void_p)]
+
+
+class SamOutStruct(C.Structure):          # nvb_sam_out
+    _fields_ = [("d_text", C.c_void_p), ("capacity", C.c_uint64), ("d_offsets", C.c_void_p), ("d_rejected", C.c_void_p)]
 
 
 class MapqParamsStruct(C.Structure):       # nvb_mapq_params

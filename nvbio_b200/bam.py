@@ -55,6 +55,16 @@ class ContigTable:
             self._dev[dev] = torch.from_numpy(self.begin.astype(np.uint32).view(np.int32)).to(dev)
         return self._dev[dev]
 
+    def device_names(self, dev="cuda"):
+        """(bytes, offsets) of the names on the device: name j = bytes[offsets[j]:offsets[j + 1]], offsets uint32 [n + 1] (int32 tensor)"""
+        dev = torch.device(dev)
+        key = ("names", dev)
+        if key not in self._dev:
+            raw = [nm.encode() for nm in self.names]
+            off = np.concatenate([[0], np.cumsum([len(b) for b in raw])]).astype(np.uint32)
+            self._dev[key] = (torch.frombuffer(bytearray(b"".join(raw)), dtype=torch.uint8).to(dev), torch.from_numpy(off.view(np.int32)).to(dev))
+        return self._dev[key]
+
 
 def numbered_names(n: int, prefix: str = "r") -> List[str]:
     """read names prefix0, prefix1, ... for synthetic runs"""
@@ -231,11 +241,8 @@ def bam_records_all(al, finished: FinishedAlignments, reads: PackedStringSet, co
 
 def bam_header(contigs: ContigTable, program: str = "nvbio_b200", sort_order: str = "unsorted") -> bytes:
     """BAM header bytes: magic, the SAM header text (@HD with SO:sort_order, one @SQ per contig, @PG) and the reference list"""
-    if sort_order not in ("unknown", "unsorted", "queryname", "coordinate"):
-        raise ValueError("bam_header: sort_order %r is not one of the SAM specification's" % sort_order)
-    text = "@HD\tVN:1.0\tSO:%s\n" % sort_order + "".join("@SQ\tSN:%s\tLN:%d\n" % (nm, ln) for nm, ln in zip(contigs.names, contigs.lengths)) + \
-        "@PG\tID:%s\tPN:%s\n" % (program, program)
-    t = text.encode()
+    from .sam import sam_header
+    t = sam_header(contigs, program, sort_order).encode()
     out = [b"BAM\1", struct.pack("<i", len(t)), t, struct.pack("<i", len(contigs.names))]
     for nm, ln in zip(contigs.names, contigs.lengths):
         b = nm.encode() + b"\0"

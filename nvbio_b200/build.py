@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libnvbio_b200.so")
-SOURCES = ["fm_kernels.cu", "gotoh_kernels.cu", "sa_build.cu", "pipeline.cu", "host_pipeline.cu", "map_kernels.cu", "finish.cu", "bam.cu", "bgzf.cu", "bam_sort.cu"]
+SOURCES = ["fm_kernels.cu", "gotoh_kernels.cu", "sa_build.cu", "pipeline.cu", "host_pipeline.cu", "map_kernels.cu", "finish.cu", "bam.cu", "bgzf.cu", "bam_sort.cu", "sam.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
          "-Wno-deprecated-declarations", "-Xcompiler", "-fPIC"] + os.environ.get("NVB_NVCC_EXTRA", "").split()
