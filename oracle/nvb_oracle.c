@@ -515,11 +515,12 @@ void orc_banded_gotoh_window(int B, int type, const orc_scheme* S, const i32* qt
  * full M x B direction matrix visits the same cells with the same bits.
  * ops: the backtracer's pushes in END -> START order (0 SUBSTITUTION 'M', 1 INSERTION 'I', 2 DELETION 'D');
  * clips = (M - sink.y, source.y).  Returns the number of ops (may exceed max_ops: then truncated).
+ * Substitution scores as orc_banded_gotoh_one: qtab == NULL -> the scheme's constants, else qtab[2*qq] / qtab[2*qq+1] with qq = Q[i].
  * ---------------------------------------------------------------------------------------------- */
 enum { D_SUB = 0, D_INS = 1, D_DEL = 2, D_SINK = 3, D_INS_EXT = 4, D_DEL_EXT = 8 };
 
-u32 orc_banded_traceback_one(int B, int type, const orc_scheme* S,
-                             const u8* P, u32 M, const u8* T, u32 N,
+u32 orc_banded_traceback_one(int B, int type, const orc_scheme* S, const i32* qtab,
+                             const u8* P, const u8* Q, u32 M, const u8* T, u32 N,
                              i32* out_score, u32* sink_xy, u32* source_xy, u8* ops, u32 max_ops, u32* clips)
 {
     i32 best = ORC_SINK_MIN; u32 bx = 0xFFFFFFFFu, by = 0xFFFFFFFFu;
@@ -534,10 +535,12 @@ u32 orc_banded_traceback_one(int B, int type, const orc_scheme* S,
     for (int j = 1; j < B; ++j) H[j] = (type == 0) ? S->text_gap_open + (j - 1) * S->text_gap_ext : 0;
     for (int j = 0; j < B; ++j) F[j] = INF;
     for (int j = 0; j < B - 1; ++j) { const u32 g = ((u32)j < N) ? T[j] : 255u; cache[j] = packed_cache ? (g & 3u) : g; }
-#define SUB(g, q) (((u8)(g) == (q)) ? S->match : S->mismatch)
+#define SUB(g, q) (((u8)(g) == (q)) ? s_eq : s_ne)
     for (u32 i = 0; i < M; ++i)
     {
         const u8 q = P[i];
+        const u8 qq = Q ? Q[i] : 0;
+        const i32 s_eq = qtab ? qtab[2 * qq] : S->match, s_ne = qtab ? qtab[2 * qq + 1] : S->mismatch;
         u8 edir = D_SUB;
         {   /* j = 0 */
             const i32 ftop = F[1] + Ge, htop = H[1] + Go;
@@ -619,13 +622,13 @@ u32 orc_banded_traceback_one(int B, int type, const orc_scheme* S,
     return n_ops;
 }
 
-void orc_banded_traceback(int B, int type, const orc_scheme* S,
-                          const u8* pat, const u32* p_off, const u32* p_len,
+void orc_banded_traceback(int B, int type, const orc_scheme* S, const i32* qtab,
+                          const u8* pat, const u8* qual, const u32* p_off, const u32* p_len,
                           const u8* txt, const u32* t_off, const u32* t_len, u32 n, u32 max_ops,
                           i32* score, u32* sink_xy, u32* source_xy, u8* ops, u32* n_ops, u32* clips)
 {
     for (u32 i = 0; i < n; ++i)
-        n_ops[i] = orc_banded_traceback_one(B, type, S, pat + p_off[i], p_len[i], txt + t_off[i], t_len[i],
+        n_ops[i] = orc_banded_traceback_one(B, type, S, qtab, pat + p_off[i], qual ? qual + p_off[i] : NULL, p_len[i], txt + t_off[i], t_len[i],
                                             &score[i], &sink_xy[2 * i], &source_xy[2 * i], ops + (size_t)i * max_ops, max_ops, &clips[2 * i]);
 }
 
@@ -695,8 +698,9 @@ void orc_gotoh_full(int type, const orc_scheme* S, const i32* qtab,
  * bits say whether E / F were extended rather than opened.  Walk from the sink: H -> follow hdir; E -> push INSERTION, column-1,
  * stay in E while the bit is set; F likewise with DELETION, row-1.  SEMI_GLOBAL / GLOBAL finish along the first row
  * (INSERTIONs), GLOBAL along the first column (DELETIONs).  ops in END -> START order; clips = (M - sink.y, source.y).
+ * Substitution scores as orc_gotoh_full_one (qtab / Q may be NULL).
  * ---------------------------------------------------------------------------------------------- */
-u32 orc_gotoh_full_traceback_one(int type, const orc_scheme* S, const u8* P, u32 M, const u8* T, u32 N,
+u32 orc_gotoh_full_traceback_one(int type, const orc_scheme* S, const i32* qtab, const u8* P, const u8* Q, u32 M, const u8* T, u32 N,
                                  i32* out_score, u32* sink_xy, u32* source_xy, u8* ops, u32 max_ops, u32* clips)
 {
     i32 best = ORC_SINK_MIN; u32 bx = 0xFFFFFFFFu, by = 0xFFFFFFFFu;
@@ -721,7 +725,8 @@ u32 orc_gotoh_full_traceback_one(int type, const orc_scheme* S, const u8* P, u32
             const i32 eleft = E + Ge, hleft = H[r * W + c - 1] + Go;
             E = imax(eleft, hleft);
             const u8 edir = eleft > hleft ? D_INS_EXT : D_SUB;
-            const i32 diagonal = H[(r - 1) * W + c - 1] + ((T[r - 1] == P[c - 1]) ? S->match : S->mismatch);
+            const i32 s_eq = qtab ? qtab[2 * (Q ? Q[c - 1] : 0)] : S->match, s_ne = qtab ? qtab[2 * (Q ? Q[c - 1] : 0) + 1] : S->mismatch;
+            const i32 diagonal = H[(r - 1) * W + c - 1] + ((T[r - 1] == P[c - 1]) ? s_eq : s_ne);
             const i32 top = f, left = E;
             i32 h = imax(imax(left, top), diagonal);
             if (type == 1) h = imax(h, 0);
@@ -772,12 +777,12 @@ u32 orc_gotoh_full_traceback_one(int type, const orc_scheme* S, const u8* P, u32
     return n_ops;
 }
 
-void orc_gotoh_full_traceback(int type, const orc_scheme* S,
-                              const u8* pat, const u32* p_off, const u32* p_len,
+void orc_gotoh_full_traceback(int type, const orc_scheme* S, const i32* qtab,
+                              const u8* pat, const u8* qual, const u32* p_off, const u32* p_len,
                               const u8* txt, const u32* t_off, const u32* t_len, u32 n, u32 max_ops,
                               i32* score, u32* sink_xy, u32* source_xy, u8* ops, u32* n_ops, u32* clips)
 {
     for (u32 i = 0; i < n; ++i)
-        n_ops[i] = orc_gotoh_full_traceback_one(type, S, pat + p_off[i], p_len[i], txt + t_off[i], t_len[i],
+        n_ops[i] = orc_gotoh_full_traceback_one(type, S, qtab, pat + p_off[i], qual ? qual + p_off[i] : NULL, p_len[i], txt + t_off[i], t_len[i],
                                                 &score[i], &sink_xy[2 * i], &source_xy[2 * i], ops + (size_t)i * max_ops, max_ops, &clips[2 * i]);
 }

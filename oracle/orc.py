@@ -158,13 +158,13 @@ class Oracle(_Base):
         return score, sx, sy, ok
 
 
-def _oracle_traceback(self, band, typ, scheme, pat, p_off, p_len, txt, t_off, t_len, max_ops=512):
-    """Oracle.banded_traceback: ops in END->START push order (0 M, 1 I, 2 D), clips = (M - sink.y, source.y)"""
+def _oracle_traceback(self, band, typ, scheme, pat, p_off, p_len, txt, t_off, t_len, max_ops=512, qual=None, qtab=None):
+    """Oracle.banded_traceback: ops in END->START push order (0 M, 1 I, 2 D), clips = (M - sink.y, source.y); optional per-base
+    qualities + 256x2 score table as in banded_gotoh"""
     pat, p_off, p_len, txt, t_off, t_len, n, o = _tb_args(pat, p_off, p_len, txt, t_off, t_len, max_ops)
-    if len(scheme) == 4:
-        scheme = (scheme[0], scheme[1], scheme[2], scheme[3], scheme[2], scheme[3])
-    s = np.array(scheme, dtype=np.int32)
-    self.lib.orc_banded_traceback(C.c_int(band), C.c_int(typ), _p(s), _p(pat), _p(p_off), _p(p_len), _p(txt), _p(t_off), _p(t_len),
+    s = _scheme6(scheme)
+    qual, qtab = _qual_args(qual, qtab)
+    self.lib.orc_banded_traceback(C.c_int(band), C.c_int(typ), _p(s), _p(qtab), _p(pat), _p(qual), _p(p_off), _p(p_len), _p(txt), _p(t_off), _p(t_len),
                                   C.c_uint32(n), C.c_uint32(max_ops), _p(o["score"]), _p(o["sink"]), _p(o["source"]), _p(o["ops"]),
                                   _p(o["n_ops"]), _p(o["clips"]))
     return o
@@ -195,16 +195,26 @@ def _oracle_window(self, band, typ, scheme, pat, p_off, p_len, txt, t_off, t_len
     return state
 
 
-def _oracle_full_traceback(self, typ, scheme, pat, p_off, p_len, txt, t_off, t_len, max_ops=1024):
-    """Oracle.gotoh_full_traceback: aln::alignment_traceback restated; ops END->START (0 M, 1 I, 2 D)"""
+def _oracle_full_traceback(self, typ, scheme, pat, p_off, p_len, txt, t_off, t_len, max_ops=1024, qual=None, qtab=None):
+    """Oracle.gotoh_full_traceback: aln::alignment_traceback restated; ops END->START (0 M, 1 I, 2 D); optional qualities + table"""
     pat, p_off, p_len, txt, t_off, t_len, n, o = _tb_args(pat, p_off, p_len, txt, t_off, t_len, max_ops)
-    if len(scheme) == 4:
-        scheme = (scheme[0], scheme[1], scheme[2], scheme[3], scheme[2], scheme[3])
-    s = np.array(scheme, dtype=np.int32)
-    self.lib.orc_gotoh_full_traceback(C.c_int(typ), _p(s), _p(pat), _p(p_off), _p(p_len), _p(txt), _p(t_off), _p(t_len),
+    s = _scheme6(scheme)
+    qual, qtab = _qual_args(qual, qtab)
+    self.lib.orc_gotoh_full_traceback(C.c_int(typ), _p(s), _p(qtab), _p(pat), _p(qual), _p(p_off), _p(p_len), _p(txt), _p(t_off), _p(t_len),
                                       C.c_uint32(n), C.c_uint32(max_ops), _p(o["score"]), _p(o["sink"]), _p(o["source"]), _p(o["ops"]),
                                       _p(o["n_ops"]), _p(o["clips"]))
     return o
+
+
+def _scheme6(scheme):
+    if len(scheme) == 4:
+        scheme = (scheme[0], scheme[1], scheme[2], scheme[3], scheme[2], scheme[3])
+    return np.array(scheme, dtype=np.int32)
+
+
+def _qual_args(qual, qtab):
+    return (None if qual is None else np.ascontiguousarray(qual, dtype=np.uint8),
+            None if qtab is None else np.ascontiguousarray(qtab, dtype=np.int32))
 
 
 def _tb_args(pat, p_off, p_len, txt, t_off, t_len, max_ops):
@@ -316,6 +326,27 @@ class Ref(_Base):
                                           _p(pat), _p(p_off), _p(p_len), _p(txt), _p(t_off), _p(t_len), C.c_uint32(n), C.c_uint32(max_ops),
                                           _p(o["score"]), _p(o["sink"]), _p(o["source"]), _p(o["ops"]), _p(o["n_ops"]), _p(o["clips"]))
         assert r == 0
+        return o
+
+    def banded_traceback_q(self, band, typ, scheme, pat, p_off, p_len, txt, t_off, t_len, qual, qtab, max_ops=512):
+        """aln::banded_alignment_traceback<band,1024,32> with the table-driven scheme (TableGotohScheme in ref_shim.cpp) and per-base
+        qualities; scheme as banded_gotoh (only its gap costs are used); bands 7 / 15 / 31"""
+        pat, p_off, p_len, txt, t_off, t_len, n, o = _tb_args(pat, p_off, p_len, txt, t_off, t_len, max_ops)
+        qual, qtab = _qual_args(qual, qtab)
+        r = self.lib.ref_banded_traceback_q(C.c_int(band), C.c_int(typ), _p(_scheme6(scheme)), _p(qtab), _p(pat), _p(qual), _p(p_off), _p(p_len),
+                                            _p(txt), _p(t_off), _p(t_len), C.c_uint32(n), C.c_uint32(max_ops),
+                                            _p(o["score"]), _p(o["sink"]), _p(o["source"]), _p(o["ops"]), _p(o["n_ops"]), _p(o["clips"]))
+        assert r == 0, r
+        return o
+
+    def gotoh_full_traceback_q(self, typ, scheme, pat, p_off, p_len, txt, t_off, t_len, qual, qtab, max_ops=1024):
+        """aln::alignment_traceback<256,512,64> with the table-driven scheme and per-base qualities"""
+        pat, p_off, p_len, txt, t_off, t_len, n, o = _tb_args(pat, p_off, p_len, txt, t_off, t_len, max_ops)
+        qual, qtab = _qual_args(qual, qtab)
+        r = self.lib.ref_gotoh_full_traceback_q(C.c_int(typ), _p(_scheme6(scheme)), _p(qtab), _p(pat), _p(qual), _p(p_off), _p(p_len),
+                                                _p(txt), _p(t_off), _p(t_len), C.c_uint32(n), C.c_uint32(max_ops),
+                                                _p(o["score"]), _p(o["sink"]), _p(o["source"]), _p(o["ops"]), _p(o["n_ops"]), _p(o["clips"]))
+        assert r == 0, r
         return o
 
     def generic_rank(self, word_bits, K, text, qi, qc):

@@ -302,6 +302,59 @@ void run_full_traceback(const aln::SimpleGotohScheme scheme,
     }
 }
 
+// the two tracebacks above with the table-driven scheme and the patterns' own base qualities in place of trivial_quality_string()
+template <uint32 BAND, aln::AlignmentType TYPE>
+void run_traceback_q(const TableGotohScheme scheme,
+                   const uint8* pat, const uint8* qual, const uint32* p_off, const uint32* p_len,
+                   const uint8* txt, const uint32* t_off, const uint32* t_len,
+                   uint32 n, uint32 max_ops, int32* score, uint32* sink_xy, uint32* source_xy,
+                   uint8* ops, uint32* n_ops, uint32* clips)
+{
+    #pragma omp parallel for schedule(static)
+    for (int64 i = 0; i < int64(n); ++i)
+    {
+        RecordingBacktracer bt; bt.ops = ops + uint64(i)*max_ops; bt.n = 0; bt.cap = max_ops; bt.n_clips = 0; bt.clips[0] = bt.clips[1] = 0;
+        const aln::Alignment<int32> a = aln::banded_alignment_traceback<BAND,1024u,32u>(
+            aln::make_gotoh_aligner<TYPE>( scheme ),
+            str_view( p_len[i], pat + p_off[i] ),
+            str_view( p_len[i], qual + p_off[i] ),
+            str_view( t_len[i], txt + t_off[i] ),
+            INT_MIN,
+            bt );
+        score[i] = a.score;
+        sink_xy[2*i] = a.sink.x;     sink_xy[2*i+1] = a.sink.y;
+        source_xy[2*i] = a.source.x; source_xy[2*i+1] = a.source.y;
+        n_ops[i] = bt.n;
+        clips[2*i] = bt.clips[0]; clips[2*i+1] = bt.clips[1];
+    }
+}
+
+template <aln::AlignmentType TYPE>
+void run_full_traceback_q(const TableGotohScheme scheme,
+                   const uint8* pat, const uint8* qual, const uint32* p_off, const uint32* p_len,
+                   const uint8* txt, const uint32* t_off, const uint32* t_len,
+                   uint32 n, uint32 max_ops, int32* score, uint32* sink_xy, uint32* source_xy,
+                   uint8* ops, uint32* n_ops, uint32* clips)
+{
+    #pragma omp parallel for schedule(dynamic,4)
+    for (int64 i = 0; i < int64(n); ++i)
+    {
+        RecordingBacktracer bt; bt.ops = ops + uint64(i)*max_ops; bt.n = 0; bt.cap = max_ops; bt.n_clips = 0; bt.clips[0] = bt.clips[1] = 0;
+        const aln::Alignment<int32> a = aln::alignment_traceback<256u,512u,64u>(
+            aln::make_gotoh_aligner<TYPE>( scheme ),
+            str_view( p_len[i], pat + p_off[i] ),
+            str_view( p_len[i], qual + p_off[i] ),
+            str_view( t_len[i], txt + t_off[i] ),
+            INT_MIN,
+            bt );
+        score[i] = a.score;
+        sink_xy[2*i] = a.sink.x;     sink_xy[2*i+1] = a.sink.y;
+        source_xy[2*i] = a.source.x; source_xy[2*i+1] = a.source.y;
+        n_ops[i] = bt.n;
+        clips[2*i] = bt.clips[0]; clips[2*i+1] = bt.clips[1];
+    }
+}
+
 } // anonymous namespace
 
 // generic rank dictionary (SURVEY 8a row a6): the reference's rank_dictionary over a PLAIN big-endian 2-bit PackedStream of 32- or 64-bit
@@ -491,6 +544,41 @@ int ref_gotoh_full_q(int type, const int32* scheme6, const int32* qtab,
     case 0: run_full_q<aln::GLOBAL>     ( s, pat,qual,p_off,p_len, txt,t_off,t_len, n, score,sink_x,sink_y ); return 0;
     case 1: run_full_q<aln::LOCAL>      ( s, pat,qual,p_off,p_len, txt,t_off,t_len, n, score,sink_x,sink_y ); return 0;
     case 2: run_full_q<aln::SEMI_GLOBAL>( s, pat,qual,p_off,p_len, txt,t_off,t_len, n, score,sink_x,sink_y ); return 0;
+    }
+    return -1;
+}
+
+// quality-table tracebacks (scheme6 = {unused, unused, pgo, pge, tgo, tge}): the banded one at every band ref_banded_gotoh_q
+// instantiates, the full-matrix one with patterns up to 256 and texts up to 512 symbols
+int ref_banded_traceback_q(int band, int type, const int32* scheme6, const int32* qtab,
+                           const uint8* pat, const uint8* qual, const uint32* p_off, const uint32* p_len,
+                           const uint8* txt, const uint32* t_off, const uint32* t_len,
+                           uint32 n, uint32 max_ops, int32* score, uint32* sink_xy, uint32* source_xy,
+                           uint8* ops, uint32* n_ops, uint32* clips)
+{
+    TableGotohScheme s; s.tab = qtab; s.pgo = scheme6[2]; s.pge = scheme6[3]; s.tgo = scheme6[4]; s.tge = scheme6[5];
+#define REF_TQ(B) switch (type) { \
+    case 0: run_traceback_q<B,aln::GLOBAL>     ( s, pat,qual,p_off,p_len, txt,t_off,t_len, n, max_ops, score,sink_xy,source_xy,ops,n_ops,clips ); return 0; \
+    case 1: run_traceback_q<B,aln::LOCAL>      ( s, pat,qual,p_off,p_len, txt,t_off,t_len, n, max_ops, score,sink_xy,source_xy,ops,n_ops,clips ); return 0; \
+    case 2: run_traceback_q<B,aln::SEMI_GLOBAL>( s, pat,qual,p_off,p_len, txt,t_off,t_len, n, max_ops, score,sink_xy,source_xy,ops,n_ops,clips ); return 0; } return -1;
+    switch (band) { case 7: REF_TQ(7) case 15: REF_TQ(15) case 31: REF_TQ(31) }
+#undef REF_TQ
+    return -1;
+}
+
+int ref_gotoh_full_traceback_q(int type, const int32* scheme6, const int32* qtab,
+                               const uint8* pat, const uint8* qual, const uint32* p_off, const uint32* p_len,
+                               const uint8* txt, const uint32* t_off, const uint32* t_len,
+                               uint32 n, uint32 max_ops, int32* score, uint32* sink_xy, uint32* source_xy,
+                               uint8* ops, uint32* n_ops, uint32* clips)
+{
+    TableGotohScheme s; s.tab = qtab; s.pgo = scheme6[2]; s.pge = scheme6[3]; s.tgo = scheme6[4]; s.tge = scheme6[5];
+    for (uint32 i = 0; i < n; ++i) if (p_len[i] > 256u || t_len[i] > 512u) return -2;
+    switch (type)
+    {
+    case 0: run_full_traceback_q<aln::GLOBAL>     ( s, pat,qual,p_off,p_len, txt,t_off,t_len, n, max_ops, score,sink_xy,source_xy,ops,n_ops,clips ); return 0;
+    case 1: run_full_traceback_q<aln::LOCAL>      ( s, pat,qual,p_off,p_len, txt,t_off,t_len, n, max_ops, score,sink_xy,source_xy,ops,n_ops,clips ); return 0;
+    case 2: run_full_traceback_q<aln::SEMI_GLOBAL>( s, pat,qual,p_off,p_len, txt,t_off,t_len, n, max_ops, score,sink_xy,source_xy,ops,n_ops,clips ); return 0;
     }
     return -1;
 }

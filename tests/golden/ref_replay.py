@@ -101,9 +101,19 @@ class _Replay:
 _recorders = []
 
 
-def reference():
-    """the live reference library (recording when NVB_RECORD_REF is set), else the stored answers"""
-    if orc.Ref.available():
+def live_exports(symbols):
+    """whether oracle/_ref/libnvbio_ref.so is built and exports every one of `symbols` (an _ref/ built from an older oracle/ref_shim.cpp,
+    used as is where no nvbio tree is at hand to rebuild it, lacks the newer entry points)"""
+    if not orc.Ref.available():
+        return False
+    lib = orc.Ref().lib
+    return all(hasattr(lib, s) for s in symbols)
+
+
+def reference(symbols=()):
+    """the live reference library (recording when NVB_RECORD_REF is set) where it is built and exports `symbols`, else the stored
+    answers"""
+    if live_exports(symbols):
         if os.environ.get("NVB_RECORD_REF"):
             _recorders.append(_Recorder(orc.Ref()))
             return _recorders[-1]

@@ -227,11 +227,11 @@ extern "C" {
 } // extern "C"
 template <int B, int TYPE>
 static void run_traceback(const GotohScheme& S, const uint32_t* pw, uint32_t pbits, uint32_t pbe, const uint32_t* poff, const uint32_t* plen,
-                          const uint32_t* tw, uint32_t tbits, uint32_t tbe, const uint32_t* toff, const uint32_t* tlen, uint32_t n, uint32_t max_ops,
+                          const uint8_t* quals, const uint32_t* tw, uint32_t tbits, uint32_t tbe, const uint32_t* toff, const uint32_t* tlen, uint32_t n, uint32_t max_ops,
                           int32_t* score, uint32_t* sink_xy, uint32_t* source_xy, uint8_t* ops, uint32_t* n_ops) {
     for (uint32_t a = 0; a < n; ++a) {
         std::vector<uint32_t> dirs((size_t)(plen[a] + 1) * DirWords<B>::N);
-        const SinkResult r = gotoh_generic_impl<B, TYPE, true>(S, pw, pbits, pbe, poff[a], plen[a], nullptr, tw, tbits, tbe, toff[a], tlen[a], dirs.data());
+        const SinkResult r = gotoh_generic_impl<B, TYPE, true>(S, pw, pbits, pbe, poff[a], plen[a], quals, tw, tbits, tbe, toff[a], tlen[a], dirs.data());
         score[a] = r.score; sink_xy[2 * a] = r.x; sink_xy[2 * a + 1] = r.y;
         uint32_t sx = 0xFFFFFFFFu, sy = 0xFFFFFFFFu, cnt = 0;
         if (r.x != 0xFFFFFFFFu && r.y != 0xFFFFFFFFu) cnt = gotoh_walk<B, TYPE>(dirs.data(), r, ops + (size_t)a * max_ops, max_ops, sx, sy);
@@ -420,15 +420,18 @@ int hh_gotoh_full_traceback(int type, const int32_t* scheme6,
     return 0;
 }
 
-int hh_gotoh_traceback(int band, int type, const int32_t* scheme6,
-                       const uint32_t* pw, uint32_t pbits, uint32_t pbe, const uint32_t* poff, const uint32_t* plen,
+// qtab (256 x 2) and quals (one per pattern symbol, at the patterns' offsets) may be NULL: the scheme's constants
+int hh_gotoh_traceback(int band, int type, const int32_t* scheme6, const int32_t* qtab,
+                       const uint32_t* pw, uint32_t pbits, uint32_t pbe, const uint32_t* poff, const uint32_t* plen, const uint8_t* quals,
                        const uint32_t* tw, uint32_t tbits, uint32_t tbe, const uint32_t* toff, const uint32_t* tlen, uint32_t n, uint32_t max_ops,
                        int32_t* score, uint32_t* sink_xy, uint32_t* source_xy, uint8_t* ops, uint32_t* n_ops) {
-    GotohScheme S; S.match = scheme6[0]; S.mismatch = scheme6[1]; S.pgo = scheme6[2]; S.pge = scheme6[3]; S.tgo = scheme6[4]; S.tge = scheme6[5]; S.qtab = nullptr; S.one = 1u; S.keymul = 32u;
+    GotohScheme S; S.match = scheme6[0]; S.mismatch = scheme6[1]; S.pgo = scheme6[2]; S.pge = scheme6[3]; S.tgo = scheme6[4]; S.tge = scheme6[5]; S.qtab = qtab; S.one = 1u; S.keymul = 32u;
     switch (band) {
-    case 7:  TYPE_SWITCH(7,  run_traceback, S, pw, pbits, pbe, poff, plen, tw, tbits, tbe, toff, tlen, n, max_ops, score, sink_xy, source_xy, ops, n_ops)
-    case 15: TYPE_SWITCH(15, run_traceback, S, pw, pbits, pbe, poff, plen, tw, tbits, tbe, toff, tlen, n, max_ops, score, sink_xy, source_xy, ops, n_ops)
-    case 31: TYPE_SWITCH(31, run_traceback, S, pw, pbits, pbe, poff, plen, tw, tbits, tbe, toff, tlen, n, max_ops, score, sink_xy, source_xy, ops, n_ops)
+    case 3:  TYPE_SWITCH(3,  run_traceback, S, pw, pbits, pbe, poff, plen, quals, tw, tbits, tbe, toff, tlen, n, max_ops, score, sink_xy, source_xy, ops, n_ops)
+    case 5:  TYPE_SWITCH(5,  run_traceback, S, pw, pbits, pbe, poff, plen, quals, tw, tbits, tbe, toff, tlen, n, max_ops, score, sink_xy, source_xy, ops, n_ops)
+    case 7:  TYPE_SWITCH(7,  run_traceback, S, pw, pbits, pbe, poff, plen, quals, tw, tbits, tbe, toff, tlen, n, max_ops, score, sink_xy, source_xy, ops, n_ops)
+    case 15: TYPE_SWITCH(15, run_traceback, S, pw, pbits, pbe, poff, plen, quals, tw, tbits, tbe, toff, tlen, n, max_ops, score, sink_xy, source_xy, ops, n_ops)
+    case 31: TYPE_SWITCH(31, run_traceback, S, pw, pbits, pbe, poff, plen, quals, tw, tbits, tbe, toff, tlen, n, max_ops, score, sink_xy, source_xy, ops, n_ops)
     }
     return -1;
 }

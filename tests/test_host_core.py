@@ -293,8 +293,8 @@ def test_gotoh_traceback(H, O, band, typ):
         score = np.zeros(n, np.int32); sink = np.zeros((n, 2), np.uint32); source = np.zeros((n, 2), np.uint32)
         ops = np.zeros((n, max_ops), np.uint8); n_ops = np.zeros(n, np.uint32)
         s6 = np.array(scheme + (scheme[2], scheme[3]), np.int32)
-        r = H.hh_gotoh_traceback(C.c_int(band), C.c_int(typ), _p(s6), _p(pw), C.c_uint32(4), C.c_uint32(1), _p(u32(p_off)), _p(u32(p_len)),
-                                 _p(tw), C.c_uint32(2), C.c_uint32(1), _p(u32(t_off)), _p(u32(t_len)), C.c_uint32(n), C.c_uint32(max_ops),
+        r = H.hh_gotoh_traceback(C.c_int(band), C.c_int(typ), _p(s6), None, _p(pw), C.c_uint32(4), C.c_uint32(1), _p(u32(p_off)), _p(u32(p_len)),
+                                 None, _p(tw), C.c_uint32(2), C.c_uint32(1), _p(u32(t_off)), _p(u32(t_len)), C.c_uint32(n), C.c_uint32(max_ops),
                                  _p(score), _p(sink), _p(source), _p(ops), _p(n_ops))
         assert r == 0
         assert np.array_equal(score, want["score"]) and np.array_equal(sink, want["sink"]) and np.array_equal(source, want["source"])
