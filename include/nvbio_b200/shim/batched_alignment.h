@@ -23,6 +23,7 @@
 #include <nvbio_b200/shim/views.h>
 #include <nvbio/alignment/alignment.h>
 #include <nvbio/alignment/batched.h>
+#include <limits>
 
 namespace nvbio {
 namespace aln {
@@ -102,6 +103,88 @@ struct is_accelerated
                               gotoh_scheme_of<aligner_type>::supported &&
                               is_best_sink<sink_type>::value;
 };
+/// Bounds of the DP values a batch can produce, from its scheme and the stream's length bounds: no H exceeds `hi` (a match, or the
+/// best quality-table score, on every row), and no H, E or F of a real path falls below `lo` (the worst single cost on each of the at most
+/// max_pattern_length + max_text_length steps, opening included).  `match` is the scheme's match(0), the reference's give-up rate.
+struct score_range { int64 hi, lo, match; };
+
+template <typename stream_type>
+score_range score_range_of(const stream_type& stream)
+{
+    typedef typename stream_type::aligner_type aligner_type;
+    const nvb_gotoh_scheme s = gotoh_scheme_of<aligner_type>::get( stream.aligner() );
+    const int64 best  = nvbio::max( nvbio::max( int64( s.match ), int64( 0 ) ), int64( s.d_qual_table ? s.qual_table_max : 0 ) );
+    const int64 worst = nvbio::min( nvbio::min( nvbio::min( int64( s.mismatch ), int64( 0 ) ), int64( s.d_qual_table ? s.qual_table_min : 0 ) ),
+                                    nvbio::min( nvbio::min( int64( s.pattern_gap_open ), int64( s.pattern_gap_ext ) ),
+                                                nvbio::min( int64( s.text_gap_open ), int64( s.text_gap_ext ) ) ) );
+    const int64 max_p = stream_binding<stream_type>::max_pattern_length( stream ), max_t = stream_binding<stream_type>::max_text_length( stream );
+    score_range r; r.hi = best * max_p; r.lo = 2 * worst * (max_p + max_t); r.match = s.match;
+    return r;
+}
+
+/// A sink narrower than int32 (BestSink<int16>): the reference computes int32 cell scores and reports them through the sink's own
+/// type -- LOCAL every cell, SEMI_GLOBAL every cell of the last row, GLOBAL one cell -- keeping the best of the NARROWED values, while
+/// the engine reports the int32 best once.  The two agree when every score the alignment type can report fits the sink's type
+/// (GLOBAL always: one report either way; LOCAL reports no negative score); a batch whose bounds allow more runs the reference's kernel.
+template <typename stream_type>
+struct sink_fits
+{
+    typedef typename stream_type::aligner_type  aligner_type;
+    typedef typename stream_type::context_type  context_type;
+    typedef typename std::decay< decltype( std::declval<context_type&>().sink.score ) >::type score_type;
+
+    static bool check(const stream_type& stream)
+    {
+        if (sizeof(score_type) >= sizeof(int32) || gotoh_scheme_of<aligner_type>::TYPE == int(GLOBAL)) return true;
+        const score_range r = score_range_of( stream );
+        const int64 lo = gotoh_scheme_of<aligner_type>::TYPE == int(LOCAL) ? 0 : r.lo;
+        return r.hi <= int64( std::numeric_limits<score_type>::max() ) && lo >= int64( std::numeric_limits<score_type>::min() );
+    }
+};
+
+/// flag[0] |= 1 if some alignment's context.min_score could make the reference's staged unit give up on it: after a window that ends
+/// before the pattern does, it stops when the band's best H < min_score + remaining rows x match (gotoh_banded_inl.h:622-633).  The
+/// band's best H is at least `lo`, so an alignment with min_score + pattern_length x match <= lo is never given up on.
+template <typename stream_type>
+__global__ void give_up_kernel(const stream_type stream, const int64 lo, const int64 match, uint32* flag)
+{
+    typedef typename stream_type::context_type context_type;
+    const uint32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= stream.size()) return;
+    context_type context;
+    if (stream.init_context( i, &context ) &&
+        int64( context.min_score ) + int64( stream.pattern_length( i, &context ) ) * match > lo)
+        atomicOr( flag, 1u );
+}
+
+/// DeviceStagedThreadScheduler: the reference scores 32-row windows (batched_stream.h:128,161-176) and carries the band between them in
+/// short2 checkpoints (utils.h:52, gotoh_banded_inl.h:177-184), which wrap any H or F outside the int16 range, and it gives up on an
+/// alignment whose min_score is out of reach.  The engine's single pass equals those passes when neither can happen: every H, E and F
+/// of a real path within [SHRT_MIN + 32, 32767], and no min_score in reach of a give-up.  Anything else runs the reference's kernel.
+template <typename stream_type>
+struct staged_fits
+{
+    static bool check(const stream_type& stream)
+    {
+        const score_range r = score_range_of( stream );
+        if (r.hi > 32767 || r.lo < int64( std::numeric_limits<int16>::min() ) + 32) return false;
+        const uint32 n = stream.size();
+        if (n == 0u) return true;
+        uint32* d_flag = (uint32*)scratch( SCRATCH_SCORE, sizeof(uint32) );
+        uint32  h_flag = 0u;
+        check_cuda( cudaMemset( d_flag, 0, sizeof(uint32) ), "cudaMemset" );
+        give_up_kernel<<<(n + 127u) / 128u,128>>>( stream, r.lo, r.match, d_flag );
+        check_cuda( cudaMemcpy( &h_flag, d_flag, sizeof(uint32), cudaMemcpyDeviceToHost ), "cudaMemcpy" );
+        return h_flag == 0u;
+    }
+private:
+    static void check_cuda(const cudaError_t e, const char* what) { if (e != cudaSuccess) nvbio::b200::check( NVB_E_INVALID, what ); }
+};
+template <typename stream_type, typename scheduler_type>
+struct scheduler_fits { static bool check(const stream_type&) { return true; } };
+template <typename stream_type>
+struct scheduler_fits<stream_type, DeviceStagedThreadScheduler> { static bool check(const stream_type& s) { return staged_fits<stream_type>::check( s ); } };
+
 template <uint32 BAND_LEN> struct is_band_supported
 {
     static const bool value = (BAND_LEN == 3u || BAND_LEN == 5u || BAND_LEN == 7u || BAND_LEN == 15u || BAND_LEN == 31u || BAND_LEN == 63u);
@@ -290,7 +373,11 @@ struct BandedScoreBatch
         run( stream, temp_size, temp, std::integral_constant<bool,accelerated>() );
     }
 private:
-    void run(const stream_type& stream, uint64, uint8*, std::true_type)  { m_engine.enact( stream, BAND_LEN ); }
+    void run(const stream_type& stream, uint64 temp_size, uint8* temp, std::true_type)
+    {
+        if (sink_fits<stream_type>::check( stream ) && scheduler_fits<stream_type,scheduler_type>::check( stream )) m_engine.enact( stream, BAND_LEN );
+        else                                         run( stream, temp_size, temp, std::false_type() );
+    }
     void run(const stream_type& stream, uint64 temp_size, uint8* temp, std::false_type)
     {
         m_reference.enact( unbound_stream<stream_type>( stream ), temp_size, temp );
@@ -317,7 +404,11 @@ struct ScoreBatch
         run( stream, temp_size, temp, std::integral_constant<bool,accelerated>() );
     }
 private:
-    void run(const stream_type& stream, uint64, uint8*, std::true_type)  { m_engine.enact( stream, 0u ); }
+    void run(const stream_type& stream, uint64 temp_size, uint8* temp, std::true_type)
+    {
+        if (sink_fits<stream_type>::check( stream )) m_engine.enact( stream, 0u );
+        else                                         run( stream, temp_size, temp, std::false_type() );
+    }
     void run(const stream_type& stream, uint64 temp_size, uint8* temp, std::false_type)
     {
         m_reference.enact( unbound_stream<stream_type>( stream ), temp_size, temp );
@@ -346,8 +437,9 @@ struct BatchedBandedAlignmentScore<
         priv::AlignmentStream< GotohAligner<TYPE,SimpleGotohScheme,algorithm_tag>, pattern_set, trivial_quality_string_set, text_set, sink_iterator >,
         DeviceThreadBlockScheduler<BLOCKDIM,MINBLOCKS> > {};
 
-/// banded, staged scheduler (batched_banded_inl.h:170-241): the DPX kernels need no staging, every alignment is scored in one
-/// pass; the results are the same by construction (windowed scoring in consecutive passes == one pass, gotoh_banded_inl.h:132-199)
+/// banded, staged scheduler (batched_banded_inl.h:170-241): the DPX kernels need no staging, every alignment is scored in one pass,
+/// which equals the reference's windowed passes where staged_fits holds (no int16 wrap in its checkpoints, no give-up on min_score);
+/// other batches run the reference's staged kernel
 template <uint32 BAND_LEN,
           AlignmentType TYPE, typename algorithm_tag, typename pattern_set, typename text_set, typename sink_iterator>
 struct BatchedBandedAlignmentScore<

@@ -120,7 +120,10 @@ void map_exact(const ReadsDef::type& read_batch, const FMIndexDef::type fmi, con
     if (b200::is_supported<ReadsDef::type,FMIndexDef::type>::value)
         b200::map_queues( NVB_MAP_EXACT, read_batch, fmi, retry, queues, reseed, hits, params, fw, rc );
     else
+    {
         map_exact_t( read_batch, fmi, rfmi, retry, queues, reseed, hits, params, fw, rc );
+        nvbio::b200::stats().fallbacks++;
+    }
 }
 void map_approx(const ReadsDef::type& read_batch, const FMIndexDef::type fmi, const FMIndexDef::type rfmi, const uint32 retry,
                 const nvbio::cuda::PingPongQueuesView<uint32> queues, uint8* reseed, SeedHitDequeArrayDeviceView hits,
@@ -129,7 +132,10 @@ void map_approx(const ReadsDef::type& read_batch, const FMIndexDef::type fmi, co
     if (b200::is_supported<ReadsDef::type,FMIndexDef::type>::value && 3u * params.seed_len + 1u <= NVB_MAP_MAX_PUSHES)
         b200::map_queues( NVB_MAP_APPROX, read_batch, fmi, retry, queues, reseed, hits, params, fw, rc );
     else
+    {
         map_approx_t( read_batch, fmi, rfmi, retry, queues, reseed, hits, params, fw, rc );
+        nvbio::b200::stats().fallbacks++;
+    }
 }
 void map(const ReadsDef::type& read_batch, const FMIndexDef::type fmi, const FMIndexDef::type rfmi, const uint32 retry,
          const nvbio::cuda::PingPongQueuesView<uint32> queues, uint8* reseed, SeedHitDequeArrayDeviceView hits,
@@ -138,7 +144,7 @@ void map(const ReadsDef::type& read_batch, const FMIndexDef::type fmi, const FMI
     // the dispatch of map_t (mapping_inl.h:816-855)
     if (params.allow_sub)
     {
-        if (params.subseed_len == 0) map_case_pruning_t( read_batch, fmi, rfmi, retry, queues, reseed, hits, params, fw, rc );   // needs the reverse index: reference
+        if (params.subseed_len == 0) { map_case_pruning_t( read_batch, fmi, rfmi, retry, queues, reseed, hits, params, fw, rc ); nvbio::b200::stats().fallbacks++; }   // needs the reverse index: reference
         else                         map_approx( read_batch, fmi, rfmi, retry, queues, reseed, hits, params, fw, rc );
     }
     else

@@ -1,7 +1,7 @@
 // tests/shim/nvbowtie_harness.cu -- TEST INFRASTRUCTURE: a caller of nvBowtie's NON-template mapping entry points (boundary B-A2,
 // nvBowtie/bowtie2/cuda/mapping.h: map_exact / map_approx / map / gather_ranges) written against nvBowtie's own PODs -- ReadsDef::type,
 // FMIndexDef::type, PingPongQueuesView<uint32>, SeedHitDequeArray(DeviceView), ParamsPOD -- exactly as aligner_best_approx.h:150-240
-// drives them.  This ONE object file is linked twice (tests/shim/Makefile):
+// drives them.  This ONE object file is linked twice (oracle/ref_shim.mk):
 //     nvbowtie_harness_ref    + nvBowtie's own mapping.cu, compiled where it lies (its sm_35-era kernels recompiled for sm_90a)
 //     nvbowtie_harness_b200   + tests/shim/nvbowtie_mapping_b200.cu (include/nvbio_b200/shim/nvbowtie_mapping.h) + libnvbio_b200.so
 // Both runs dump, per configuration: every read's deque size, its SeedHits in canonical (sorted) order, the range sizes in pop_top()
@@ -22,6 +22,9 @@
 
 using namespace nvbio;
 using namespace nvbio::bowtie2::cuda;
+
+// defined by the shim's replacement of mapping.cu (tests/shim/nvbowtie_mapping_b200.cu) only
+extern "C" void nvbowtie_shim_calls(unsigned long long* mapped, unsigned long long* fallbacks) __attribute__((weak));
 
 struct Rng
 {
@@ -80,6 +83,10 @@ int main(int argc, char** argv)
             const uint32 dst = rng.below( genome_len - 400u );
             for (uint32 j = 0; j < 300u; ++j) G[dst + j] = uint8( G[src + j] );
         }
+    }
+    {                                                             // a tandem repeat of an 11 bp unit over 5% of the genome: SA ranges ~1,800 rows wide
+        const uint32 src = rng.below( genome_len / 2u ), span = genome_len / 20u;
+        for (uint32 j = 11u; j < span; ++j) G[src + j] = uint8( G[src + j % 11u] );
     }
     std::vector<int32> h_sa( genome_len + 1u );
     gen_sa( genome_len, G, &h_sa[0] );
@@ -151,16 +158,24 @@ int main(int argc, char** argv)
     nvbio::cuda::PingPongQueuesView<uint32> queues;
     queues.in_size = uint32( h_queue.size() ); queues.in_queue = thrust::raw_pointer_cast( d_queue.data() ); queues.out_size = NULL; queues.out_queue = NULL;
 
-    struct Config { const char* name; int algo; uint32 seed_len, max_hits, subseed_len, retry; bool fw, rc; float k, m; };
+    struct Config { const char* name; int algo; uint32 seed_len, max_hits, subseed_len, retry, min_read_len; bool fw, rc; float k, m; };
     const Config configs[] = {
-        { "exact_r0",   0, 22u, 100u,  0u, 0u, true,  true,  1.0f, 0.75f },      // nvBowtie --local defaults: seed interval 1 + 0.75 sqrt(len)
-        { "exact_r1",   0, 20u, 100u,  0u, 1u, true,  true,  1.0f, 1.15f },      // end-to-end interval function, second reseeding round
-        { "exact_fw",   0, 16u, 100u,  0u, 0u, true,  false, 1.0f, 0.75f },
-        { "approx_r0",  1, 22u, 100u, 11u, 0u, true,  true,  1.0f, 0.75f },
-        { "approx_rc",  1, 20u, 100u, 10u, 2u, false, true,  1.0f, 1.15f },
-        { "map_sub",    2, 22u, 100u, 11u, 0u, true,  true,  1.0f, 0.75f },      // through map(): allow_sub with a subseed -> approximate
-        { "map_nosub",  3, 22u, 100u,  0u, 0u, true,  true,  1.0f, 0.75f },      // through map(): no substitutions -> exact
-        { "exact_tiny", 0, 12u,   6u,  0u, 0u, true,  true,  0.0f, 0.40f },      // short seeds, 6-slot deques: they overflow (sizes compared)
+        { "exact_r0",   0, 22u, 100u,  0u, 0u, 20u, true,  true,  1.0f, 0.75f },      // nvBowtie --local defaults: seed interval 1 + 0.75 sqrt(len)
+        { "exact_r1",   0, 20u, 100u,  0u, 1u, 20u, true,  true,  1.0f, 1.15f },      // end-to-end interval function, second reseeding round
+        { "exact_fw",   0, 16u, 100u,  0u, 0u, 20u, true,  false, 1.0f, 0.75f },
+        { "approx_r0",  1, 22u, 100u, 11u, 0u, 20u, true,  true,  1.0f, 0.75f },
+        { "approx_rc",  1, 20u, 100u, 10u, 2u, 20u, false, true,  1.0f, 1.15f },
+        { "map_sub",    2, 22u, 100u, 11u, 0u, 20u, true,  true,  1.0f, 0.75f },      // through map(): allow_sub with a subseed -> approximate
+        { "map_nosub",  3, 22u, 100u,  0u, 0u, 20u, true,  true,  1.0f, 0.75f },      // through map(): no substitutions -> exact
+        { "exact_tiny", 0, 12u,   6u,  0u, 0u, 20u, true,  true,  0.0f, 0.40f },      // short seeds, 6-slot deques: they overflow (sizes compared)
+        // edges: one-slot deques; min_read_len above the seed length (reads of 60..69 bp are filtered, shorter ones too);
+        // the NVB_MAP_MAX_PUSHES gate of map_approx (3 L + 1 ranges per seed): L = 33 is mapped by the shim, L = 34 falls back to
+        // the reference's map_approx_t; map() with allow_sub and no subseed takes the reference's case pruning
+        { "exact_h1",   0, 16u,   1u,  0u, 0u, 20u, true,  true,  1.0f, 0.75f },
+        { "exact_min70",0, 16u, 100u,  0u, 1u, 70u, true,  true,  1.0f, 0.75f },
+        { "approx_s33", 1, 33u, 100u, 16u, 0u, 20u, true,  true,  1.0f, 0.75f },
+        { "approx_s34", 1, 34u, 100u, 17u, 1u, 20u, true,  true,  1.0f, 0.75f },
+        { "approx_h1",  1, 14u,   1u,  7u, 2u, 20u, true,  true,  0.0f, 0.40f },
     };
     const uint32 n_configs = sizeof(configs) / sizeof(configs[0]);
     std::string json = "{\"program\": \"nvbowtie_mapping\", \"reads\": " + std::to_string( n_reads ) + ", \"queue\": " + std::to_string( h_queue.size() );
@@ -170,12 +185,12 @@ int main(int argc, char** argv)
         ParamsPOD params;
         memset( &params, 0, sizeof(params) );
         params.seed_len = cfg.seed_len; params.seed_freq = SimpleFunc( SimpleFunc::SqrtFunc, cfg.k, cfg.m );
-        params.max_hits = cfg.max_hits; params.max_reseed = 2u; params.rep_seeds = 4u; params.subseed_len = cfg.subseed_len; params.min_read_len = 20u;
+        params.max_hits = cfg.max_hits; params.max_reseed = 2u; params.rep_seeds = 4u; params.subseed_len = cfg.subseed_len; params.min_read_len = cfg.min_read_len;
         params.allow_sub = (cfg.algo == 1 || cfg.algo == 2) ? 1u : 0u;
 
         const uint32 arena = n_reads * cfg.max_hits;
         SeedHitDequeArray deques;
-        deques.m_hits.resize( arena ); deques.m_counts.assign( n_reads, 0u ); deques.m_index.assign( n_reads, 0u );
+        deques.m_hits.resize( arena ); deques.m_counts.assign( n_reads, 0u ); deques.m_index.assign( n_reads, 0xFFFFFFFFu );
         deques.m_probs.resize( 2u * size_t(arena) + 1024u ); deques.m_probs_index.assign( n_reads, 0u );
         deques.m_pool.assign( 1u, 0u ); deques.m_probs_pool.assign( 1u, 0u );
         SeedHitDequeArrayDeviceView hits(
@@ -199,10 +214,12 @@ int main(int argc, char** argv)
         cudaMemcpy( h_hindex.data(), thrust::raw_pointer_cast( deques.m_index.data() ),  4u * n_reads, cudaMemcpyDeviceToHost );
         cudaMemcpy( h_reseed.data(), thrust::raw_pointer_cast( d_reseed.data() ), h_queue.size(), cudaMemcpyDeviceToHost );
         cudaMemcpy( h_hits.data(), thrust::raw_pointer_cast( deques.m_hits.data() ), 8u * size_t(arena), cudaMemcpyDeviceToHost );
-        std::vector<uint64> canon; std::vector<uint32> canon_sizes; uint32 total_hits = 0u, overflowed = 0u;
+        std::vector<uint64> canon; std::vector<uint32> canon_sizes, empty_index; uint32 total_hits = 0u, overflowed = 0u;
         for (uint32 r = 0; r < n_reads; ++r)
         {
-            std::vector<uint64> v( h_hits.begin() + h_hindex[r], h_hits.begin() + h_hindex[r] + h_counts[r] );
+            std::vector<uint64> v;
+            if (h_counts[r]) v.assign( h_hits.begin() + h_hindex[r], h_hits.begin() + h_hindex[r] + h_counts[r] );
+            else             empty_index.push_back( h_hindex[r] );      // untouched (0xFFFFFFFF) unless a deque was allocated for the read
             std::sort( v.begin(), v.end() );
             canon.insert( canon.end(), v.begin(), v.end() );
             std::vector<uint32> sz; for (size_t i = 0; i < v.size(); ++i) sz.push_back( uint32( v[i] >> 32 ) & 0xFFFFFu );
@@ -215,6 +232,7 @@ int main(int argc, char** argv)
         dump( out, std::string( cfg.name ) + "_counts.bin", h_counts );
         dump( out, std::string( cfg.name ) + "_sizes.bin",  canon_sizes );
         dump( out, std::string( cfg.name ) + "_reseed.bin", h_reseed );
+        dump( out, std::string( cfg.name ) + "_empty_index.bin", empty_index );
         if (cfg.max_hits >= 100u) dump( out, std::string( cfg.name ) + "_hits.bin", canon );
 
         // gather_ranges over an inclusive scan of the counts, then pop everything
@@ -236,7 +254,13 @@ int main(int argc, char** argv)
                   cfg.name, ms, total_hits, overflowed, (unsigned long long)range_total, pop_order_ok );
         json += buf;
     }
-    json += "}";
+    unsigned long long mapped = 0u, fallbacks = 0u;
+    if (nvbowtie_shim_calls) { nvbowtie_shim_calls( &mapped, &fallbacks ); json += ", \"shim\": 1"; }
+    else json += ", \"shim\": 0";
+    uint32 short_reads = 0u, below_seed = 0u;
+    for (uint32 r = 0; r < n_reads; ++r) { short_reads += lens[r] < 20u; below_seed += lens[r] < 22u; }
+    json += ", \"reads_below_20\": " + std::to_string( short_reads ) + ", \"reads_below_22\": " + std::to_string( below_seed );
+    json += ", \"b200_calls\": {\"mapped\": " + std::to_string( mapped ) + ", \"fallbacks\": " + std::to_string( fallbacks ) + "}}";
     printf( "%s\n", json.c_str() );
     return 0;
 }

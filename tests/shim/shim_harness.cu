@@ -6,7 +6,7 @@
 //                         headers and libnvbio_b200.so is linked -- nothing else changes
 //
 // and run on the same deterministic inputs; every result array is dumped so that the two runs can be compared bit for bit
-// (tools/shim_compare.py).  Two programs:
+// (tests/test_gpu_shim.py; oracle/ref_shim.mk builds both).  Three programs (the third, edges, is described at run_edges):
 //
 //   fmmap <outdir> [genome_len] [n_reads] [read_len]
 //       the seed -> rank -> locate -> diagonal -> window -> banded DP -> best-per-read loop of nvbio's fmmap example
@@ -393,8 +393,10 @@ struct TestStream
         text_string             text;
     };
 
-    TestStream(aligner_type _aligner, const uint32 _count, const uint32* _patterns, const uint32* _text, int16* _scores) :
-        m_aligner( _aligner ), m_count( _count ), m_patterns( storage_iterator( _patterns ) ), m_text( storage_iterator( _text ) ), m_scores( _scores ) {}
+    TestStream(aligner_type _aligner, const uint32 _count, const uint32* _patterns, const uint32* _text, int16* _scores,
+               const int32 _min_score = Field_traits<int32>::min()) :
+        m_aligner( _aligner ), m_count( _count ), m_patterns( storage_iterator( _patterns ) ), m_text( storage_iterator( _text ) ), m_scores( _scores ),
+        m_min_score( _min_score ) {}
 
     NVBIO_FORCEINLINE NVBIO_HOST_DEVICE const aligner_type& aligner() const { return m_aligner; }
     NVBIO_FORCEINLINE NVBIO_HOST_DEVICE uint32 max_pattern_length() const { return M; }
@@ -406,7 +408,7 @@ struct TestStream
     NVBIO_FORCEINLINE NVBIO_HOST_DEVICE
     bool init_context(const uint32 i, context_type* context) const
     {
-        context->min_score = Field_traits<int32>::min();
+        context->min_score = m_min_score;                   // the staged scheduler gives up on alignments that cannot reach it
         context->sink      = aln::BestSink<int32>();
         return (i % 1000u) != 999u;                         // a few alignments are skipped: output() still runs for them
     }
@@ -427,6 +429,7 @@ struct TestStream
     pattern_input   m_patterns;
     text_input      m_text;
     int16*          m_scores;
+    int32           m_min_score;
 };
 
 #if defined(NVBIO_B200_SHIM)
@@ -469,12 +472,13 @@ static void fill_words(Rng& rng, const uint32 alphabet, const uint64 n_symbols, 
 
 template <uint32 BAND_LEN, uint32 M, uint32 N, typename scheduler_type, typename aligner_type>
 static float run_banded_batch(const std::string& out, const char* name, const aligner_type aligner, const uint32 n_tasks,
-                              const thrust::device_vector<uint32>& pat, const thrust::device_vector<uint32>& txt)
+                              const thrust::device_vector<uint32>& pat, const thrust::device_vector<uint32>& txt,
+                              const int32 min_score = Field_traits<int32>::min())
 {
     typedef aln::TestStream<aligner_type,M,N>                                       stream_type;
     typedef aln::BatchedBandedAlignmentScore<BAND_LEN,stream_type,scheduler_type>   batch_type;
     thrust::device_vector<int16> scores( n_tasks, int16(-7) );
-    stream_type stream( aligner, n_tasks, thrust::raw_pointer_cast( pat.data() ), thrust::raw_pointer_cast( txt.data() ), thrust::raw_pointer_cast( scores.data() ) );
+    stream_type stream( aligner, n_tasks, thrust::raw_pointer_cast( pat.data() ), thrust::raw_pointer_cast( txt.data() ), thrust::raw_pointer_cast( scores.data() ), min_score );
     batch_type batch;
     const uint64 temp_size = batch_type::max_temp_storage( M, N, n_tasks );
     thrust::device_vector<uint8> temp( temp_size ? temp_size : 1u );
@@ -617,9 +621,333 @@ static int run_batch(const std::string& out, const uint32 n_tasks)
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------------------
+// program 3: edges -- the same entry points at the shapes where a forwarding layer goes wrong
+// ---------------------------------------------------------------------------------------------------
+// One batch of n alignments against windows of a 2-bit big-endian "genome" (a SparseStringSet of (begin, end) ranges), patterns in a
+// ConcatenatedStringSet.  Per alignment i, a pattern length L (0, 1..40, 60..200, or 700..830: past 801 - BAND_LEN, the longest
+// pattern the packed 16-bit kernels take, so one call mixes both routes) and a window kind:
+//   FULL   L + BAND_LEN - 1 symbols            SHORT1  one symbol fewer           RANDOM  a length in [max(L, 62), L + BAND_LEN - 1]
+//   BELOW  L - 1 symbols (the DP does not run: the sink keeps its defaults)        EMPTY   no symbols
+// and L = 0 (an empty pattern) against a window of 62..67 symbols.
+// Why no other windows: the reference's banded kernel loads the first BAND_LEN - 1 text symbols before it looks at the text's
+// length (gotoh_banded_inl.h:441-442) and reads past a window of fewer than BAND_LEN - 1 symbols that is not shorter than the
+// pattern, so such a window has no defined result.  Every window here that the DP runs on (text_len >= L) has text_len >= BAND_LEN - 1:
+// for L >= 1, FULL and SHORT1 have L + BAND_LEN - 1 and L + BAND_LEN - 2 >= BAND_LEN - 1 symbols and RANDOM at least 62 >= BAND_LEN - 1;
+// an empty pattern gets 62..67.
+// The staged scheduler loads BAND_LEN - 1 symbols from every 32-row window's start (batched_stream.h:161-176), so its batch uses
+// FULL in place of RANDOM (every other kind keeps that load inside the window).
+enum { W_FULL = 0, W_SHORT1, W_RANDOM, W_BELOW, W_EMPTY, W_KINDS };
+static const uint32 EDGE_MAX_P = 830u, EDGE_MIN_T = 62u, EDGE_MAX_BAND = 63u;
+
+struct EdgeInputs
+{
+    uint32 n;
+    std::vector<uint32> genome;                  // 2-bit big-endian words
+    std::vector<uint32> p_len, p_sym_off;        // pattern i: symbols [p_sym_off, +p_len) of the pattern stream
+    std::vector<uint8>  p_sym;                   // 0..3, 4 = N
+    std::vector<uint32> t_begin, kind;           // window i begins at t_begin[i]; its length depends on the band and the kind
+    uint32 genome_len;
+};
+
+static EdgeInputs make_edge_inputs(Rng& rng, const uint32 n)
+{
+    EdgeInputs in; in.n = n;
+    in.genome_len = n * 40u + 4096u;
+    in.genome.assign( in.genome_len / 16u + 8u, 0u );
+    PackedStream<uint32*,uint8,2u,true> G( &in.genome[0] );
+    for (uint32 i = 0; i < in.genome_len; ++i) G[i] = uint8( rng.below( 4u ) );
+    uint32 off = 0u;
+    for (uint32 i = 0; i < n; ++i)
+    {
+        const uint32 c = rng.below( 100u );
+        const uint32 L = c < 3u ? 0u : c < 20u ? 1u + rng.below( 40u ) : c < 90u ? 60u + rng.below( 141u ) : 700u + rng.below( EDGE_MAX_P - 700u + 1u );
+        const uint32 k = L == 0u ? W_RANDOM : (i % 11u == 3u ? W_BELOW : i % 11u == 7u ? W_EMPTY : i % 5u == 1u ? W_SHORT1 : i % 5u == 2u ? W_RANDOM : W_FULL);
+        const uint32 begin = rng.below( in.genome_len - EDGE_MAX_P - EDGE_MAX_BAND - 8u );
+        in.p_len.push_back( L ); in.p_sym_off.push_back( off ); in.t_begin.push_back( begin ); in.kind.push_back( k );
+        // the pattern: the window's text shifted by a few symbols, with substitutions, N's (1 in 8 patterns) and the odd deletion
+        const uint32 shift = rng.below( 4u );
+        const bool with_n = rng.below( 8u ) == 0u;
+        uint32 src = begin + shift;
+        for (uint32 j = 0; j < L; ++j)
+        {
+            if (rng.below( 200u ) == 0u) src += 1u + rng.below( 2u );
+            uint8 s = uint8( G[src++] );
+            const double u = rng.unit();
+            if (u < 0.03) s = uint8( (s + 1u + rng.below( 3u )) & 3u );
+            else if (with_n && u < 0.05) s = 4u;
+            in.p_sym.push_back( s );
+        }
+        off += L;
+    }
+    return in;
+}
+
+static uint32 edge_window_len(const EdgeInputs& in, const uint32 i, const uint32 band, const bool staged, Rng& rng)
+{
+    const uint32 L = in.p_len[i];
+    if (L == 0u) return EDGE_MIN_T + rng.below( 6u );
+    switch (in.kind[i])
+    {
+    case W_SHORT1: return L + band - 2u;
+    case W_BELOW:  return L - 1u;
+    case W_EMPTY:  return 0u;
+    case W_RANDOM: if (!staged) { const uint32 lo = nvbio::max( L, EDGE_MIN_T ), hi = L + band - 1u; return lo >= hi ? hi : lo + rng.below( hi - lo + 1u ); }
+    default:       return L + band - 1u;
+    }
+}
+
+/// the pattern symbols packed BITS per symbol (2-bit patterns: an N becomes A, as a 2-bit packer would store it)
+template <uint32 BITS, bool BE>
+static std::vector<uint32> pack_patterns(const EdgeInputs& in)
+{
+    std::vector<uint32> w( (in.p_sym.size() * BITS + 31u) / 32u + 8u, 0u );
+    PackedStream<uint32*,uint8,BITS,BE> P( &w[0] );
+    for (size_t j = 0; j < in.p_sym.size(); ++j) P[j] = BITS == 2u ? uint8( in.p_sym[j] & 3u ) : in.p_sym[j];
+    return w;
+}
+
+struct EdgeRun
+{
+    std::string out, json;
+    uint32 banded_calls, full_calls, fallback_calls;
+    EdgeRun(const std::string& o) : out( o ), banded_calls( 0u ), full_calls( 0u ), fallback_calls( 0u ) {}
+    void add(const std::string& key, const uint64 v) { json += ", \"" + key + "\": " + std::to_string( v ); }
+};
+
+template <typename sink_type>
+static void dump_sinks(EdgeRun& run, const std::string& name, const thrust::device_vector<sink_type>& sinks, const uint32 n)
+{
+    thrust::device_vector<int32> score( n ); thrust::device_vector<uint2> sink( n );
+    if (n) split_sinks_kernel<<<(n + 255u) / 256u,256>>>( n, thrust::raw_pointer_cast( sinks.data() ), thrust::raw_pointer_cast( score.data() ), thrust::raw_pointer_cast( sink.data() ) );
+    cuda_check( name.c_str() );
+    dump( run.out, (name + "_scores.bin").c_str(), score, n );
+    dump( run.out, (name + "_sinks.bin").c_str(), sink, n );
+}
+
+/// one aln::batch_banded_alignment_score<BAND_LEN> call over the edge inputs (the first n alignments), through priv::AlignmentStream
+template <uint32 BAND_LEN, typename sink_score, uint32 PBITS, bool PBE, typename aligner_type, typename scheduler_type>
+static void edge_banded(EdgeRun& run, const std::string& name, const EdgeInputs& in, const uint32 n, const aligner_type aligner,
+                        const scheduler_type scheduler, const bool staged, const bool fallback = false)
+{
+    typedef PackedStream<const uint32*,uint8,PBITS,PBE>                 pattern_stream;
+    typedef PackedStream<const uint32*,uint8,2u,true>                   text_stream;
+    typedef ConcatenatedStringSet<pattern_stream,const uint32*>         pattern_set;
+    typedef SparseStringSet<text_stream,const uint2*>                   text_set;
+    Rng rng( 0x5851F42D4C957F2Dull + BAND_LEN );                        // window lengths: the same for every call with this band
+    std::vector<uint32> poff( n + 1u ); std::vector<uint2> trange( n );
+    uint32 max_p = 1u, max_t = 1u;
+    for (uint32 i = 0; i < n; ++i)
+    {
+        const uint32 tl = edge_window_len( in, i, BAND_LEN, staged, rng );
+        poff[i] = in.p_sym_off[i]; trange[i] = make_uint2( in.t_begin[i], in.t_begin[i] + tl );
+        max_p = nvbio::max( max_p, in.p_len[i] ); max_t = nvbio::max( max_t, tl );
+    }
+    poff[n] = n ? in.p_sym_off[n-1u] + in.p_len[n-1u] : 0u;
+    const std::vector<uint32> h_pat = pack_patterns<PBITS,PBE>( in );
+    thrust::device_vector<uint32> d_pat( h_pat ), d_txt( in.genome ), d_poff( poff );
+    thrust::device_vector<uint2>  d_trange( trange );
+    const pattern_set patterns( n, pattern_stream( thrust::raw_pointer_cast( d_pat.data() ) ), thrust::raw_pointer_cast( d_poff.data() ) );
+    const text_set    texts( n, text_stream( thrust::raw_pointer_cast( d_txt.data() ) ), thrust::raw_pointer_cast( d_trange.data() ) );
+    thrust::device_vector< aln::BestSink<sink_score> > sinks( nvbio::max( n, 1u ) );
+    aln::batch_banded_alignment_score<BAND_LEN>( aligner, patterns, texts, thrust::raw_pointer_cast( sinks.data() ), scheduler, max_p, max_t );
+    dump_sinks( run, name, sinks, n );
+    if (fallback) run.fallback_calls++; else run.banded_calls++;
+}
+
+/// the same on the harness's user-bound TestStream (fixed M x (M + BAND_LEN) strings, 4-bit little-endian patterns)
+template <uint32 BAND_LEN, typename scheduler_type, typename aligner_type>
+static void edge_test_stream(EdgeRun& run, const char* name, Rng& rng, const uint32 n, const aligner_type aligner, const bool fallback = false,
+                             const int32 min_score = Field_traits<int32>::min())
+{
+    static const uint32 M = 150u, N = M + BAND_LEN;
+    std::vector<uint32> h_txt, h_pat;
+    fill_words<2u>( rng, 4u, uint64(N) * n, h_txt );
+    h_pat.assign( (uint64(M) * n * 4u + 31u) / 32u + 4u, 0u );
+    PackedStream<uint32*,uint8,2u,false> T( &h_txt[0] ); PackedStream<uint32*,uint8,4u,false> P( &h_pat[0] );
+    for (uint32 t = 0; t < n; ++t)
+    {
+        const uint32 shift = rng.below( BAND_LEN / 2u + 1u );
+        for (uint32 j = 0; j < M; ++j)
+        {
+            uint8 c = T[ uint64(t) * N + nvbio::min( j + shift, N - 1u ) ];
+            const double u = rng.unit();
+            if (u < 0.03) c = uint8( rng.below( 4u ) ); else if (u < 0.035) c = 4u;
+            P[ uint64(t) * M + j ] = c;
+        }
+    }
+    thrust::device_vector<uint32> pat( h_pat ), txt( h_txt );
+    run_banded_batch<BAND_LEN,M,N,scheduler_type>( run.out, name, aligner, n, pat, txt, min_score );
+    if (fallback) run.fallback_calls += 3u; else run.banded_calls += 3u;     // run_banded_batch enacts three times
+}
+
+/// full matrix through aln::batch_alignment_score: mixed (M, N) in one batch, some N < M
+template <typename sink_score, typename aligner_type>
+static void edge_full(EdgeRun& run, const std::string& name, const EdgeInputs& in, const uint32 n, const aligner_type aligner)
+{
+    typedef PackedStream<const uint32*,uint8,4u,false>                  pattern_stream;
+    typedef PackedStream<const uint32*,uint8,2u,true>                   text_stream;
+    typedef ConcatenatedStringSet<pattern_stream,const uint32*>         pattern_set;
+    typedef SparseStringSet<text_stream,const uint2*>                   text_set;
+    Rng rng( 0x1B873593ull );
+    // patterns: the first n non-empty patterns of the edge inputs cut to at most 300 symbols; texts of 1..600 symbols, a fifth of them
+    // shorter than their pattern (the full-matrix DP takes every pattern and text length >= 1)
+    std::vector<uint32> poff; std::vector<uint2> trange;
+    uint32 max_p = 1u, max_t = 1u;
+    for (uint32 i = 0; poff.size() < n && i < in.n; ++i)
+    {
+        if (in.p_len[i] == 0u) continue;
+        const uint32 L = nvbio::min( in.p_len[i], 300u );
+        const uint32 tl = rng.below( 5u ) == 0u ? 1u + rng.below( L ) : L + rng.below( 301u );
+        poff.push_back( in.p_sym_off[i] ); trange.push_back( make_uint2( in.t_begin[i], in.t_begin[i] + tl ) );
+        max_p = nvbio::max( max_p, L ); max_t = nvbio::max( max_t, tl );
+    }
+    const uint32 m = uint32( poff.size() );
+    // a ConcatenatedStringSet takes lengths from consecutive offsets: give each pattern its own copy of L symbols instead
+    std::vector<uint8> sym; std::vector<uint32> off( m + 1u );
+    {
+        uint32 t = 0u;
+        for (uint32 i = 0; t < m && i < in.n; ++i)
+        {
+            if (in.p_len[i] == 0u) continue;
+            const uint32 L = nvbio::min( in.p_len[i], 300u );
+            off[t++] = uint32( sym.size() );
+            for (uint32 j = 0; j < L; ++j) sym.push_back( in.p_sym[ in.p_sym_off[i] + j ] );
+        }
+        off[m] = uint32( sym.size() );
+    }
+    std::vector<uint32> h_pat( (sym.size() * 4u + 31u) / 32u + 8u, 0u );
+    { PackedStream<uint32*,uint8,4u,false> P( &h_pat[0] ); for (size_t j = 0; j < sym.size(); ++j) P[j] = sym[j]; }
+    thrust::device_vector<uint32> d_pat( h_pat ), d_txt( in.genome ), d_poff( off );
+    thrust::device_vector<uint2>  d_trange( trange );
+    const pattern_set patterns( m, pattern_stream( thrust::raw_pointer_cast( d_pat.data() ) ), thrust::raw_pointer_cast( d_poff.data() ) );
+    const text_set    texts( m, text_stream( thrust::raw_pointer_cast( d_txt.data() ) ), thrust::raw_pointer_cast( d_trange.data() ) );
+    thrust::device_vector< aln::BestSink<sink_score> > sinks( m );
+    aln::batch_alignment_score( aligner, patterns, texts, thrust::raw_pointer_cast( sinks.data() ), aln::DeviceThreadScheduler(), max_p, max_t );
+    dump_sinks( run, name, sinks, m );
+    run.full_calls++;
+}
+
+static int run_edges(const std::string& out, const uint32 n)
+{
+    Rng rng( 0xA0761D6478BD642Full );
+    const EdgeInputs in = make_edge_inputs( rng, n );
+    EdgeRun run( out );
+    run.json = "{\"program\": \"edges\", \"n\": " + std::to_string( n );
+    // what the batch holds: pattern lengths per route, window kinds, N's
+    {
+        uint64 empty_p = 0u, long_p = 0u, with_n = 0u, kinds[W_KINDS] = { 0u, 0u, 0u, 0u, 0u };
+        for (uint32 i = 0; i < n; ++i)
+        {
+            if (in.p_len[i] == 0u) ++empty_p; else kinds[ in.kind[i] ]++;
+            if (in.p_len[i] > 801u - EDGE_MAX_BAND) ++long_p;
+            for (uint32 j = 0; j < in.p_len[i]; ++j) if (in.p_sym[ in.p_sym_off[i] + j ] == 4u) { ++with_n; break; }
+        }
+        run.add( "empty_patterns", empty_p ); run.add( "long_patterns", long_p ); run.add( "patterns_with_n", with_n );
+        run.add( "full_windows", kinds[W_FULL] ); run.add( "short1_windows", kinds[W_SHORT1] ); run.add( "random_windows", kinds[W_RANDOM] );
+        run.add( "below_windows", kinds[W_BELOW] ); run.add( "empty_windows", kinds[W_EMPTY] );
+    }
+    const aln::SimpleGotohScheme sc( 2, -2, -5, -3 );
+    const aln::DeviceThreadScheduler thread;
+    const aln::DeviceStagedThreadScheduler staged;
+
+    // every band the shim accelerates x the three alignment types, BestSink<int32>, 4-bit little-endian patterns with N's
+#define EDGE_TYPES(B) \
+    edge_banded<B,int32,4u,false>( run, "b" #B "_global", in, n, aln::make_gotoh_aligner<aln::GLOBAL>( sc ), thread, false ); \
+    edge_banded<B,int32,4u,false>( run, "b" #B "_local",  in, n, aln::make_gotoh_aligner<aln::LOCAL>( sc ), thread, false ); \
+    edge_banded<B,int32,4u,false>( run, "b" #B "_semi",   in, n, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( sc ), thread, false ); \
+    edge_banded<B,int16,4u,false>( run, "b" #B "_local_i16", in, n, aln::make_gotoh_aligner<aln::LOCAL>( sc ), thread, false );
+    EDGE_TYPES(3) EDGE_TYPES(5) EDGE_TYPES(7) EDGE_TYPES(15) EDGE_TYPES(31) EDGE_TYPES(63)
+#undef EDGE_TYPES
+    edge_banded<15,int16,4u,false>( run, "b15_global_i16", in, n, aln::make_gotoh_aligner<aln::GLOBAL>( sc ), thread, false );
+    edge_banded<15,int16,4u,false>( run, "b15_semi_i16",   in, n, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( sc ), thread, false );
+    // the other packings: 4-bit big-endian, 2-bit big- and little-endian patterns
+    edge_banded<31,int32,4u,true >( run, "b31_local_p4be",  in, n, aln::make_gotoh_aligner<aln::LOCAL>( sc ), thread, false );
+    edge_banded<31,int32,2u,true >( run, "b31_global_p2be", in, n, aln::make_gotoh_aligner<aln::GLOBAL>( sc ), thread, false );
+    edge_banded<31,int32,2u,false>( run, "b31_semi_p2le",   in, n, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( sc ), thread, false );
+    // the staged scheduler over priv::AlignmentStream
+    edge_banded<15,int32,4u,false>( run, "b15_global_staged", in, n, aln::make_gotoh_aligner<aln::GLOBAL>( sc ), staged, true );
+    edge_banded<63,int32,4u,false>( run, "b63_local_staged",  in, n, aln::make_gotoh_aligner<aln::LOCAL>( sc ), staged, true );
+    edge_banded<3,int16,4u,false> ( run, "b3_semi_staged_i16", in, n, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( sc ), staged, true );
+    // deliberate fall-backs: a band the kernels do not implement runs the reference's own kernel
+    edge_banded<9,int32,4u,false>( run, "b9_local_fallback", in, n, aln::make_gotoh_aligner<aln::LOCAL>( sc ), thread, false, true );
+    // scratch arenas: grow, reuse at the boundaries of the layout kernels' 128-thread blocks, grow again, shrink
+    {
+        const uint32 sizes[6] = { 1u, 127u, 128u, 129u, n, 5u };
+        for (uint32 s = 0; s < 6u; ++s)
+            edge_banded<31,int32,4u,false>( run, "b31_global_n" + std::to_string( sizes[s] ) + "_" + std::to_string( s ), in, sizes[s], aln::make_gotoh_aligner<aln::GLOBAL>( sc ), thread, false );
+    }
+    // scores outside the int16 range: 150 bp near-exact patterns under (300, -200, -500, -300)
+    {
+        Rng r2( 0x9FB21C651E98DF25ull );
+        EdgeInputs big = make_edge_inputs( r2, 2048u );
+        for (uint32 i = 0; i < big.n; ++i) { big.kind[i] = W_FULL; }
+        // cut every pattern to 150 symbols (or keep it shorter) by rebuilding the pattern stream
+        std::vector<uint8> sym; std::vector<uint32> len, off;
+        for (uint32 i = 0; i < big.n; ++i)
+        {
+            const uint32 L = big.p_len[i] == 0u ? 0u : 150u;
+            off.push_back( uint32( sym.size() ) ); len.push_back( L );
+            PackedStream<const uint32*,uint8,2u,true> G( &big.genome[0] );
+            for (uint32 j = 0; j < L; ++j) { uint8 c = uint8( G[ big.t_begin[i] + 3u + j ] ); if (r2.below( 100u ) == 0u) c = uint8( (c + 1u) & 3u ); sym.push_back( c ); }
+        }
+        big.p_sym = sym; big.p_len = len; big.p_sym_off = off;
+        const aln::SimpleGotohScheme wide( 300, -200, -500, -300 );
+        edge_banded<15,int32,4u,false>( run, "wide_b15_global",     big, big.n, aln::make_gotoh_aligner<aln::GLOBAL>( wide ), thread, false );
+        edge_banded<15,int32,4u,false>( run, "wide_b15_local",      big, big.n, aln::make_gotoh_aligner<aln::LOCAL>( wide ), thread, false );
+        edge_banded<15,int32,4u,false>( run, "wide_b15_semi",       big, big.n, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( wide ), thread, false );
+        edge_banded<15,int16,4u,false>( run, "wide_b15_global_i16", big, big.n, aln::make_gotoh_aligner<aln::GLOBAL>( wide ), thread, false );
+        // BestSink<int16>: GLOBAL reports once and stays accelerated; LOCAL and SEMI_GLOBAL keep the best of many narrowed reports, which
+        // one report of the int32 best cannot reproduce once scores leave the int16 range, so the shim runs the reference's kernel
+        edge_banded<15,int16,4u,false>( run, "wide_b15_local_i16",  big, big.n, aln::make_gotoh_aligner<aln::LOCAL>( wide ), thread, false, true );
+        edge_banded<15,int16,4u,false>( run, "wide_b15_semi_i16",   big, big.n, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( wide ), thread, false, true );
+        // the staged scheduler carries the band between 32-row windows in short2 checkpoints: H near 37,000 at row 128 wraps there, so
+        // the reference's staged scores differ from one pass and the shim runs the reference's staged kernel
+        edge_banded<15,int32,4u,false>( run, "wide_b15_global_staged", big, big.n, aln::make_gotoh_aligner<aln::GLOBAL>( wide ), staged, true, true );
+        edge_banded<15,int32,4u,false>( run, "wide_b15_local_staged",  big, big.n, aln::make_gotoh_aligner<aln::LOCAL>( wide ), staged, true, true );
+        edge_banded<15,int32,4u,false>( run, "wide_b15_semi_staged",   big, big.n, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( wide ), staged, true, true );
+    }
+    // the user-bound stream at the outer bands, both schedulers, and one band it does not take
+    {
+        Rng r3( 0xE7037ED1A0B428DBull );
+        const uint32 nt = 4096u;
+        edge_test_stream<3, aln::DeviceThreadScheduler>      ( run, "ts_b3_global_thread", r3, nt, aln::make_gotoh_aligner<aln::GLOBAL>( sc ) );
+        edge_test_stream<63,aln::DeviceStagedThreadScheduler>( run, "ts_b63_semi_staged",  r3, nt, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( sc ) );
+        edge_test_stream<5, aln::DeviceStagedThreadScheduler>( run, "ts_b5_local_staged",  r3, nt, aln::make_gotoh_aligner<aln::LOCAL>( sc ) );
+        edge_test_stream<9, aln::DeviceThreadScheduler>      ( run, "ts_b9_local_fallback", r3, nt, aln::make_gotoh_aligner<aln::LOCAL>( sc ), true );
+        // a min_score in reach (150 bp x match 2 = 300 at most): the staged scheduler gives up on alignments that fall behind after a
+        // 32-row window, so the shim runs the reference's staged kernel; under the thread scheduler min_score changes nothing
+        edge_test_stream<15,aln::DeviceStagedThreadScheduler>( run, "ts_b15_local_staged_min", r3, nt, aln::make_gotoh_aligner<aln::LOCAL>( sc ), true, 200 );
+        edge_test_stream<15,aln::DeviceThreadScheduler>      ( run, "ts_b15_local_thread_min", r3, nt, aln::make_gotoh_aligner<aln::LOCAL>( sc ), false, 200 );
+    }
+    // full matrix
+    {
+        const uint32 nf = nvbio::min( n, 3000u );
+        const aln::SimpleGotohScheme fs( 2, -1, -2, -1 );
+        edge_full<int32>( run, "full_global",     in, nf, aln::make_gotoh_aligner<aln::GLOBAL>( fs ) );
+        edge_full<int32>( run, "full_local",      in, nf, aln::make_gotoh_aligner<aln::LOCAL>( fs ) );
+        edge_full<int32>( run, "full_semi",       in, nf, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( fs ) );
+        edge_full<int16>( run, "full_global_i16", in, nf, aln::make_gotoh_aligner<aln::GLOBAL>( fs ) );
+        edge_full<int16>( run, "full_local_i16",  in, nf, aln::make_gotoh_aligner<aln::LOCAL>( fs ) );
+        edge_full<int16>( run, "full_semi_i16",   in, nf, aln::make_gotoh_aligner<aln::SEMI_GLOBAL>( fs ) );
+    }
+    uint64 b200_calls[3] = { 0u, 0u, 0u };
+#if defined(NVBIO_B200_SHIM)
+    { const nvbio::b200::shim_stats& st = nvbio::b200::stats(); b200_calls[0] = st.banded_score; b200_calls[1] = st.full_score; b200_calls[2] = st.fallbacks; }
+    run.json += ", \"shim\": 1";
+#else
+    run.json += ", \"shim\": 0";
+#endif
+    run.json += ", \"planned\": {\"banded\": " + std::to_string( run.banded_calls ) + ", \"full\": " + std::to_string( run.full_calls ) +
+                ", \"fallbacks\": " + std::to_string( run.fallback_calls ) + "}";
+    run.json += ", \"b200_calls\": {\"banded\": " + std::to_string( b200_calls[0] ) + ", \"full\": " + std::to_string( b200_calls[1] ) + ", \"fallbacks\": " + std::to_string( b200_calls[2] ) + "}}";
+    printf( "%s\n", run.json.c_str() );
+    return 0;
+}
+
 int main(int argc, char** argv)
 {
-    if (argc < 3) { fprintf( stderr, "usage: shim_harness fmmap|batch <outdir> [sizes...]\n" ); return 1; }
+    if (argc < 3) { fprintf( stderr, "usage: shim_harness fmmap|batch|edges <outdir> [sizes...]\n" ); return 1; }
     const std::string mode = argv[1], out = argv[2];
     try
     {
@@ -627,6 +955,8 @@ int main(int argc, char** argv)
             return run_fmmap( out, argc > 3 ? uint32( atoll( argv[3] ) ) : 4000000u, argc > 4 ? uint32( atoll( argv[4] ) ) : 50000u, argc > 5 ? uint32( atoll( argv[5] ) ) : 100u );
         if (mode == "batch")
             return run_batch( out, argc > 3 ? uint32( atoll( argv[3] ) ) : 65536u );
+        if (mode == "edges")
+            return run_edges( out, argc > 3 ? uint32( atoll( argv[3] ) ) : 20000u );
     }
     catch (const std::exception& e) { fprintf( stderr, "exception: %s\n", e.what() ); return 4; }
     return 1;

@@ -1,129 +1,36 @@
-"""The drop-in boundary on the reference's side (SURVEY 8b, B-A1 / B-B1 / B-A2 / B-B2), checked where an nvbio source tree is at hand.
-
-tests/shim/*.cu are programs written against nvbio's own types -- io::FMIndexDataDevice::fm_index_type, FMIndexFilterDevice::rank/locate
-over an InfixSet of 4-bit reads, aln::batch_banded_alignment_score<31>, BatchedBandedAlignmentScore<...>::enact on a user-defined stream,
-aln::batch_alignment_score, nvBowtie's map_* entry points and its best-score extension -- compiled twice by `make -C tests/shim REF=<nvbio
-tree>`: once as is (the reference's own templates and kernels, `_ref`) and once with include/nvbio_b200/shim/*.h + libnvbio_b200.so
-(`_b200`).  Both builds need nvbio's headers (and nvBowtie's sources), so this check cannot be part of the test suite, which runs without
-them.  Run it on a GPU after that build:
+"""Run the drop-in boundary checks of tests/test_gpu_shim.py outside pytest and print each build's timings.
 
     python tools/shim_compare.py
 
-It runs both builds of every harness on the same deterministic inputs and fails unless every result array is byte-identical and the
-`_b200` build really went through the nvbio_b200 kernels (call counters, no fall-backs)."""
-import filecmp
-import json
+The checks themselves live in the test module (one copy); this only runs them one by one on a GPU, after oracle/ref_shim.mk has built
+oracle/_ref/shim, and prints the reference build's and the shim build's *_ms / *_gcups figures side by side."""
 import os
-import subprocess
 import sys
 import tempfile
 
-import numpy as np
+import pytest
 
-BIN = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "shim", "_bin")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-
-def _run(binary, args, out):
-    os.makedirs(out, exist_ok=True)
-    r = subprocess.run([binary] + args[:1] + [out] + args[1:], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, "%s failed: %s" % (os.path.basename(binary), (r.stderr or r.stdout)[-800:])
-    return json.loads(r.stdout.strip().splitlines()[-1])
-
-
-def _same_dumps(a, b):
-    fa, fb = sorted(os.listdir(a)), sorted(os.listdir(b))
-    assert fa == fb and fa, (fa, fb)
-    diff = [f for f in fa if not filecmp.cmp(os.path.join(a, f), os.path.join(b, f), shallow=False)]
-    assert not diff, "arrays differ between the reference build and the shim build: %s" % diff
-    return fa
-
-
-def _pair(name):
-    ref, b2 = os.path.join(BIN, name + "_ref"), os.path.join(BIN, name + "_b200")
-    assert os.path.exists(ref) and os.path.exists(b2), "%s_{ref,b200} not built: make -C tests/shim REF=<nvbio tree>" % name
-    return ref, b2
-
-
-def fmmap_program_identical_with_and_without_shim(tmp):
-    REF, B200 = _pair("shim_harness")
-    ref = _run(REF, ["fmmap", "3000000", "40000", "100"], os.path.join(tmp, "ref"))
-    b2 = _run(B200, ["fmmap", "3000000", "40000", "100"], os.path.join(tmp, "b200"))
-    files = _same_dumps(os.path.join(tmp, "ref"), os.path.join(tmp, "b200"))
-    assert {"fmmap_ranges.bin", "fmmap_slots.bin", "fmmap_hits.bin", "fmmap_scores_i16.bin", "fmmap_sinks_i32.bin", "fmmap_best_i32.bin"} <= set(files)
-    assert ref["hits"] == b2["hits"] and ref["hits"] > ref["reads"]
-    assert ref["shim"] == 0 and b2["shim"] == 1
-    c = b2["b200_calls"]
-    assert c["fm_rank"] == 3 and c["fm_locate"] == 6 and c["banded"] == 6 and c["fallbacks"] == 0, c
-    print("fmmap: reference ms", {k: ref[k] for k in ref if k.endswith("_ms")}, "shim ms", {k: b2[k] for k in b2 if k.endswith("_ms")})
-
-
-def batch_program_identical_with_and_without_shim(tmp):
-    REF, B200 = _pair("shim_harness")
-    ref = _run(REF, ["batch", "65536"], os.path.join(tmp, "ref"))
-    b2 = _run(B200, ["batch", "65536"], os.path.join(tmp, "b200"))
-    files = _same_dumps(os.path.join(tmp, "ref"), os.path.join(tmp, "b200"))
-    assert len(files) == 7 + 6
-    c = b2["b200_calls"]
-    assert c["banded"] == 21 and c["full"] == 9 and c["fallbacks"] == 0, c
-    print("batch GCUPS: reference", {k: ref[k] for k in ref if k.endswith("gcups")}, "shim", {k: b2[k] for k in b2 if k.endswith("gcups")})
-
-
-def nvbowtie_mapping_entry_points_identical(tmp):
-    """boundary B-A2: nvBowtie's non-template map_exact / map_approx / map / gather_ranges (nvBowtie/bowtie2/cuda/mapping.h) called on
-    nvBowtie's own PODs by ONE harness object, linked once against nvBowtie's mapping.cu and once against
-    tests/shim/nvbowtie_mapping_b200.cu + libnvbio_b200.so: deque sizes, the SeedHits of every read (canonical order), the range sizes
-    in pop_top() order, reseed flags and gather_ranges totals are identical; both leave valid priority deques behind"""
-    outs = {}
-    for name, binary in zip(("ref", "b200"), _pair("nvbowtie_harness")):
-        d = os.path.join(tmp, name); os.makedirs(d)
-        r = subprocess.run([binary, d, "400000", "4000"], capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, "%s failed: %s" % (name, (r.stderr or r.stdout)[-800:])
-        outs[name] = json.loads(r.stdout.strip().splitlines()[-1])
-    files = _same_dumps(os.path.join(tmp, "ref"), os.path.join(tmp, "b200"))
-    assert "exact_r0_hits.bin" in files and "approx_r0_hits.bin" in files and "exact_tiny_sizes.bin" in files
-    for cfg in ("exact_r0", "exact_r1", "exact_fw", "approx_r0", "approx_rc", "map_sub", "map_nosub", "exact_tiny"):
-        a, b = outs["ref"][cfg], outs["b200"][cfg]
-        assert a["hits"] == b["hits"] > 0 and a["range_total"] == b["range_total"] and a["full_deques"] == b["full_deques"], (cfg, a, b)
-        assert a["pop_order_ok"] == 1 and b["pop_order_ok"] == 1, cfg
-    assert outs["ref"]["exact_tiny"]["full_deques"] > 100
-    print("nvBowtie mapping ms: reference", {k: v["ms"] for k, v in outs["ref"].items() if isinstance(v, dict)},
-          "b200", {k: v["ms"] for k, v in outs["b200"].items() if isinstance(v, dict)})
-
-
-def nvbowtie_score_best_identical_with_and_without_shim(tmp):
-    """boundary B-B2: nvBowtie's best-score extension (detail::banded_score_best = the body of score_best_t / score_best,
-    score_best_inl.h:154-234) on nvBowtie's own types -- reversed DNA_N reads with base qualities, 2-bit genome, HitQueues,
-    SmithWatermanScoringScheme<> (--local preset and end-to-end default, quality-dependent mismatch penalties), ParamsPOD -- compiled
-    as is and with include/nvbio_b200/shim/nvbowtie_scoring.h: hit.score (incl. the worst_score clamp) and hit.sink of every hit equal"""
-    outs = {}
-    for name, binary in zip(("ref", "b200"), _pair("nvbowtie_score_harness")):
-        d = os.path.join(tmp, name); os.makedirs(d)
-        r = subprocess.run([binary, d, "2000000", "20000", "200000"], capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, "%s failed: %s" % (name, (r.stderr or r.stdout)[-800:])
-        outs[name] = json.loads(r.stdout.strip().splitlines()[-1])
-    files = _same_dumps(os.path.join(tmp, "ref"), os.path.join(tmp, "b200"))
-    assert len(files) == 8
-    sc = np.fromfile(os.path.join(tmp, "ref", "local_b31_score.bin"), np.int32)
-    assert (sc > 60).mean() > 0.5 and (sc != 12345).all()
-    assert outs["b200"]["b200_calls"] == {"banded": 12, "fallbacks": 0}
-    print("nvBowtie score_best ms: reference", {k: v for k, v in outs["ref"].items() if k.endswith("_ms")},
-          "b200", {k: v for k, v in outs["b200"].items() if k.endswith("_ms")})
-
-
-CHECKS = (fmmap_program_identical_with_and_without_shim, batch_program_identical_with_and_without_shim,
-          nvbowtie_mapping_entry_points_identical, nvbowtie_score_best_identical_with_and_without_shim)
+from tests import test_gpu_shim as T  # noqa: E402
 
 
 def main():
     failed = 0
-    for check in CHECKS:
+    for check in T.CHECKS:
         with tempfile.TemporaryDirectory() as tmp:
             try:
-                check(tmp)
-                print("ok  ", check.__name__)
+                ref, b2 = check(tmp)
             except AssertionError as e:
                 failed += 1
                 print("FAIL", check.__name__, e)
+                continue
+            except pytest.skip.Exception as e:         # a binary is not built
+                failed += 1
+                print("SKIP", check.__name__, e)
+                continue
+            timing = lambda r: {k: v for k, v in r.items() if k.endswith("_ms") or k.endswith("gcups")}
+            print("ok  ", check.__name__, "reference", timing(ref), "shim", timing(b2))
     sys.exit(1 if failed else 0)
 
 
