@@ -496,6 +496,50 @@ int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     const nvb_mapq_params* mapq, const nvb_mapq_out* mapq_out,
                     void* d_temp, size_t* temp_bytes, void* stream);
 
+/* Reseeding rounds (single end; nvBowtie's -R / --rep-seeds, params.cpp:126-127, aligner_best_approx.h:206-283; DESIGN.md 3.18).
+ * Call with the arguments of nvb_seed_extend_mapq (best_alignment, mapq and mapq_out each optional; mapq and mapq_out together) plus:
+ *   Round 0 is every read with exactly nvb_seed_extend's seeds; round r >= 1 covers only the reads flagged after round r - 1, in read
+ *   order.  Each string (forward, and the reverse complement with both_strands) is seeded at o_r + k*I for every k with o_r + k*I + L <= its
+ *   length, o_r = r * floor(I / (max_reseed + 1)), I = seed_interval, L = seed_len.  A read's base qualities go with it into every round.
+ *   Flag rule after round r < max_reseed, over the round's seeds of both strings: range_count = the seeds with a non-empty SA range (a seed
+ *   with an N has an empty one), range_sum = the sum of their full range sizes y - x + 1 (not capped by max_seed_hits), both in wrapping
+ *   uint32 arithmetic as nvb_map_seeds'.  A read is flagged when range_count == 0, range_sum >= rep_seeds * range_count, or its best
+ *   alignment over rounds 0 .. r is below d_min_score[len] or absent.
+ *   A read's candidates are the union of its rounds' jobs.  The best alignment: higher score, then earlier round, then nvb_seed_extend's tie
+ *   index within the round (a later round replaces the best only with a strictly higher score).  Second best, MAPQ, distinctness and the
+ *   traceback follow nvb_seed_extend_mapq's rules over that union with the tie index ordered by (round, tie); the results do not depend on
+ *   the path, the de-duplication, the exact shortcut or the seed split.  A job found in several rounds may be scored in each.
+ *   Per-hit outputs: round-major, within a round nvb_seed_extend's order for the round's reads; d_hit_read is the original string id
+ *   (read * strands + strand).  hit_capacity is shared by all rounds (round r keeps at most hit_capacity minus the hits kept before it).
+ *   d_n_hits = (hits kept, hits found, distinct jobs), each summed over the rounds.
+ *   Host round trip: after every round but the last the number of flagged reads is read back (one stream synchronisation per round, so the
+ *   call returns after rounds 0 .. max_reseed - 1 have run), to size the next round's grids and to stop when no read is flagged.
+ *   The temp size covers every read flagged in every round.
+ * NVB_E_INVALID before any CUDA call: reseed == NULL, d_min_score == NULL, max_read_len < reads->length, max_reseed > 254, or max_reseed > 0
+ * with seed_interval < max_reseed + 1 -- a deliberate deviation from nvBowtie, whose shifted seeds would all repeat round 0's there; the
+ * other checks are nvb_seed_extend_mapq's.  With max_reseed == 0 every output is that of nvb_seed_extend[_traceback|_mapq]. */
+typedef struct nvb_reseed_params {
+    uint32_t       max_reseed;    /* nvBowtie -R: rounds after the first; 0 = exactly nvb_seed_extend[_traceback|_mapq]   */
+    uint32_t       rep_seeds;     /* nvBowtie --rep-seeds (300)                                                          */
+    const int32_t* d_min_score;   /* device [max_read_len + 1]: a read is aligned when its best score >= d_min_score[len] */
+    uint32_t       max_read_len;
+} nvb_reseed_params;
+typedef struct nvb_reseed_out {
+    uint8_t*  d_rounds;           /* [n_reads] or NULL: the number of rounds read r was seeded in, 1 .. max_reseed + 1    */
+    uint32_t* d_active;           /* [max_reseed + 1] or NULL: the number of reads seeded in each round                   */
+} nvb_reseed_out;
+
+int nvb_seed_extend_reseed(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_reads,
+                    const nvb_seed_extend_params* params, uint32_t hit_capacity,
+                    int32_t* d_best_score, uint32_t* d_best_pos,
+                    uint32_t* d_n_hits, uint32_t* d_hit_read, nvb_uint2* d_hit_window,
+                    int32_t* d_hit_score, nvb_uint2* d_hit_sink,
+                    const nvb_best_alignment_out* best_alignment,
+                    const nvb_mapq_params* mapq, const nvb_mapq_out* mapq_out,
+                    const nvb_reseed_params* reseed, const nvb_reseed_out* reseed_out,
+                    void* d_temp, size_t* temp_bytes, void* stream);
+
 /* Up to k distinct alignments of every read, each traced (single end; nvBowtie's all-mapping mode, --all / -a, params.cpp:140-142,
  * aligner_all.h:49-235 and 278-690, with the per-read limit of Bowtie2's -k).  Call with the arguments of nvb_seed_extend_mapq, with
  * best_alignment == NULL; the best, second-best and MAPQ outputs are exactly those of nvb_seed_extend_mapq for the same inputs.

@@ -16,6 +16,7 @@
 #include <cub/agent/single_pass_scan_operators.cuh>
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 #include <cub/device/device_segmented_sort.cuh>
 #include <mutex>
 
@@ -32,6 +33,7 @@ struct PipeGeom {
     uint32_t band;
     uint32_t max_seed_hits;
     uint32_t genome_len;
+    uint32_t seed_offset;    // read offset of every string's first seed (nvb_seed_extend_reseed's round offset; 0 elsewhere)
 };
 
 // string s = 2*read + strand (strands==2) or read: copy / reverse-complement into an aligned slot.
@@ -170,7 +172,7 @@ pipe_seed_match_kernel(const FmIndex f, const PipeGeom g, const uint32_t* __rest
         if (live) {
             const uint32_t s = q / g.seeds_per_string, k = q % g.seeds_per_string;
             const uint32_t len = slen[s];
-            const uint32_t pos = k * g.seed_interval;
+            const uint32_t pos = g.seed_offset + k * g.seed_interval;
             if (pos + g.seed_len <= len) {
                 if (genome) {
                     const uint32_t st = fm_match_locate_one<BITS, true, DEFER ? FM_DEFER : FM_WHOLE>(f, genome, words, s * g.stride + pos, g.seed_len, x, y);
@@ -214,7 +216,7 @@ pipe_seed_match_wide_kernel(const FmIndex f, const PipeGeom g, const uint32_t* _
         const uint32_t s = q / g.seeds_per_string, k = q % g.seeds_per_string;
         const uint2 r = ranges[q];
         uint32_t x = r.x, y = r.y;
-        if (fm_match_locate_one<BITS, true, FM_RESUME>(f, genome, words, s * g.stride + k * g.seed_interval, g.seed_len, x, y) == FM_EMPTY) { x = 1; y = 0; }
+        if (fm_match_locate_one<BITS, true, FM_RESUME>(f, genome, words, s * g.stride + g.seed_offset + k * g.seed_interval, g.seed_len, x, y) == FM_EMPTY) { x = 1; y = 0; }
         ranges[q] = make_uint2(x, y);
         if (sizes) sizes[q] = seed_range_hits(make_uint2(x, y), g.max_seed_hits);
     }
@@ -253,7 +255,7 @@ pipe_expand_hits_kernel(const FmIndex f, const PipeGeom g, const uint2* __restri
     const uint32_t base = excl[q], kept = counts[0];
     const uint32_t x = ranges[q].x;
     const uint32_t s = q / g.seeds_per_string, k = q % g.seeds_per_string;
-    const uint32_t seed_begin = k * g.seed_interval;
+    const uint32_t seed_begin = g.seed_offset + k * g.seed_interval;
     const uint32_t len = slen[s];
     for (uint32_t j = 0; j < sz; ++j) {
         const uint32_t h = base + j;
@@ -405,7 +407,7 @@ pipe_resolve_reads_kernel(const FmIndex f, const PipeGeom g, const uint2* __rest
                     const uint32_t s = r * g.strands + strand, len = strand ? len1 : len0;
                     const bool located = rq.y == 0xFFFFFFFFu;                          // already a text position (fm_match_locate_one)
                     const uint32_t sz = seed_range_hits(rq, g.max_seed_hits);
-                    const uint32_t base = run, x = rq.x, seed_begin = k * g.seed_interval;
+                    const uint32_t base = run, x = rq.x, seed_begin = g.seed_offset + k * g.seed_interval;
                     run += sz;
                     for (uint32_t j = 0; j < sz; ++j) {
                         const uint32_t h = base + j;
@@ -686,6 +688,118 @@ pipe_export_hits_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, c
     if (h >= counts[0]) return;
     if (out_read)   out_read[h] = hit_string[h];              // string id = read*strands + strand
     if (out_window) out_window[h] = make_uint2(t_off[h], t_off[h] + t_len[h]);
+}
+
+// ---------------------------------------------------------------------------------------------
+// reseeding rounds (nvb_seed_extend_reseed).  Round r runs the stages above on the reads flagged after round r - 1 (round 0: every
+// read), compacted in read order, with the seeds shifted by reseed_offset(r).  map[i] = the original read of round read i (NULL in
+// round 0).  Each round's scored alignments are folded into one candidate list over the original reads, on which the best, second-best,
+// MAPQ and traceback stages then run once.
+// ---------------------------------------------------------------------------------------------
+
+// round r's scored alignments appended to the union at base + j: the original string, its pattern in round 0's [fw, rc] strings (the
+// same symbols), and tie index t0 + tie with t0 = the hits kept by the earlier rounds, so that every tie of round r exceeds every tie of
+// an earlier round and the key orders by (score, round, tie).  The cross-round best key of the original read rides along
+__global__ void __launch_bounds__(256)
+reseed_fold_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict__ map, const uint32_t base, const uint32_t t0,
+                   uint32_t* __restrict__ u_string, uint32_t* __restrict__ u_tie, const Jobs u, int32_t* __restrict__ u_score,
+                   uint2* __restrict__ u_sink, unsigned long long* __restrict__ key)
+{
+    const uint32_t n = *c.count;
+    for (uint32_t j = blockIdx.x * 256 + threadIdx.x; j < n; j += gridDim.x * 256) {
+        const uint32_t s = c.string[j], read = map ? map[s / g.strands] : s / g.strands, os = read * g.strands + s % g.strands;
+        const uint32_t o = base + j, tie = t0 + c.tie(j);
+        const int32_t sc = c.score[j];
+        const uint2 sk = c.sink[j];
+        u_string[o] = os; u_tie[o] = tie;
+        u.p_off[o] = os * g.stride; u.p_len[o] = c.jobs.p_len[j]; u.t_off[o] = c.jobs.t_off[j]; u.t_len[o] = c.jobs.t_len[j];
+        u_score[o] = sc; u_sink[o] = sk;
+        if (job_aligned(sk)) atomicMax(key + read, make_best_key(sc, tie));
+    }
+}
+
+// one thread per round read: range_count / range_sum over the final SA ranges of its seeds on both strings (a located single row counts
+// 1; an N seed has an empty range), then reseed_read with the best alignment of rounds 0 .. r
+__global__ void __launch_bounds__(256)
+reseed_flag_kernel(const PipeGeom g, const uint2* __restrict__ ranges, const uint32_t* __restrict__ map, const uint32_t* __restrict__ str_len,
+                   const unsigned long long* __restrict__ key, const int32_t* __restrict__ min_score, const uint32_t rep_seeds,
+                   uint8_t* __restrict__ flag)
+{
+    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= g.n_reads) return;
+    const uint32_t per_read = g.strands * g.seeds_per_string;
+    const uint2* rr = ranges + (size_t)i * per_read;
+    uint32_t range_sum = 0u, range_count = 0u;
+    for (uint32_t q = 0; q < per_read; ++q) {
+        const uint2 v = rr[q];
+        if (v.y != 0xFFFFFFFFu && v.x > v.y) continue;
+        range_sum += v.y == 0xFFFFFFFFu ? 1u : v.y - v.x + 1u;
+        ++range_count;
+    }
+    const unsigned long long k = key[map ? map[i] : i];
+    const bool aligned = k != 0ull && best_key_score(k) >= min_score[str_len[i * g.strands]];
+    flag[i] = reseed_read(range_sum, range_count, rep_seeds, aligned) ? 1u : 0u;
+}
+
+// the next round's [fw, rc] strings, lengths and base qualities gathered from round 0's (g: the next round's geometry, one thread per
+// output word); rounds[map[i]] = round + 1
+__global__ void __launch_bounds__(256)
+reseed_gather_kernel(const PipeGeom g, const uint32_t* __restrict__ map, const uint32_t* __restrict__ words0, const uint32_t* __restrict__ len0,
+                     const uint8_t* __restrict__ quals0, uint32_t* __restrict__ words, uint32_t* __restrict__ len, uint8_t* __restrict__ quals,
+                     uint8_t* __restrict__ rounds, const uint32_t round)
+{
+    const uint32_t spw = 32u / g.bits, wps = g.stride / spw;
+    const uint64_t t = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (t >= (uint64_t)g.n_strings * wps) return;
+    const uint32_t s = (uint32_t)(t / wps), w = (uint32_t)(t % wps), read = map[s / g.strands], os = read * g.strands + s % g.strands;
+    words[t] = words0[(size_t)os * wps + w];
+    if (quals)
+        for (uint32_t b = 0; b < spw; ++b) quals[(size_t)s * g.stride + w * spw + b] = quals0[(size_t)os * g.stride + w * spw + b];
+    if (w == 0) {
+        len[s] = len0[os];
+        if (rounds && s % g.strands == 0u) rounds[read] = (uint8_t)(round + 1u);
+    }
+}
+
+// the round's kept hits as per-hit outputs (out_* already offset by the hits of earlier rounds), with the original string id
+__global__ void __launch_bounds__(256)
+reseed_export_hits_kernel(const PipeGeom g, const uint32_t* __restrict__ counts, const uint32_t* __restrict__ map,
+                          const uint32_t* __restrict__ hit_string, const uint32_t* __restrict__ t_off, const uint32_t* __restrict__ t_len,
+                          uint32_t* __restrict__ out_read, uint2* __restrict__ out_window)
+{
+    const uint32_t h = blockIdx.x * 256 + threadIdx.x;
+    if (h >= counts[0]) return;
+    const uint32_t s = hit_string[h];
+    if (out_read)   out_read[h] = (map ? map[s / g.strands] : s / g.strands) * g.strands + s % g.strands;
+    if (out_window) out_window[h] = make_uint2(t_off[h], t_off[h] + t_len[h]);
+}
+
+// totals over the rounds: [0] hits kept, [1] hits found, [2] distinct jobs, [3] union candidates; active[round] = the round's reads
+__global__ void reseed_counts_kernel(const uint32_t* __restrict__ counts, const bool dedup, const bool per_read, uint32_t* __restrict__ totals,
+                                     uint32_t* __restrict__ active, const uint32_t round, const uint32_t n_round)
+{
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    const uint32_t jobs = dedup ? (counts[0] ? counts[2] : 0u) : counts[0];      // (a round that kept no hit scored no job)
+    totals[0] += counts[0]; totals[1] += counts[1]; totals[2] += jobs; totals[3] += per_read ? jobs : counts[0];
+    if (active) active[round] = n_round;
+}
+
+// every read's best score from the cross-round key (INT_MIN / 0xFFFFFFFF / strand 0 without one); pipe_winner_kernel adds end and strand
+__global__ void __launch_bounds__(256)
+reseed_best_kernel(const uint32_t n_reads, const unsigned long long* __restrict__ key, int32_t* __restrict__ best_score,
+                   uint32_t* __restrict__ best_pos, uint8_t* __restrict__ best_strand)
+{
+    const uint32_t r = blockIdx.x * 256 + threadIdx.x;
+    if (r >= n_reads) return;
+    const unsigned long long k = key[r];
+    best_score[r] = k ? best_key_score(k) : INT_MIN;
+    best_pos[r] = 0xFFFFFFFFu; best_strand[r] = 0;
+}
+
+__global__ void __launch_bounds__(256) reseed_iota_kernel(const uint32_t n, uint32_t* __restrict__ map)
+{
+    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+    if (i < n) map[i] = i;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1151,6 +1265,7 @@ struct PipeCall : SeedExtendReq {
     char *cs_scan_tmp, *cs_sort_tmp; size_t cs_scan_bytes, cs_sort_bytes;
     uint32_t *pc_fw, *pc_n, *pc_end, *pc_tie, *se_pos; int32_t* pc_score;   // paired MAPQ (PMO): merged candidates per read
     uint32_t *al_slice_n, n_slices; Jobs al_jobs;                           // nvb_seed_extend_all: traceback slices, jobs
+    const Scored* uni;                                                      // nvb_seed_extend_reseed: every round's candidates (scored())
 
     int stage(int i) const { return (int)cudaEventRecord(SE->ev[i], s); }    // boundary i of nvb_seed_extend_stage_ms
 
@@ -1292,6 +1407,16 @@ struct PipeCall : SeedExtendReq {
         return launched();
     }
 
+    // 3. per-hit path: hit slots, the exclusive sum of the clamped range sizes (the per-read path takes them inside its stage 4)
+    int hit_slots() const
+    {
+        if (per_read) return NVB_OK;
+        size_t bytes = scan_bytes;
+        NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(scan_tmp, bytes, sizes, excl, (int)nq, s));
+        pipe_count_kernel<<<1, 32, 0, s>>>(excl, sizes, nq, hit_capacity, counts);
+        return launched();
+    }
+
     // 4'-6'. per-read path: hit slots, locate, window, distinct jobs, exact shortcut and the claimed best per read in one kernel (stage 4),
     // the DP over the jobs left to it and their scatter into the best per read (6), the DP winners' results (7)
     int extend_per_read() const
@@ -1371,7 +1496,7 @@ struct PipeCall : SeedExtendReq {
     int best_traceback() const
     {
         const uint32_t rgrid = (g.n_reads + 255) / 256;
-        if (per_read) {
+        if (per_read || uni) {
             pipe_empty_jobs_kernel<<<rgrid, 256, 0, s>>>(g.n_reads, best.p_off, best.p_len, best.t_off, best.t_len, BA->d_strand);
             NVB_LAUNCH_CHECK();
             const uint32_t jgrid = resident_grid(hit_capacity);
@@ -1407,6 +1532,7 @@ struct PipeCall : SeedExtendReq {
     // the alignments the extension scored: the per-read path's distinct jobs, the per-hit path's kept hits
     Scored scored() const
     {
+        if (uni) return *uni;
         return per_read ? Scored{counts + 2, j_string, j_first, jobs, job_score, job_sink} : Scored{counts, hit_string, nullptr, hits, h_score, h_sink};
     }
 
@@ -1549,7 +1675,110 @@ struct PipeCall : SeedExtendReq {
     }
 };
 
-static int seed_extend_impl(const SeedExtendReq& R, void* d_temp, size_t* temp_bytes, void* stream)
+// nvb_seed_extend_reseed: its buffers, carved after the PipeCall's, and its rounds
+struct ReseedCall {
+    const nvb_reseed_params* RP; const nvb_reseed_out* RO;
+    uint32_t *map[2], *totals; uint8_t* flag; unsigned long long* key;   // totals: [0..3] reseed_counts_kernel's, [4] the next round's reads
+    uint32_t *r_words, *r_len; uint8_t* r_quals;                           // rounds >= 1: the round's [fw, rc] strings
+    uint32_t *u_string, *u_tie; Jobs u; int32_t* u_score; uint2* u_sink;   // every round's candidates (reseed_fold_kernel)
+    char* sel_tmp; size_t sel_bytes;
+
+    int carve(const PipeCall& c, void* base, size_t& need)
+    {
+        const uint32_t n = c.g.n_reads, cap = c.hit_capacity;
+        TempCarver tc(base);
+        map[0] = tc.take<uint32_t>(n); map[1] = tc.take<uint32_t>(n); flag = tc.take<uint8_t>((size_t)n + 16);
+        totals = tc.take<uint32_t>(8); key = tc.take<unsigned long long>(n);
+        r_words = tc.take<uint32_t>((size_t)c.g.n_strings * (c.g.stride / (32u / c.g.bits)) + 4); r_len = tc.take<uint32_t>(c.g.n_strings);
+        r_quals = c.P->d_read_quals ? tc.take<uint8_t>((size_t)c.g.n_strings * c.g.stride + 16) : nullptr;
+        u_string = tc.take<uint32_t>(cap); u_tie = tc.take<uint32_t>(cap); u = take_jobs(tc, cap);
+        u_score = tc.take<int32_t>(cap); u_sink = tc.take<uint2>(cap);
+        sel_bytes = 0;
+        NVB_CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, sel_bytes, map[0], flag, map[1], totals + 4, (int)n, c.s));
+        sel_tmp = tc.take<char>(sel_bytes);
+        need = tc.total();
+        return NVB_OK;
+    }
+
+    // Round r: the stages of nvb_seed_extend on the round's reads, their scored alignments folded into the union, then (r < max_reseed)
+    // the flags and the next round's reads, whose count is read back: one stream synchronisation per round.  After the last round the
+    // best alignment, its traceback, the second best and the MAPQ of every read over the union.
+    int run(PipeCall& c)
+    {
+        const cudaStream_t s = c.s;
+        const PipeGeom g0 = c.g;
+        const uint32_t n = g0.n_reads, cap = c.hit_capacity, n_rounds = RP->max_reseed + 1u;
+        uint32_t* const words0 = c.str_words; uint32_t* const len0 = c.str_len; uint8_t* const quals0 = c.str_quals;
+        int32_t* const h_score0 = c.h_score; uint2* const h_sink0 = c.h_sink;
+        uint8_t* const rounds = RO ? RO->d_rounds : nullptr; uint32_t* const active = RO ? RO->d_active : nullptr;
+        const uint32_t rgrid = (n + 255) / 256;
+        NVB_CUDA_TRY(cudaMemsetAsync(totals, 0, 8 * sizeof(uint32_t), s));
+        NVB_CUDA_TRY(cudaMemsetAsync(key, 0, sizeof(unsigned long long) * n, s));
+        if (rounds) NVB_CUDA_TRY(cudaMemsetAsync(rounds, 1, n, s));
+        if (active) NVB_CUDA_TRY(cudaMemsetAsync(active, 0, sizeof(uint32_t) * n_rounds, s));
+        reseed_iota_kernel<<<rgrid, 256, 0, s>>>(n, map[0]);
+        NVB_LAUNCH_CHECK();
+        NVB_TRY(default_stage_events(&c.SE));
+        NVB_TRY(c.stage(0));
+        NVB_TRY(c.make_strings()); NVB_TRY(c.stage(1));
+        uint32_t n_r = n, host[5] = {0u, 0u, 0u, 0u, 0u};
+        int cur = 0;
+        for (uint32_t r = 0; r < n_rounds && n_r; ++r) {
+            const uint32_t kept = host[0], base = host[3];      // hits kept and candidates of the rounds before r
+            c.g.n_reads = n_r; c.g.n_strings = n_r * g0.strands; c.nq = c.g.n_strings * g0.seeds_per_string;
+            c.g.seed_offset = reseed_offset(r, g0.seed_interval, RP->max_reseed);
+            if (r) {
+                reseed_gather_kernel<<<(uint32_t)(((uint64_t)c.g.n_strings * (g0.stride / (32u / g0.bits)) + 255) / 256), 256, 0, s>>>(
+                    c.g, map[cur], words0, len0, quals0, r_words, r_len, quals0 ? r_quals : nullptr, rounds, r);
+                NVB_LAUNCH_CHECK();
+                c.str_words = r_words; c.str_len = r_len; c.str_quals = quals0 ? r_quals : nullptr;
+            }
+            c.hit_capacity = cap - kept;
+            c.h_score = c.hit_score ? c.hit_score + kept : h_score0;
+            c.h_sink = c.hit_sink ? (uint2*)c.hit_sink + kept : h_sink0;
+            NVB_TRY(c.match_seeds()); NVB_TRY(c.stage(2));
+            NVB_TRY(c.hit_slots());   NVB_TRY(c.stage(3));
+            NVB_TRY(c.per_read ? c.extend_per_read() : c.extend_per_hit());
+            if (c.hit_capacity) {
+                if (c.hit_read || c.hit_window) {
+                    reseed_export_hits_kernel<<<(c.hit_capacity + 255) / 256, 256, 0, s>>>(c.g, c.counts, map[cur], c.hit_string, c.hits.t_off,
+                        c.hits.t_len, c.hit_read ? c.hit_read + kept : nullptr, c.hit_window ? (uint2*)c.hit_window + kept : nullptr);
+                    NVB_LAUNCH_CHECK();
+                }
+                reseed_fold_kernel<<<resident_grid(c.hit_capacity), 256, 0, s>>>(c.g, c.scored(), map[cur], base, kept, u_string, u_tie, u,
+                                                                                  u_score, u_sink, key);
+                NVB_LAUNCH_CHECK();
+            }
+            reseed_counts_kernel<<<1, 32, 0, s>>>(c.counts, c.dedup, c.per_read, totals, active, r, n_r);
+            NVB_LAUNCH_CHECK();
+            if (r + 1u == n_rounds) break;
+            reseed_flag_kernel<<<(n_r + 255) / 256, 256, 0, s>>>(c.g, c.ranges, map[cur], c.str_len, key, RP->d_min_score, RP->rep_seeds, flag);
+            NVB_LAUNCH_CHECK();
+            size_t bytes = sel_bytes;
+            NVB_CUDA_TRY(cub::DeviceSelect::Flagged(sel_tmp, bytes, map[cur], flag, map[cur ^ 1], totals + 4, (int)n_r, s));
+            NVB_CUDA_TRY(cudaMemcpyAsync(host, totals, sizeof(host), cudaMemcpyDeviceToHost, s));
+            NVB_CUDA_TRY(cudaStreamSynchronize(s));
+            n_r = host[4]; cur ^= 1;
+        }
+        c.g = g0; c.str_words = words0; c.str_len = len0; c.str_quals = quals0; c.hit_capacity = cap;
+        const Scored U{totals + 3, u_string, u_tie, u, u_score, u_sink};
+        c.uni = &U; c.best_key = key;
+        reseed_best_kernel<<<rgrid, 256, 0, s>>>(n, key, c.best_score, c.best_pos, c.rb_strand);
+        NVB_LAUNCH_CHECK();
+        if (cap) {
+            pipe_winner_kernel<<<resident_grid(cap), 256, 0, s>>>(g0, U, key, Jobs{}, c.best_pos, c.rb_strand);
+            NVB_LAUNCH_CHECK();
+        }
+        if (c.BA) NVB_TRY(c.best_traceback());
+        if (c.MO) NVB_TRY(c.second_best());
+        if (c.n_hits) NVB_CUDA_TRY(cudaMemcpyAsync(c.n_hits, totals, 3 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+        NVB_TRY(c.stage(7));
+        c.SE->valid = true;
+        return NVB_OK;
+    }
+};
+
+static int seed_extend_impl(const SeedExtendReq& R, void* d_temp, size_t* temp_bytes, void* stream, ReseedCall* RS = nullptr)
 {
     // The entry points check only what cannot be seen here: that the structs they require are there, and the pair count before
     // 2 * n_pairs is formed.  The order below decides which code a call with several faults gets: the paired traceback's read length
@@ -1602,10 +1831,13 @@ static int seed_extend_impl(const SeedExtendReq& R, void* d_temp, size_t* temp_b
     c.eligible = c.per_read && P->type == NVB_LOCAL && g.bits == 2 && P->band_len <= 32 && !SC.d_qual_table && SC.match > 0 && SC.mismatch < 0 &&
                  SC.pattern_gap_open < 0 && SC.pattern_gap_ext <= 0 && SC.text_gap_open < 0 && SC.text_gap_ext <= 0;
     c.seed_split = c.per_read && c.f.sa_shift == 0u && c.f.ktab_k && g.seed_len > c.f.ktab_k && g_seed_split;
-    size_t need = 0;
+    size_t need = 0, rs_need = 0;
     NVB_TRY(c.carve(d_temp, need));
+    if (RS) NVB_TRY(RS->carve(c, d_temp ? (char*)d_temp + need : nullptr, rs_need));
+    need += rs_need;
     if (!d_temp || *temp_bytes < need) { *temp_bytes = need; return NVB_E_TEMP_SIZE; }
     if (R.n_reads == 0) {
+        if (RS && RS->RO && RS->RO->d_active) NVB_CUDA_TRY(cudaMemsetAsync(RS->RO->d_active, 0, sizeof(uint32_t) * (RS->RP->max_reseed + 1u), s));
         if (R.AO) {
             NVB_CUDA_TRY(cudaMemsetAsync(R.AO->d_first, 0, sizeof(uint32_t), s));
             NVB_CUDA_TRY(cudaMemsetAsync(R.AO->d_count, 0, 2 * sizeof(uint32_t), s));
@@ -1613,18 +1845,12 @@ static int seed_extend_impl(const SeedExtendReq& R, void* d_temp, size_t* temp_b
         return NVB_OK;
     }
 
+    if (RS) return RS->run(c);
     NVB_TRY(default_stage_events(&c.SE));
     NVB_TRY(c.stage(0));
     NVB_TRY(c.make_strings()); NVB_TRY(c.stage(1));
     NVB_TRY(c.match_seeds());  NVB_TRY(c.stage(2));
-    // 3. per-hit path: hit slots, the exclusive sum of the clamped range sizes (the per-read path takes them inside its stage 4)
-    if (!c.per_read) {
-        size_t scan_bytes = c.scan_bytes;
-        NVB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(c.scan_tmp, scan_bytes, c.sizes, c.excl, (int)c.nq, s));
-        pipe_count_kernel<<<1, 32, 0, s>>>(c.excl, c.sizes, c.nq, R.hit_capacity, c.counts);
-        NVB_LAUNCH_CHECK();
-    }
-    NVB_TRY(c.stage(3));
+    NVB_TRY(c.hit_slots());    NVB_TRY(c.stage(3));
     NVB_TRY(c.per_read ? c.extend_per_read() : c.extend_per_hit());       // records stages 4 to 6
     if (R.hit_capacity && (R.hit_read || R.hit_window)) {
         pipe_export_hits_kernel<<<(R.hit_capacity + 255) / 256, 256, 0, s>>>(g, c.counts, c.hit_string, c.hits.t_off, c.hits.t_len, R.hit_read,
@@ -1718,6 +1944,29 @@ extern "C" int nvb_seed_extend_mapq(const nvb_fm_index* fmi, const uint32_t* d_g
     R.best_score = d_best_score; R.best_pos = d_best_pos; R.n_hits = d_n_hits; R.hit_read = d_hit_read; R.hit_window = d_hit_window;
     R.hit_score = d_hit_score; R.hit_sink = d_hit_sink; R.BA = best_alignment; R.MP = mapq; R.MO = mapq_out;
     return seed_extend_impl(R, d_temp, temp_bytes, stream);
+}
+
+extern "C" int nvb_seed_extend_reseed(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_reads,
+                    const nvb_seed_extend_params* P, uint32_t hit_capacity,
+                    int32_t* d_best_score, uint32_t* d_best_pos,
+                    uint32_t* d_n_hits, uint32_t* d_hit_read, nvb_uint2* d_hit_window,
+                    int32_t* d_hit_score, nvb_uint2* d_hit_sink,
+                    const nvb_best_alignment_out* best_alignment,
+                    const nvb_mapq_params* mapq, const nvb_mapq_out* mapq_out,
+                    const nvb_reseed_params* reseed, const nvb_reseed_out* reseed_out,
+                    void* d_temp, size_t* temp_bytes, void* stream)
+{
+    if (!reseed || !reseed->d_min_score || !reads || reseed->max_read_len < reads->length) return NVB_E_INVALID;
+    if (reseed->max_reseed > 254u) return NVB_E_INVALID;                         // d_rounds counts up to max_reseed + 1 in a byte
+    if (P && reseed->max_reseed && P->seed_interval < reseed->max_reseed + 1u) return NVB_E_INVALID;   // every offset would be 0
+    SeedExtendReq R = {};
+    R.fmi = fmi; R.genome = d_genome; R.reads = reads; R.n_reads = n_reads; R.P = P; R.hit_capacity = hit_capacity;
+    R.best_score = d_best_score; R.best_pos = d_best_pos; R.n_hits = d_n_hits; R.hit_read = d_hit_read; R.hit_window = d_hit_window;
+    R.hit_score = d_hit_score; R.hit_sink = d_hit_sink; R.BA = best_alignment; R.MP = mapq; R.MO = mapq_out;
+    ReseedCall RS = {};
+    RS.RP = reseed; RS.RO = reseed_out;
+    return seed_extend_impl(R, d_temp, temp_bytes, stream, &RS);
 }
 
 extern "C" int nvb_seed_extend_all(const nvb_fm_index* fmi, const uint32_t* d_genome,

@@ -206,6 +206,21 @@ __host__ __device__ __forceinline__ bool job_aligned(uint2 sink) { return sink.x
 // MAPQ and of nvb_seed_extend_all)
 __host__ __device__ __forceinline__ bool reportable(int32_t score, uint2 sink, int32_t min_score) { return job_aligned(sink) && score >= min_score; }
 
+// nvb_seed_extend_reseed: the first seed of round r starts at r * floor(I / (max_reseed + 1)) (nvBowtie's retry stride,
+// mapping_inl.h:553-565)
+__host__ __device__ __forceinline__ uint32_t reseed_offset(uint32_t round, uint32_t seed_interval, uint32_t max_reseed)
+{
+    return round * (seed_interval / (max_reseed + 1u));
+}
+
+// nvb_seed_extend_reseed: a read goes on to the next round when its round's seeds found no SA range, their mean range size reached
+// rep_seeds (range_sum >= rep_seeds * range_count in wrapping uint32 arithmetic, as map_seeds_kernel and mapping_inl.h:586-588), or its
+// best alignment so far does not reach its min score (aligner_init.cu:422-437's mark_unaligned)
+__host__ __device__ __forceinline__ bool reseed_read(uint32_t range_sum, uint32_t range_count, uint32_t rep_seeds, bool aligned)
+{
+    return range_count == 0u || range_sum >= rep_seeds * range_count || !aligned;
+}
+
 // (end, strand) of a candidate packed for select_distinct
 __host__ __device__ __forceinline__ unsigned long long end_strand(uint32_t end, uint32_t strand) { return ((unsigned long long)end << 1) | (strand & 1u); }
 

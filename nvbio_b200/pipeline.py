@@ -6,7 +6,7 @@ from typing import Optional
 import torch
 import numpy as np
 from ._lib import (lib, check, SeedExtendParamsStruct, BestAlignmentOutStruct, PairParamsStruct, PairOutStruct, MapqParamsStruct, MapqOutStruct,
-                   PairMapqOutStruct, AllParamsStruct, AllOutStruct)
+                   PairMapqOutStruct, AllParamsStruct, AllOutStruct, ReseedParamsStruct, ReseedOutStruct)
 from .strings import PackedStringSet
 from .fmindex import FMIndexDevice
 from . import aln
@@ -136,11 +136,14 @@ class SeedExtendWorkspace:
             self.second_strand = torch.empty(n, dtype=torch.uint8, device=dev)
             self.mapq = torch.empty(n, dtype=torch.uint8, device=dev)
         tb = C.c_size_t(0)
-        r = _call(fmi, genome, reads, params, self, None, tb)
+        r = self._call(fmi, genome, reads, params, None, tb)
         if r != -2:
             check(r, "nvb_seed_extend(size query)")
         self.temp = torch.empty(tb.value, dtype=torch.uint8, device=dev)
         self.temp_bytes = tb.value
+
+    def _call(self, fmi, genome, reads, params, temp, tb):
+        return _call(fmi, genome, reads, params, self, temp, tb)
 
 
 def _p(t):
@@ -193,6 +196,100 @@ def seed_extend(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStringSet
         workspace.mapq_params = mapq
     tb = C.c_size_t(workspace.temp_bytes)
     check(_call(fmi, genome, reads, params, workspace, workspace.temp, tb), "nvb_seed_extend")
+    return workspace
+
+
+@dataclass
+class ReseedParams:
+    """Reseeding rounds of seed_extend_reseed (nvb_reseed_params): max_reseed rounds after the first (nvBowtie -R), rep_seeds (nvBowtie
+    --rep-seeds) and min_score, an int32 tensor [max_read_len + 1] on the device: a read counts as aligned when its best score reaches
+    min_score[len] (--score-min evaluated on the host, as MapqParams.min_score)."""
+    min_score: torch.Tensor
+    max_reseed: int = 2
+    rep_seeds: int = 300
+
+    @property
+    def max_read_len(self) -> int:
+        return self.min_score.numel() - 1
+
+    @classmethod
+    def from_score_min(cls, kind: str, const: float, coeff: float, max_read_len: int, max_reseed: int = 2, rep_seeds: int = 300,
+                       device="cuda") -> "ReseedParams":
+        """nvBowtie's --score-min kind,const,coeff for lengths 0 .. max_read_len (see MapqParams.from_score_min)"""
+        tab = simple_func(kind, const, coeff, np.arange(max_read_len + 1))
+        return cls(torch.from_numpy(tab).to(device), int(max_reseed), int(rep_seeds))
+
+    @classmethod
+    def local(cls, max_read_len: int, max_reseed: int = 2, rep_seeds: int = 300, device="cuda") -> "ReseedParams":
+        """nvBowtie's --local min score, G,0,10"""
+        return cls.from_score_min("G", 0.0, 10.0, max_read_len, max_reseed, rep_seeds, device)
+
+    @classmethod
+    def end_to_end(cls, max_read_len: int, max_reseed: int = 2, rep_seeds: int = 300, device="cuda") -> "ReseedParams":
+        """nvBowtie's end-to-end min score, L,-0.6,-0.6"""
+        return cls.from_score_min("L", -0.6, -0.6, max_read_len, max_reseed, rep_seeds, device)
+
+    def struct(self) -> ReseedParamsStruct:
+        assert self.min_score.dtype == torch.int32 and self.min_score.is_cuda and self.min_score.is_contiguous()
+        p = ReseedParamsStruct()
+        p.max_reseed, p.rep_seeds, p.d_min_score, p.max_read_len = self.max_reseed, self.rep_seeds, self.min_score.data_ptr(), self.max_read_len
+        return p
+
+
+class ReseedWorkspace(SeedExtendWorkspace):
+    """SeedExtendWorkspace of seed_extend_reseed: the same fields, plus .rounds[n] (the rounds each read was seeded in) and
+    .active[max_reseed + 1] (the reads seeded in each round)"""
+
+    def __init__(self, fmi, genome, reads, params, hit_capacity, reseed: ReseedParams, keep_hits=False, traceback=False, mapq=None):
+        self.reseed = reseed
+        self.rounds = torch.empty(max(reads.count, 1), dtype=torch.uint8, device=fmi.device)[:reads.count]
+        self.active = torch.zeros(reseed.max_reseed + 1, dtype=torch.int32, device=fmi.device)
+        super().__init__(fmi, genome, reads, params, hit_capacity, keep_hits, traceback, mapq)
+
+    def _call(self, fmi, genome, reads, params, temp, tb):
+        s, rd, ps, rp = fmi.struct(), reads.struct(), params.struct(), self.reseed.struct()
+        ro = ReseedOutStruct()
+        ro.d_rounds, ro.d_active = _storage_ptr(self.rounds), self.active.data_ptr()
+        ba = mp = mo = None
+        if self.best_ops is not None:
+            ba = BestAlignmentOutStruct()
+            ba.d_ops, ba.max_ops, ba.d_n_ops = self.best_ops.data_ptr(), self.max_ops, self.best_n_ops.data_ptr()
+            ba.d_begin, ba.d_strand = self.best_begin.data_ptr(), self.best_strand.data_ptr()
+        if self.mapq is not None:
+            mp = self.mapq_params.struct()
+            mo = MapqOutStruct()
+            mo.d_second_score, mo.d_second_pos = self.second_score.data_ptr(), self.second_pos.data_ptr()
+            mo.d_second_strand, mo.d_mapq = self.second_strand.data_ptr(), self.mapq.data_ptr()
+        ref = lambda x: C.byref(x) if x is not None else None      # noqa: E731
+        return lib().nvb_seed_extend_reseed(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(reads.count), C.byref(ps),
+                                            C.c_uint32(self.hit_capacity), _p(self.best_score), _p(self.best_pos), _p(self.n_hits),
+                                            _p(self.hit_read), _p(self.hit_window), _p(self.hit_score), _p(self.hit_sink),
+                                            ref(ba), ref(mp), ref(mo), C.byref(rp), C.byref(ro),
+                                            _p(temp), C.byref(tb), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+
+
+def seed_extend_reseed(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStringSet, params: SeedExtendParams, reseed: ReseedParams,
+                       traceback: bool = False, mapq: Optional[MapqParams] = None, keep_hits: bool = False,
+                       workspace: Optional[ReseedWorkspace] = None, hit_capacity: Optional[int] = None) -> ReseedWorkspace:
+    """seed_extend with nvBowtie's reseeding rounds (nvb_seed_extend_reseed): reads whose seeds found nothing, only repeats, or no
+    alignment reaching reseed.min_score are seeded again at shifted offsets, up to reseed.max_reseed more times, and every round's
+    alignments compete for each read's best, second best and MAPQ.  Returns a ReseedWorkspace: seed_extend's fields plus .rounds and
+    .active.  The call synchronises the stream once per round after the first.  A workspace of an equally-shaped earlier call is reused
+    (reseed and mapq replace its parameters)"""
+    if workspace is None:
+        if hit_capacity is None:
+            hit_capacity = 32 * reads.count + 1024
+        workspace = ReseedWorkspace(fmi, genome, reads, params, hit_capacity, reseed, keep_hits, traceback, mapq)
+    else:
+        if reseed.max_reseed + 1 > workspace.active.numel():
+            raise ValueError("seed_extend_reseed: the workspace was created for at most %d rounds" % workspace.active.numel())
+        workspace.reseed = reseed
+        if mapq is not None:
+            if workspace.mapq is None:
+                raise ValueError("seed_extend_reseed(mapq=...): the workspace was created without mapq outputs")
+            workspace.mapq_params = mapq
+    tb = C.c_size_t(workspace.temp_bytes)
+    check(workspace._call(fmi, genome, reads, params, workspace.temp, tb), "nvb_seed_extend_reseed")
     return workspace
 
 
