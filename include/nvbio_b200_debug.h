@@ -42,6 +42,9 @@ void nvb_debug_pipeline_path(int path);
 /* seed-match stage of the per-read path with a k-mer table: 1 (default) = seeds on k-mers with three or more occurrences are finished
    by a second kernel, 0 = one pass.  Same results; for A/B timing and tests */
 void nvb_debug_seed_split(int on);
+/* *n = the number of seeds the first seed-match pass of the last two-pass call handed to the second (its todo lists).  Reads the
+   caller's temp buffer of that call, so only while it is still allocated; synchronises the device */
+int nvb_debug_seed_todo(uint32_t* n);
 
 /* extension stage of the per-read path (LOCAL, constant scheme, 2-bit reads): 1 (default) = a job whose result the exact shortcut
    proves (the best segment of the seed's band diagonal beats every gapped alignment and every other diagonal) gets it without running

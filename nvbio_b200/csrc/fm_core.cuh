@@ -454,7 +454,9 @@ constexpr uint32_t FM_ROWS_MAX = 8;
 // position x).  Backward order only (flags == 0); symbols > 3 never match.
 // MODE (the seed-match stage splits its seeds by how many dependent gathers they need, so that a warp does not wait on its slowest
 // lane): FM_WHOLE = everything in one call;  FM_DEFER = stop after the table look-up when the k-mer occurs three or more times (or
-// twice, with both occurrences spelling the whole query; with a wide table, only when the entry's contexts do not decide the seed) and
+// twice, with both occurrences spelling the whole query; with a wide table, only when the entry's contexts do not decide the seed: more
+// than 8 rows, a repeat of the whole query, a survivor isolated only by the last step, more unread symbols than the entry's contexts
+// hold, an N) and
 // return FM_DEFERRED with the range reached so far in (ox, oy);
 // FM_RESUME = continue such a query: (ox, oy) hold that range on entry, the first ktab_k steps are taken as done ((0, n) = none).
 enum { FM_EMPTY = 0, FM_RANGE = 1, FM_LOCATED = 2, FM_DEFERRED = 3 };
@@ -542,9 +544,11 @@ __host__ __device__ __forceinline__ uint32_t fm_match_locate_one(const FmIndex& 
     if (MODE != FM_RESUME && f.ktab_wide && full_sa && s == f.ktab_k && s < len && y - x >= 2u && y - x < KTAB_WIDE_ROWS) {
         // a k-mer with 3..8 occurrences on a wide table: the rule of the per-row array below, decided on the contexts that came with the
         // look-up.  They are 16 symbols long for 3 rows and 8 for 4..8, so the unread symbols are compared over min(rem, width) of them:
-        // no survivor = empty (exact: a longer remainder or a short context near the text start can only add survivors); with 3 or 4 rows
-        // (whose SA values are in the entry too) and rem <= width, one survivor that is also the only row matching the rem - 1 closest
-        // symbols = located.  Anything else is deferred or walked as without the wide half.
+        // no survivor = empty (exact: a longer remainder or a short context near the text start can only add survivors); with rem <= width,
+        // one survivor that is also the only row matching the rem - 1 closest symbols = located, at its SA value from the entry (3 or 4
+        // rows) or from the full suffix array (5 to 8 rows: one more gather).  As with the per-row array, the contexts are compared
+        // without the position test, which can only add survivors, and the single survivor's SA is tested after.  Anything else is
+        // deferred or walked as without the wide half.
         const uint32_t rem = len - s, cnt = rem < 16u ? rem : 16u;
         const bool three = (y - x == 2u);
         const uint32_t width = three ? 16u : 8u, wc = cnt < width ? cnt : width;
@@ -560,8 +564,8 @@ __host__ __device__ __forceinline__ uint32_t fm_match_locate_one(const FmIndex& 
                 near += context_equal(qw, c, wc - 1u) ? 1u : 0u;
             }
             if (full == 0u) return FM_EMPTY;
-            if (full == 1u && near == 1u && y - x <= 3u && rem <= width) {
-                const uint32_t pos = ktab_wide_sa(e, e_hi, three, hit);
+            if (full == 1u && near == 1u && rem <= width) {
+                const uint32_t pos = y - x <= 3u ? ktab_wide_sa(e, e_hi, three, hit) : gather_u32(f.ssa + x + hit);
                 if (pos == 0xFFFFFFFFu || pos < rem) return FM_EMPTY;
                 ox = pos - rem; oy = 0xFFFFFFFFu;
                 return FM_LOCATED;

@@ -1215,6 +1215,7 @@ extern "C" int nvb_seed_extend_stage_ms(float ms[7])
 static int g_perfect_shortcut = 1;     // 0 = every alignment job through the DP kernels, 2 = without the one-gap check (nvb_debug_perfect_shortcut)
 static const uint32_t* g_last_dp_count = nullptr;   // the last per-read call's count of jobs left to the DP (nvb_debug_dp_jobs)
 static int g_seed_split = 1;           // 0 = the located seed match in one pass (nvb_debug_seed_split)
+static const uint32_t* g_last_seed_todo = nullptr;  // the todo-list counters of the last two-pass seed match (nvb_debug_seed_todo)
 static int g_pipe_path = 0;            // 1 = always the per-hit path, anything else = automatic (nvb_debug_pipeline_path)
 
 #define NVB_TRY(expr) do { const int _r = (expr); if (_r != NVB_OK) return _r; } while (0)
@@ -1400,6 +1401,7 @@ struct PipeCall : SeedExtendReq {
             const uint32_t wgrid = (sm_count() * 16u + SEED_TODO_LISTS - 1u) / SEED_TODO_LISTS * SEED_TODO_LISTS;   // 16 resident CTAs per SM (H100: 2112), whole lists
             if (g.bits == 2) pipe_seed_match_wide_kernel<2><<<wgrid, SEED_BLOCK, 0, s>>>(f, g, str_words, loc_genome, ranges, sizes, seed_todo, seed_todo_n, grid1);
             else             pipe_seed_match_wide_kernel<4><<<wgrid, SEED_BLOCK, 0, s>>>(f, g, str_words, loc_genome, ranges, sizes, seed_todo, seed_todo_n, grid1);
+            g_last_seed_todo = seed_todo_n;
         } else {
             if (g.bits == 2) pipe_seed_match_kernel<2, false><<<grid, SEED_BLOCK, 0, s>>>(f, g, str_words, str_len, loc_genome, ranges, sizes, nullptr, nullptr);
             else             pipe_seed_match_kernel<4, false><<<grid, SEED_BLOCK, 0, s>>>(f, g, str_words, str_len, loc_genome, ranges, sizes, nullptr, nullptr);
@@ -1879,6 +1881,16 @@ extern "C" int nvb_debug_dp_jobs(uint32_t* n)
     if (!n || !g_last_dp_count) return NVB_E_INVALID;
     NVB_CUDA_TRY(cudaDeviceSynchronize());
     NVB_CUDA_TRY(cudaMemcpy(n, g_last_dp_count, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    return NVB_OK;
+}
+extern "C" int nvb_debug_seed_todo(uint32_t* n)
+{
+    if (!n || !g_last_seed_todo) return NVB_E_INVALID;
+    uint32_t c[SEED_TODO_LISTS * SEED_TODO_PITCH];
+    NVB_CUDA_TRY(cudaDeviceSynchronize());
+    NVB_CUDA_TRY(cudaMemcpy(c, g_last_seed_todo, sizeof(c), cudaMemcpyDeviceToHost));
+    *n = 0u;
+    for (uint32_t l = 0; l < SEED_TODO_LISTS; ++l) *n += c[l * SEED_TODO_PITCH];
     return NVB_OK;
 }
 
