@@ -698,6 +698,44 @@ int nvb_seed_extend_paired_traceback(const nvb_fm_index* fmi, const uint32_t* d_
                     const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
                     uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream);
 
+/* Reseeding rounds before pairing (paired end; nvBowtie's -R / --rep-seeds, params.cpp:126-127, in its paired loop,
+ * aligner_best_approx_paired.h:144-265; DESIGN.md 3.18).  Call with the arguments of nvb_seed_extend_paired_traceback, where
+ * mate_alignment is optional here (NULL: no traceback) and mapq / mapq_out are optional together, plus reseed / reseed_out of
+ * nvb_seed_extend_reseed:
+ *   Rounds: the 2*n_pairs mates (mate m of pair p at index m*n_pairs + p) go through nvb_seed_extend_reseed's rounds as independent
+ *   reads: round 0 seeds every mate; round r >= 1 seeds the mates flagged after round r - 1, in mate order, at reseed_offset(r, I,
+ *   max_reseed) + k*I; base qualities go with each mate into every round; hit_capacity is shared by all rounds and d_n_hits gives the
+ *   totals over all rounds, as there.
+ *   Flag rule, seed statistics only: a mate goes on when range_count == 0 or range_sum >= rep_seeds * range_count over its round's seeds
+ *   on both strings, in wrapping uint32 arithmetic (nvb_seed_extend_reseed's statistics).  Unlike the single-end call there is no
+ *   "best alignment below its min score" term: nvBowtie's paired loop takes its reseed flags from map() alone (mapping_inl.h:586-588)
+ *   and never marks unaligned mates (compare aligner_best_approx.h:267-271 with aligner_best_approx_paired.h:240-264); a mate whose
+ *   partner aligns gets its second chance from the opposite-mate rescue.  reseed->d_min_score and max_read_len are not read (NULL / 0
+ *   are accepted).
+ *   Union, then pairing: every mate's best alignment is taken over the union of its rounds with the single-end rule (higher score, then
+ *   earlier round, then tie index).  Pairing, concordance, the opposite-mate rescue, the paired MAPQ and the mate tracebacks then run
+ *   once on that union, exactly as nvb_seed_extend_paired[_mapq|_traceback] run them on a single round: candidate tie indices order by
+ *   (round, tie), so the second-best pair's tie-break is round-major; rescue_capacity and d_n_rescue keep their meaning (one rescue
+ *   pass, in pair order).
+ *   Deliberate deviation: nvBowtie scores the opposite mate for every anchor in every round; here the pairing decides once, after the
+ *   last round -- the deviation nvb_seed_extend_paired already makes within a single round.
+ * Outputs: reseed_out->d_rounds is per mate, [2*n_pairs] in the mate layout above; d_active[r] counts the mates seeded in round r; every
+ * other output means what it means in the three paired calls.  With max_reseed == 0 every output is that of nvb_seed_extend_paired,
+ * _paired_mapq or _paired_traceback (whichever the optional groups select).  n_pairs == 0: NVB_OK with d_active zeroed.
+ * Host round trip: one stream synchronisation per round after the first, as in nvb_seed_extend_reseed.
+ * Validation before any CUDA call: NVB_E_INVALID as the paired calls (pair_params or out NULL, n_pairs > 0x3FFFFFFF, both_strands == 0,
+ * max_frag == 0, min_frag > max_frag, a NULL required output field, only one of mapq / mapq_out set) and as nvb_seed_extend_reseed
+ * (reseed == NULL, max_reseed > 254, max_reseed > 0 with seed_interval < max_reseed + 1); NVB_E_UNSUPPORTED when reads->length > 512
+ * with mate_alignment. */
+int nvb_seed_extend_paired_reseed(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_pairs,
+                    const nvb_seed_extend_params* params, uint32_t hit_capacity,
+                    const nvb_pair_params* pair_params, const nvb_pair_out* out,
+                    const nvb_best_alignment_out* mate_alignment,
+                    const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
+                    const nvb_reseed_params* reseed, const nvb_reseed_out* reseed_out,
+                    uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream);
+
 /* -------------------------------------------------------------------------------------------
  * Finishing traced alignments for SAM / BAM output (nvBowtie's finish_alignment_kernel, nvBowtie/bowtie2/cuda/traceback_inl.h:520-723,
  * and what its writers derive from the result, nvbio/io/output/output_sam.cpp:198-315, output_bam.cpp:66-91,

@@ -10,7 +10,7 @@ EXPORTS = [
     "nvb_version", "nvb_error_string",
     "nvb_fm_rank", "nvb_fm_rank4", "nvb_fm_match", "nvb_fm_match_approx", "nvb_fm_locate", "nvb_fm_filter_rank", "nvb_fm_filter_locate",
     "nvb_banded_gotoh_score", "nvb_banded_gotoh_score_indirect", "nvb_banded_gotoh_traceback", "nvb_gotoh_score", "nvb_gotoh_score_indirect", "nvb_banded_gotoh_score_window", "nvb_banded_gotoh_score_best2", "nvb_gotoh_traceback", "nvb_seed_extend_paired",
-    "nvb_fm_build_occ", "nvb_fm_build_bwt", "nvb_fm_build_ktab", "nvb_fm_build_ktab_located", "nvb_fm_build_ktab_context", "nvb_fm_build_ktab_wide", "nvb_fm_build_rows", "nvb_seed_extend", "nvb_seed_extend_traceback", "nvb_seed_extend_mapq", "nvb_seed_extend_reseed", "nvb_seed_extend_all", "nvb_seed_extend_paired_mapq", "nvb_seed_extend_paired_traceback",
+    "nvb_fm_build_occ", "nvb_fm_build_bwt", "nvb_fm_build_ktab", "nvb_fm_build_ktab_located", "nvb_fm_build_ktab_context", "nvb_fm_build_ktab_wide", "nvb_fm_build_rows", "nvb_seed_extend", "nvb_seed_extend_traceback", "nvb_seed_extend_mapq", "nvb_seed_extend_reseed", "nvb_seed_extend_all", "nvb_seed_extend_paired_mapq", "nvb_seed_extend_paired_traceback", "nvb_seed_extend_paired_reseed",
     "nvb_seed_extend_stage_ms",
     "nvb_dict_rank", "nvb_dict_rank4", "nvb_dict_build_occ",
     "nvb_map_seeds", "nvb_fm_locate_init", "nvb_fm_locate_lookup", "nvb_fm_locate_sorted",

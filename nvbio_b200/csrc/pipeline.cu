@@ -719,7 +719,8 @@ reseed_fold_kernel(const PipeGeom g, const Scored c, const uint32_t* __restrict_
 }
 
 // one thread per round read: range_count / range_sum over the final SA ranges of its seeds on both strings (a located single row counts
-// 1; an N seed has an empty range), then reseed_read with the best alignment of rounds 0 .. r
+// 1; an N seed has an empty range), then reseed_read with the best alignment of rounds 0 .. r.  min_score == NULL: the seed statistics
+// alone (nvb_seed_extend_paired_reseed, whose flags nvBowtie's paired loop takes from map() only)
 __global__ void __launch_bounds__(256)
 reseed_flag_kernel(const PipeGeom g, const uint2* __restrict__ ranges, const uint32_t* __restrict__ map, const uint32_t* __restrict__ str_len,
                    const unsigned long long* __restrict__ key, const int32_t* __restrict__ min_score, const uint32_t rep_seeds,
@@ -736,8 +737,11 @@ reseed_flag_kernel(const PipeGeom g, const uint2* __restrict__ ranges, const uin
         range_sum += v.y == 0xFFFFFFFFu ? 1u : v.y - v.x + 1u;
         ++range_count;
     }
-    const unsigned long long k = key[map ? map[i] : i];
-    const bool aligned = k != 0ull && best_key_score(k) >= min_score[str_len[i * g.strands]];
+    bool aligned = true;
+    if (min_score) {
+        const unsigned long long k = key[map ? map[i] : i];
+        aligned = k != 0ull && best_key_score(k) >= min_score[str_len[i * g.strands]];
+    }
     flag[i] = reseed_read(range_sum, range_count, rep_seeds, aligned) ? 1u : 0u;
 }
 
@@ -1657,6 +1661,23 @@ struct PipeCall : SeedExtendReq {
         return NVB_OK;
     }
 
+    // every stage after the extension, in the one order every call takes, on scored() and every read's best (best_key, best_score,
+    // best_pos, rb_strand); hit_counts: the (kept, found, distinct jobs) d_n_hits reports
+    int after_extension(const uint32_t* hit_counts) const
+    {
+        if (BA && !PP) NVB_TRY(best_traceback());
+        if (MO) NVB_TRY(second_best());
+        if (AO) NVB_TRY(all_alignments());
+        if (PMO) NVB_TRY(pair_candidates());
+        if (PP) NVB_TRY(paired_rescue());
+        if (BA && PP) { NVB_TRY(best_traceback()); NVB_TRY(rescue_traceback()); }
+        if (PMO) NVB_TRY(pair_second());
+        if (n_hits) NVB_CUDA_TRY(cudaMemcpyAsync(n_hits, hit_counts, 3 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+        NVB_TRY(stage(7));
+        SE->valid = true;
+        return NVB_OK;
+    }
+
     // paired traceback of the rescued mates (after best_traceback, whose outputs they overwrite): the winning opposite-mate job of every
     // rescued pair, traced from the rescue score pass's sink on its window; begin = (window begin + source.x, source.y)
     int rescue_traceback() const
@@ -1677,7 +1698,7 @@ struct PipeCall : SeedExtendReq {
     }
 };
 
-// nvb_seed_extend_reseed: its buffers, carved after the PipeCall's, and its rounds
+// nvb_seed_extend_reseed / nvb_seed_extend_paired_reseed: their buffers, carved after the PipeCall's, and their rounds
 struct ReseedCall {
     const nvb_reseed_params* RP; const nvb_reseed_out* RO;
     uint32_t *map[2], *totals; uint8_t* flag; unsigned long long* key;   // totals: [0..3] reseed_counts_kernel's, [4] the next round's reads
@@ -1704,7 +1725,8 @@ struct ReseedCall {
 
     // Round r: the stages of nvb_seed_extend on the round's reads, their scored alignments folded into the union, then (r < max_reseed)
     // the flags and the next round's reads, whose count is read back: one stream synchronisation per round.  After the last round the
-    // best alignment, its traceback, the second best and the MAPQ of every read over the union.
+    // best alignment of every read over the union, then every later stage of the call (PipeCall::after_extension) on it: with PP the
+    // 2 * n_pairs mates went through the rounds as reads, and the pairing, rescue, paired MAPQ and mate tracebacks run once, here.
     int run(PipeCall& c)
     {
         const cudaStream_t s = c.s;
@@ -1754,7 +1776,8 @@ struct ReseedCall {
             reseed_counts_kernel<<<1, 32, 0, s>>>(c.counts, c.dedup, c.per_read, totals, active, r, n_r);
             NVB_LAUNCH_CHECK();
             if (r + 1u == n_rounds) break;
-            reseed_flag_kernel<<<(n_r + 255) / 256, 256, 0, s>>>(c.g, c.ranges, map[cur], c.str_len, key, RP->d_min_score, RP->rep_seeds, flag);
+            reseed_flag_kernel<<<(n_r + 255) / 256, 256, 0, s>>>(c.g, c.ranges, map[cur], c.str_len, key, c.PP ? nullptr : RP->d_min_score,
+                                                                 RP->rep_seeds, flag);
             NVB_LAUNCH_CHECK();
             size_t bytes = sel_bytes;
             NVB_CUDA_TRY(cub::DeviceSelect::Flagged(sel_tmp, bytes, map[cur], flag, map[cur ^ 1], totals + 4, (int)n_r, s));
@@ -1771,12 +1794,7 @@ struct ReseedCall {
             pipe_winner_kernel<<<resident_grid(cap), 256, 0, s>>>(g0, U, key, Jobs{}, c.best_pos, c.rb_strand);
             NVB_LAUNCH_CHECK();
         }
-        if (c.BA) NVB_TRY(c.best_traceback());
-        if (c.MO) NVB_TRY(c.second_best());
-        if (c.n_hits) NVB_CUDA_TRY(cudaMemcpyAsync(c.n_hits, totals, 3 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
-        NVB_TRY(c.stage(7));
-        c.SE->valid = true;
-        return NVB_OK;
+        return c.after_extension(totals);
     }
 };
 
@@ -1859,18 +1877,9 @@ static int seed_extend_impl(const SeedExtendReq& R, void* d_temp, size_t* temp_b
                                                                              (uint2*)R.hit_window);
         NVB_LAUNCH_CHECK();
     }
-    if (R.BA && !R.PP) NVB_TRY(c.best_traceback());
-    if (c.MO) NVB_TRY(c.second_best());
-    if (R.AO) NVB_TRY(c.all_alignments());
-    if (R.PMO) NVB_TRY(c.pair_candidates());
-    if (R.PP) NVB_TRY(c.paired_rescue());
-    if (R.BA && R.PP) { NVB_TRY(c.best_traceback()); NVB_TRY(c.rescue_traceback()); }
-    if (R.PMO) NVB_TRY(c.pair_second());
+    // without de-duplication every kept hit is a job (no later stage reads counts[2])
     if (!c.dedup) NVB_CUDA_TRY(cudaMemcpyAsync(c.counts + 2, c.counts, sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
-    if (R.n_hits) NVB_CUDA_TRY(cudaMemcpyAsync(R.n_hits, c.counts, 3 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
-    NVB_TRY(c.stage(7));
-    c.SE->valid = true;
-    return NVB_OK;
+    return c.after_extension(c.counts);
 }
 
 extern "C" void nvb_debug_pipeline_path(int path) { g_pipe_path = path; }
@@ -2032,6 +2041,28 @@ extern "C" int nvb_seed_extend_paired_traceback(const nvb_fm_index* fmi, const u
     R.best_score = out->d_mate_score; R.best_pos = out->d_mate_pos; R.n_hits = d_n_hits; R.PP = pair_params; R.PO = out;
     R.BA = mate_alignment; R.MP = mapq; R.PMO = mapq_out;
     return seed_extend_impl(R, d_temp, temp_bytes, stream);
+}
+
+extern "C" int nvb_seed_extend_paired_reseed(const nvb_fm_index* fmi, const uint32_t* d_genome,
+                    const nvb_string_set* reads, uint32_t n_pairs,
+                    const nvb_seed_extend_params* P, uint32_t hit_capacity,
+                    const nvb_pair_params* pair_params, const nvb_pair_out* out,
+                    const nvb_best_alignment_out* mate_alignment,
+                    const nvb_mapq_params* mapq, const nvb_pair_mapq_out* mapq_out,
+                    const nvb_reseed_params* reseed, const nvb_reseed_out* reseed_out,
+                    uint32_t* d_n_hits, void* d_temp, size_t* temp_bytes, void* stream)
+{
+    if (!pair_params || !out || n_pairs > 0x3FFFFFFFu) return NVB_E_INVALID;
+    // the flags are the seed statistics alone: d_min_score and max_read_len are not read
+    if (!reseed || reseed->max_reseed > 254u) return NVB_E_INVALID;
+    if (P && reseed->max_reseed && P->seed_interval < reseed->max_reseed + 1u) return NVB_E_INVALID;
+    SeedExtendReq R = {};
+    R.fmi = fmi; R.genome = d_genome; R.reads = reads; R.n_reads = 2u * n_pairs; R.P = P; R.hit_capacity = hit_capacity;
+    R.best_score = out->d_mate_score; R.best_pos = out->d_mate_pos; R.n_hits = d_n_hits; R.PP = pair_params; R.PO = out;
+    R.BA = mate_alignment; R.MP = mapq; R.PMO = mapq_out;
+    ReseedCall RS = {};
+    RS.RP = reseed; RS.RO = reseed_out;
+    return seed_extend_impl(R, d_temp, temp_bytes, stream, &RS);
 }
 
 extern "C" int nvb_debug_mapq_eval(const int32_t* d_best, const uint8_t* d_has_second, const int32_t* d_second, const uint32_t* d_len,

@@ -451,14 +451,17 @@ class PairedWorkspace:
             self.mate_n_ops = torch.zeros((2, n), dtype=torch.int32, device=dev)
             self.mate_begin = torch.empty((2, n, 2), dtype=torch.int32, device=dev)
         tb = C.c_size_t(0)
-        r = _call_paired(fmi, genome, reads, params, pair, self, None, tb)
+        r = self._call(fmi, genome, reads, params, pair, None, tb)
         if r != -2:
             check(r, "nvb_seed_extend_paired(size query)")
         self.temp = torch.empty(tb.value, dtype=torch.uint8, device=dev)
         self.temp_bytes = tb.value
 
+    def _call(self, fmi, genome, reads, params, pair, temp, tb):
+        return _call_paired(fmi, genome, reads, params, pair, self, temp, tb)
 
-def _call_paired(fmi, genome, reads, params, pair, ws, temp, tb):
+
+def _call_paired(fmi, genome, reads, params, pair, ws, temp, tb, reseed=None):
     s, rd, ps, pp = fmi.struct(), reads.struct(), params.struct(), pair.struct(ws.n_pairs)
     po = PairOutStruct()
     po.d_pair_score, po.d_pair_flags = ws.pair_score.data_ptr(), ws.pair_flags.data_ptr()
@@ -472,10 +475,19 @@ def _call_paired(fmi, genome, reads, params, pair, ws, temp, tb):
         mo.d_second_pair_score, mo.d_second_mate_pos = ws.second_pair_score.data_ptr(), ws.second_mate_pos.data_ptr()
         mo.d_second_mate_strand, mo.d_mate_second_score = ws.second_mate_strand.data_ptr(), ws.mate_second_score.data_ptr()
         mo.d_mate_mapq = ws.mate_mapq.data_ptr()
+    ba = None
     if ws.mate_ops is not None:
         ba = BestAlignmentOutStruct()
         ba.d_ops, ba.max_ops, ba.d_n_ops = ws.mate_ops.data_ptr(), ws.max_ops, ws.mate_n_ops.data_ptr()
         ba.d_begin, ba.d_strand = ws.mate_begin.data_ptr(), None
+    if reseed is not None:
+        rp, ro = reseed.struct(), ReseedOutStruct()
+        ro.d_rounds, ro.d_active = _storage_ptr(ws.rounds), ws.active.data_ptr()
+        ref = lambda x: C.byref(x) if x is not None else None      # noqa: E731
+        return lib().nvb_seed_extend_paired_reseed(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(ws.n_pairs), C.byref(ps),
+                                                   C.c_uint32(ws.hit_capacity), C.byref(pp), C.byref(po), ref(ba), ref(mp), ref(mo),
+                                                   C.byref(rp), C.byref(ro), _p(ws.n_hits), _p(temp), C.byref(tb), stream)
+    if ba is not None:
         return lib().nvb_seed_extend_paired_traceback(C.byref(s), _p(genome), C.byref(rd), C.c_uint32(ws.n_pairs), C.byref(ps),
                                                       C.c_uint32(ws.hit_capacity), C.byref(pp), C.byref(po), C.byref(ba),
                                                       C.byref(mp) if mp is not None else None, C.byref(mo) if mo is not None else None,
@@ -512,6 +524,48 @@ def seed_extend_paired(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedSt
         workspace.mapq_params = mapq
     tb = C.c_size_t(workspace.temp_bytes)
     check(_call_paired(fmi, genome, reads, params, pair, workspace, workspace.temp, tb), "nvb_seed_extend_paired")
+    return workspace
+
+
+class PairedReseedWorkspace(PairedWorkspace):
+    """PairedWorkspace of seed_extend_paired_reseed: the same fields, plus .rounds[2, n] (the rounds each mate was seeded in) and
+    .active[max_reseed + 1] (the mates seeded in each round)"""
+
+    def __init__(self, fmi, genome, reads, params, pair, hit_capacity, reseed: ReseedParams, mapq=None, traceback=False):
+        self.reseed = reseed
+        n = reads.count // 2
+        self.rounds = torch.empty(max(2 * n, 1), dtype=torch.uint8, device=fmi.device)[:2 * n].view(2, n)
+        self.active = torch.zeros(reseed.max_reseed + 1, dtype=torch.int32, device=fmi.device)
+        super().__init__(fmi, genome, reads, params, pair, hit_capacity, mapq, traceback)
+
+    def _call(self, fmi, genome, reads, params, pair, temp, tb):
+        return _call_paired(fmi, genome, reads, params, pair, self, temp, tb, reseed=self.reseed)
+
+
+def seed_extend_paired_reseed(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStringSet, params: SeedExtendParams, pair: PairParams,
+                              reseed: ReseedParams, mapq: Optional[MapqParams] = None, traceback: bool = False,
+                              workspace: Optional[PairedReseedWorkspace] = None, hit_capacity: Optional[int] = None) -> PairedReseedWorkspace:
+    """seed_extend_paired with nvBowtie's reseeding rounds (nvb_seed_extend_paired_reseed): mates whose seeds found nothing or only
+    repeats are seeded again at shifted offsets, up to reseed.max_reseed more times (reseed.min_score is not read: the paired flags are
+    the seed statistics alone), and the pairing, rescue, paired MAPQ and mate tracebacks then run once over every round's alignments.
+    Returns a PairedReseedWorkspace: seed_extend_paired's fields plus .rounds[2, n] and .active.  The call synchronises the stream once
+    per round after the first.  A workspace of an equally-shaped earlier call is reused (reseed and mapq replace its parameters)"""
+    if workspace is None:
+        if hit_capacity is None:
+            hit_capacity = 32 * reads.count + 1024
+        workspace = PairedReseedWorkspace(fmi, genome, reads, params, pair, hit_capacity, reseed, mapq, traceback)
+    else:
+        if reseed.max_reseed + 1 > workspace.active.numel():
+            raise ValueError("seed_extend_paired_reseed: the workspace was created for at most %d rounds" % workspace.active.numel())
+        if traceback and workspace.mate_ops is None:
+            raise ValueError("seed_extend_paired_reseed(traceback=True): the workspace was created without traceback outputs")
+        workspace.reseed = reseed
+        if mapq is not None:
+            if workspace.mate_mapq is None:
+                raise ValueError("seed_extend_paired_reseed(mapq=...): the workspace was created without mapq outputs")
+            workspace.mapq_params = mapq
+    tb = C.c_size_t(workspace.temp_bytes)
+    check(workspace._call(fmi, genome, reads, params, pair, workspace.temp, tb), "nvb_seed_extend_paired_reseed")
     return workspace
 
 
