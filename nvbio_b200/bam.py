@@ -11,6 +11,7 @@ import numpy as np
 import torch
 from ._lib import lib, check, BamInStruct, BamOutStruct, BamAllInStruct
 from .finish import FinishedAlignments
+from .fmindex import MAX_LENGTH
 from .strings import PackedStringSet
 
 NVB_E_TEMP_SIZE = -2
@@ -31,9 +32,11 @@ class ContigTable:
         self.lengths = np.asarray(lengths, np.int64)
         if (self.lengths <= 0).any():
             raise ValueError("ContigTable: contig lengths must be positive")
+        if (self.lengths >= 1 << 31).any():
+            raise ValueError("ContigTable: a contig of 2^31 or more bases has no BAM position (l_ref and POS are int32)")
         self.begin = np.concatenate([[0], np.cumsum(self.lengths)]).astype(np.int64)
-        if self.begin[-1] >= 1 << 32:
-            raise ValueError("ContigTable: the genome is longer than 2^32 - 1 symbols")
+        if self.begin[-1] > MAX_LENGTH:
+            raise ValueError("ContigTable: the genome is longer than 2^32 - 2 symbols (the longest FM-index text)")
         self._dev = {}
 
     @staticmethod

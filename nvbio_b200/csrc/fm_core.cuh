@@ -44,7 +44,7 @@ struct FmIndex {
 };
 
 static inline bool valid_fmindex(const nvb_fm_index* f) {
-    if (!f || !f->d_bwt_occ) return false;
+    if (!f || !f->d_bwt_occ || f->length > NVB_FM_MAX_LENGTH) return false;
     const uint32_t I = f->sa_interval;
     if (I != 0 && (I & (I - 1)) != 0) return false;           // power of two
     if (f->d_ktab && (f->ktab_k < 1 || f->ktab_k > 16 || f->ktab_located > 5u)) return false;

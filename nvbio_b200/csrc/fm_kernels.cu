@@ -536,8 +536,8 @@ int nvb_dict_build_occ(const void* d_text, uint32_t word_bits, uint64_t n_symbol
 int nvb_fm_build_occ(const uint32_t* d_bwt, uint32_t n, void* d_bwt_occ, uint32_t h_L2[5],
                      void* d_temp, size_t* temp_bytes, void* stream)
 {
-    if (!temp_bytes || !h_L2 || (n && (!d_bwt || !d_bwt_occ))) return NVB_E_INVALID;
-    const uint32_t n_blocks = (n + 63u) / 64u;
+    if (!temp_bytes || !h_L2 || n > NVB_FM_MAX_LENGTH || (n && (!d_bwt || !d_bwt_occ))) return NVB_E_INVALID;
+    const uint32_t n_blocks = (uint32_t)(((uint64_t)n + 63u) / 64u);     // n + 63 wraps a uint32 from n = 2^32 - 63 on
     TempCarver tc(d_temp);
     uint4* counts = tc.take<uint4>(n_blocks + 1);
     uint4* excl   = tc.take<uint4>(n_blocks + 1);

@@ -178,7 +178,7 @@ extern "C" int nvb_fm_build_bwt(const uint32_t* d_text, uint32_t n32, uint32_t* 
                                 uint32_t* d_ssa, uint32_t sa_interval, uint32_t* d_sa,
                                 void* d_temp, size_t* temp_bytes, void* stream)
 {
-    if (!temp_bytes || !h_primary || n32 == 0 || !d_text) return NVB_E_INVALID;
+    if (!temp_bytes || !h_primary || n32 == 0 || n32 > NVB_FM_MAX_LENGTH || !d_text) return NVB_E_INVALID;
     if (sa_interval == 0) sa_interval = 16;
     if (sa_interval & (sa_interval - 1)) return NVB_E_INVALID;
     const uint64_t n = n32;

@@ -9,6 +9,7 @@ from .strings import PackedStringSet
 
 MATCH_FORWARD_ORDER = 1
 MATCH_COMPLEMENT = 2
+MAX_LENGTH = 0xFFFFFFFE     # NVB_FM_MAX_LENGTH: the longest text an index may have
 
 
 # device memory that build_ktab leaves free after the per-row array (a seed + extend call's temp buffers); without that room the
