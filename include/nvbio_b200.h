@@ -599,7 +599,8 @@ int nvb_seed_extend_all(const nvb_fm_index* fmi, const uint32_t* d_genome,
  * nvBowtie/bowtie2/cuda/aligner_best_approx_paired.h, score_opposite_inl.h:90-266, alignment_utils.h:62-95 PE_POLICY_FR).
  *
  * reads = 2*n_pairs strings: mate 1 of pair p at index p, mate 2 at index n_pairs + p.  Every mate is seeded and extended
- * on its own (nvb_seed_extend with both_strands = 1, which is required).  Per pair:
+ * on its own (nvb_seed_extend with both_strands = 1, which is required).  Per pair, under the default FR policy (the other policies,
+ * --no-overlap, discordant pairs and --no-mixed: policy / flags below):
  *   - if both mates have a best alignment, on opposite strands, the forward one starting at or before the reverse one,
  *     ending at or before it, and the fragment [begin of the forward mate, end of the reverse mate) has a length in
  *     [min_frag, max_frag]: the pair is CONCORDANT as it stands (alignment begin := end - read length, clamped at 0);
@@ -617,11 +618,42 @@ int nvb_seed_extend_all(const nvb_fm_index* fmi, const uint32_t* d_genome,
  * Outputs (mate m of pair p at index m*n_pairs + p): d_pair_score (sum of the two mates' scores, INT_MIN when unpaired),
  * d_pair_flags (NVB_PAIR_*), d_mate_score (INT_MIN = unaligned), d_mate_pos (genome coordinate one past the last aligned
  * base, 0xFFFFFFFF = unaligned), d_mate_strand (0 forward, 1 reverse complement). */
+/* Orientation and options (policy / flags; nvBowtie's --fr / --rf / --ff / --rr, --no-overlap, --no-mixed, --no-discordant,
+ * params.cpp:160-170).  Zero-initialise the struct (memset or `= {0}`): every field added later means "as before" at zero, and the
+ * zeroed policy and flags are the FR pairing above, bit for bit.
+ *   policy: NVB_PE_FR (0), NVB_PE_RF, NVB_PE_FF or NVB_PE_RR.  The framing of anchor mate a aligned on strand t is nvBowtie's
+ *     frame_opposite_mate(policy, a, anchor_fw = (t == 0)) (alignment_utils.h:61-98): whether the other mate lies to the left or the
+ *     right of the anchor, and its strand.  (nvBowtie numbers io::PE_POLICY_* FF 0, FR 1, RF 2, RR 3; here 0 is FR so that a zeroed
+ *     struct keeps today's pairing.)  Concordance, with (left, o) the framing of mate 1: mate 2 is on strand o and, with L / R the left
+ *     / right mate as framed, L.b <= R.b, L.e <= R.e, R.e > L.b and min_frag <= R.e - L.b <= max_frag -- the FR test above for NVB_PE_FR.
+ *     The rescue aligns the other mate's strand-o string against [b, min(b + max_frag, genome length)) when it lies to the right of an
+ *     anchor at [b, e), against [max(e - max_frag, 0), e) when it lies to the left; the rescued mate gets strand o.
+ *   NVB_PE_NO_OVERLAP: concordance also needs L.e <= R.b, and the rescue window starts at e (right) / ends at b (left).
+ *   NVB_PE_DISCORDANT (requires mapq / mapq_out): after the rescue, an UNPAIRED pair whose two mates both have a best alignment with
+ *     score >= d_min_score[len] and no single-end second alignment (second score INT_MIN: both unique) becomes NVB_PAIR_DISCORDANT
+ *     (nvBowtie's mark_discordant, aligner_init.cu:459-482).  Off at zero, although nvBowtie's default is on: a zeroed struct keeps
+ *     today's outputs.  A discordant pair reports pair score s1 + s2, the mates' single-end alignments and tracebacks, no second pair,
+ *     and both mates' MAPQ = BowtieMapq2(s1 + s2, no second, perfect (len1 + len2) * match_bonus, min d_min_score[len1] +
+ *     d_min_score[len2]), as MapqFunctorPE scores it.
+ *   NVB_PE_NO_MIXED: after the discordant marking, both mates of every pair still UNPAIRED are reported unaligned in every output
+ *     (score INT_MIN, pos 0xFFFFFFFF, strand 0, MAPQ 0, mate second score INT_MIN, n_ops 0, begin (0xFFFFFFFF, 0xFFFFFFFF)).  With
+ *     NVB_PE_DISCORDANT also set, discordant pairs are still reported (Bowtie2's meaning of the two options).  Deliberate deviation:
+ *     nvBowtie tracks no unpaired alignment under --no-mixed and so never marks a discordant pair there.
+ * NVB_E_INVALID (before any CUDA call) for policy > 3 or an unknown flag bit, and for NVB_PE_DISCORDANT without mapq / mapq_out. */
 typedef struct nvb_pair_params {
     uint32_t min_frag, max_frag;
     int32_t  min_mate_score;
     uint32_t rescue_capacity;
+    uint32_t policy;            /* NVB_PE_FR (0), NVB_PE_RF, NVB_PE_FF, NVB_PE_RR */
+    uint32_t flags;             /* NVB_PE_NO_OVERLAP | NVB_PE_DISCORDANT | NVB_PE_NO_MIXED */
 } nvb_pair_params;
+#define NVB_PE_FR               0u
+#define NVB_PE_RF               1u
+#define NVB_PE_FF               2u
+#define NVB_PE_RR               3u
+#define NVB_PE_NO_OVERLAP       1u
+#define NVB_PE_DISCORDANT       2u
+#define NVB_PE_NO_MIXED         4u
 typedef struct nvb_pair_out {
     int32_t*  d_pair_score;     /* [n_pairs]   */
     uint32_t* d_pair_flags;     /* [n_pairs]   */
@@ -631,9 +663,10 @@ typedef struct nvb_pair_out {
     uint32_t* d_n_rescue;       /* [2] full-DP jobs run, wanted (may be NULL) */
 } nvb_pair_out;
 #define NVB_PAIR_UNPAIRED       0u
-#define NVB_PAIR_CONCORDANT     1u    /* the mates' independent best alignments form a proper FR pair */
+#define NVB_PAIR_CONCORDANT     1u    /* the mates' independent best alignments form a proper pair under the policy */
 #define NVB_PAIR_RESCUED_MATE1  2u    /* mate 1 was placed by the opposite-mate DP next to mate 2's alignment */
 #define NVB_PAIR_RESCUED_MATE2  4u
+#define NVB_PAIR_DISCORDANT     8u    /* not concordant, both mates aligned uniquely (NVB_PE_DISCORDANT): a pair without the proper-pair bit */
 
 int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d_genome,
                     const nvb_string_set* reads, uint32_t n_pairs,
@@ -646,19 +679,20 @@ int nvb_seed_extend_paired(const nvb_fm_index* fmi, const uint32_t* d_genome,
  * unchanged for the same inputs; call the pair it reports P*.
  *   Mate candidates: those of nvb_seed_extend_mapq for that read (score s, strand t, end e, tie index), begin b = e - len clamped at 0,
  *   and only those with s >= d_min_score[len].  Candidates with equal (strand, end) are merged into the one with the highest (s, -tie).
- *   Candidate pairs of a pair that is not UNPAIRED: (1) every FR-concordant combination of one candidate of each mate (the concordance
- *   test above), score s1 + s2; (2) every opposite-mate job the call ran (j < rescue_capacity) whose score rs reaches min_mate_score and
- *   d_min_score[len]: the anchor's single-end best plus the rescued alignment (end = window begin + sink.x, strand opposite to the
- *   anchor), score = anchor score + rs, the rescued mate's tie index 0xFFFFFFFF.  Rescues exist only for pairs that were not concordant
- *   as they stood.
+ *   Candidate pairs of a CONCORDANT or RESCUED pair: (1) every combination of one candidate of each mate that is concordant under the
+ *   policy and flags (the concordance test of nvb_pair_params), score s1 + s2; (2) every opposite-mate job the call ran
+ *   (j < rescue_capacity) whose score rs reaches min_mate_score and d_min_score[len]: the anchor's single-end best plus the rescued
+ *   alignment (end = window begin + sink.x, strand as the policy frames it), score = anchor score + rs, the rescued mate's tie index
+ *   0xFFFFFFFF.  Rescues exist only for pairs that were not concordant as they stood.  A DISCORDANT pair has no candidate pair.
  *   A candidate pair is not distinct from P* when both of its mates fail the single-end test against P*'s matching mate (same strand,
  *   end within len/2).  The second-best pair is the distinct candidate pair with the largest score, ties to the smaller mate-1 tie index,
  *   then the smaller mate-2 tie index -- one answer whatever the job order, path, de-duplication, exact shortcut or seed split.
  *   A distinct pair may score ABOVE P*: two non-best alignments can be concordant where the bests are not and the rescue missed them.
  *   It is still reported as the second pair (a low MAPQ); how the best pair is chosen does not change.
  *   d_mate_mapq of a CONCORDANT or RESCUED pair, both mates: BowtieMapq2 with best = pair score, the second pair's score when there is
- *   one, perfect = (len1 + len2) * match_bonus, min = d_min_score[len1] + d_min_score[len2], monotone when match_bonus == 0.  Mates of an
- *   UNPAIRED pair: their single-end MAPQ (nvb_seed_extend_mapq on the 2n reads); an unaligned mate: 0.
+ *   one, perfect = (len1 + len2) * match_bonus, min = d_min_score[len1] + d_min_score[len2], monotone when match_bonus == 0; of a
+ *   DISCORDANT pair the same without a second.  Mates of an UNPAIRED pair: their single-end MAPQ (nvb_seed_extend_mapq on the 2n reads),
+ *   0 under NVB_PE_NO_MIXED; an unaligned mate: 0.
  * Mate m of pair p at index m * n_pairs + p, as in nvb_pair_out.  Validation as nvb_seed_extend_paired and nvb_seed_extend_mapq:
  * NVB_E_INVALID when mapq, mapq_out, d_min_score, d_second_pair_score or d_mate_mapq is NULL, or max_read_len < reads->length.
  * The temp size grows by about 36 bytes per unit of hit_capacity plus 28 bytes per read; nvb_seed_extend_paired does not carve it. */
@@ -682,8 +716,8 @@ int nvb_seed_extend_paired_mapq(const nvb_fm_index* fmi, const uint32_t* d_genom
  * nvb_seed_extend_paired_mapq for the same inputs; concordance still uses begin = end - length.  mate_alignment is required and laid out
  * over the 2*n_pairs mates (mate m of pair p at index m * n_pairs + p), its fields meaning what they mean in nvb_best_alignment_out;
  * d_strand may be NULL (d_mate_strand holds the same).  Per mate:
- *   - unaligned: n_ops = 0, begin = (0xFFFFFFFF, 0xFFFFFFFF);
- *   - keeping its own single-end best (CONCORDANT and UNPAIRED pairs, the anchor of a rescued pair): the banded traceback of that
+ *   - unaligned (a mate of an UNPAIRED pair under NVB_PE_NO_MIXED included): n_ops = 0, begin = (0xFFFFFFFF, 0xFFFFFFFF);
+ *   - keeping its own single-end best (CONCORDANT, DISCORDANT and UNPAIRED pairs, the anchor of a rescued pair): the banded traceback of that
  *     best (strand, window) job, equal to what nvb_seed_extend_traceback reports for the read when the 2*n_pairs mates run single end;
  *   - rescued (NVB_PAIR_RESCUED_MATE1 / 2): the full-matrix traceback of the winning opposite-mate job (the mate on the rescue strand
  *     against the rescue window), equal to nvb_gotoh_traceback of that job: begin = (window begin + source.x, source.y), the traced
@@ -722,7 +756,8 @@ int nvb_seed_extend_paired_traceback(const nvb_fm_index* fmi, const uint32_t* d_
  *   (round, tie), so the second-best pair's tie-break is round-major; rescue_capacity and d_n_rescue keep their meaning (one rescue
  *   pass, in pair order).
  *   Deliberate deviation: nvBowtie scores the opposite mate for every anchor in every round; here the pairing decides once, after the
- *   last round -- the deviation nvb_seed_extend_paired already makes within a single round.
+ *   last round -- the deviation nvb_seed_extend_paired already makes within a single round.  The policy and flags of pair_params apply
+ *   to that one pairing; NVB_PE_DISCORDANT needs mapq / mapq_out.
  * Outputs: reseed_out->d_rounds is per mate, [2*n_pairs] in the mate layout above; d_active[r] counts the mates seeded in round r; every
  * other output means what it means in the three paired calls.  With max_reseed == 0 every output is that of nvb_seed_extend_paired,
  * _paired_mapq or _paired_traceback (whichever the optional groups select).  n_pairs == 0: NVB_OK with d_active zeroed.
@@ -811,7 +846,8 @@ int nvb_finish_alignments(const uint32_t* d_genome, uint32_t genome_len,
  * mate sees an unmapped mate.
  * A mapped record:
  *   FLAG   0x10 on strand 1; paired: 0x1, 0x40 / 0x80 for mate 1 / 2, 0x2 when the pair is CONCORDANT or RESCUED and both mates are
- *          mapped, 0x8 when the mate is unmapped, 0x20 when the mate is mapped on strand 1;
+ *          mapped (never for NVB_PAIR_DISCORDANT: such records carry 0x1, 0x40 / 0x80 and the mate fields without 0x2), 0x8 when
+ *          the mate is unmapped, 0x20 when the mate is mapped on strand 1;
  *   MAPQ   d_mapq, 255 without it;   bin = reg2bin(pos, pos + M + D) (the specification's, hts_reg2bin(beg, end, 14, 5));
  *   CIGAR  the finish output;  SEQ the strand's string (strand 1 reverse-complemented, as the traceback saw it) in BAM's 4-bit
  *          =ACMGRSVTWYHKDBN code (A 1, C 2, G 4, T 8, N 15);  QUAL reversed for strand 1, all 0xFF without qualities;

@@ -9,6 +9,7 @@ from .fmindex import (FMIndexDevice, FMIndexFilterDevice, rank, rank4, match, ma
                       MATCH_FORWARD_ORDER, MATCH_COMPLEMENT)
 from . import aln                                                                # noqa: F401
 from .pipeline import SeedExtendParams, seed_extend, StreamingSeedExtend, PairParams, seed_extend_paired, MapqParams, seed_extend_all, AllAlignments, ReseedParams, seed_extend_reseed, seed_extend_paired_reseed     # noqa: F401
+from .pipeline import PAIR_UNPAIRED, PAIR_CONCORDANT, PAIR_RESCUED_MATE1, PAIR_RESCUED_MATE2, PAIR_DISCORDANT    # noqa: F401
 from .finish import finish_alignments, FinishedAlignments                        # noqa: F401
 from .bam import ContigTable, BamRecords, bam_records, bam_records_all, bam_header, write_bam, numbered_names    # noqa: F401
 from .bgzf import BgzfBlocks, BgzfCall, bgzf_compress                           # noqa: F401

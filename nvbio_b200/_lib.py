@@ -121,7 +121,8 @@ class AllOutStruct(C.Structure):            # nvb_all_out
 
 
 class PairParamsStruct(C.Structure):        # nvb_pair_params
-    _fields_ = [("min_frag", C.c_uint32), ("max_frag", C.c_uint32), ("min_mate_score", C.c_int32), ("rescue_capacity", C.c_uint32)]
+    _fields_ = [("min_frag", C.c_uint32), ("max_frag", C.c_uint32), ("min_mate_score", C.c_int32), ("rescue_capacity", C.c_uint32),
+                ("policy", C.c_uint32), ("flags", C.c_uint32)]
 
 
 class PairOutStruct(C.Structure):           # nvb_pair_out

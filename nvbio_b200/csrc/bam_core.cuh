@@ -139,7 +139,8 @@ __host__ __device__ inline uint64_t bam_plan_record(const BamIn& in, uint32_t k,
     if (mate) {
         const bool mm = mate->state == BAM_MAPPED;
         flag |= 0x1u | ((k & 1u) ? 0x80u : 0x40u);
-        if (in.pair_flags[k >> 1] != NVB_PAIR_UNPAIRED && mapped && mm) flag |= 0x2u;
+        const uint32_t pf = in.pair_flags[k >> 1];
+        if ((pf == NVB_PAIR_CONCORDANT || pf == NVB_PAIR_RESCUED_MATE1 || pf == NVB_PAIR_RESCUED_MATE2) && mapped && mm) flag |= 0x2u;
         if (!mm) flag |= 0x8u;
         else if (mate->strand) flag |= 0x20u;
         if (mapped) {

@@ -67,6 +67,10 @@ static inline StrSet make_strset(const nvb_string_set* s) {
 static inline bool valid_strset(const nvb_string_set* s) {
     return s && s->d_words && (s->bits == 2 || s->bits == 4 || s->bits == 8);
 }
+// a known pairing policy and no unknown flag bit (nvb_pair_params)
+static inline bool valid_pair_policy(const nvb_pair_params* pp) {
+    return pp->policy <= NVB_PE_RR && (pp->flags & ~(NVB_PE_NO_OVERLAP | NVB_PE_DISCORDANT | NVB_PE_NO_MIXED)) == 0u;
+}
 
 __host__ __device__ __forceinline__ uint32_t str_off(const StrSet& s, uint32_t i) { return s.offsets ? s.offsets[i] : i * s.stride; }
 __host__ __device__ __forceinline__ uint32_t str_len(const StrSet& s, uint32_t i) { return s.lengths ? s.lengths[i] : s.length; }

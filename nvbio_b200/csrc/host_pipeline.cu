@@ -103,6 +103,9 @@ extern "C" int nvb_pipeline_create(const nvb_fm_index* fmi, const uint32_t* d_ge
     if (!fmi || !d_genome || !params || !out || n_reads == 0 || depth == 0 || depth > 16) return NVB_E_INVALID;
     if (!(read_bits == 2 || read_bits == 4) || (uint64_t)words_per_read * (32u / read_bits) < read_len) return NVB_E_INVALID;
     if (pair_params && (n_reads & 1u)) return NVB_E_INVALID;
+    // every policy and flag but NVB_PE_DISCORDANT passes through to nvb_seed_extend_paired; the pipeline has no MAPQ stage to mark
+    // discordant pairs with
+    if (pair_params && (!valid_pair_policy(pair_params) || (pair_params->flags & NVB_PE_DISCORDANT))) return NVB_E_INVALID;
     nvb_pipeline* p = new (std::nothrow) nvb_pipeline();
     if (!p) return (int)cudaErrorMemoryAllocation;
     *out = nullptr;

@@ -978,13 +978,8 @@ pair_classify_kernel(const PipeGeom g, const uint32_t n_pairs, const nvb_pair_pa
     for (int k = 0; k < 2; ++k) {
         mate_score[k * n_pairs + p] = m[k].score; mate_pos[k * n_pairs + p] = m[k].end; mate_strand[k * n_pairs + p] = (uint8_t)m[k].strand;
     }
-    bool conc = m[0].has && m[1].has && (m[0].strand != m[1].strand);
-    if (conc) {
-        const MateBest& f = m[0].strand == 0 ? m[0] : m[1];
-        const MateBest& r = m[0].strand == 0 ? m[1] : m[0];
-        conc = fr_concordant(f.beg, f.end, r.beg, r.end, pp.min_frag, pp.max_frag);
-    }
-    if (conc) {
+    if (m[0].has && m[1].has &&
+        pe_concordant(pp.policy, pp.flags, m[0].strand, m[0].beg, m[0].end, m[1].strand, m[1].beg, m[1].end, pp.min_frag, pp.max_frag)) {
         pair_score[p] = m[0].score + m[1].score; pair_flags[p] = NVB_PAIR_CONCORDANT;
         want[2 * p] = want[2 * p + 1] = 0u;
         return;
@@ -995,8 +990,7 @@ pair_classify_kernel(const PipeGeom g, const uint32_t n_pairs, const nvb_pair_pa
         uint32_t w = 0u, ps = 0u, to = 0u, tl = 0u;
         if (m[a].has && m[a].score >= pp.min_mate_score) {
             const uint32_t o_read = (uint32_t)(1 - a) * n_pairs + p;
-            if (m[a].strand == 0u) { to = m[a].beg; const uint32_t e = (g.genome_len - to) < pp.max_frag ? g.genome_len : to + pp.max_frag; tl = e - to; ps = 2u * o_read + 1u; }
-            else                   { to = m[a].end > pp.max_frag ? m[a].end - pp.max_frag : 0u; tl = m[a].end - to; ps = 2u * o_read; }
+            ps = 2u * o_read + pe_rescue_window(pp.policy, pp.flags, (uint32_t)a, m[a].strand, m[a].beg, m[a].end, pp.max_frag, g.genome_len, to, tl);
             w = (tl >= 1u && str_len[ps] >= 1u) ? 1u : 0u;
         }
         want[2 * p + a] = w; w_pstr[2 * p + a] = ps; w_toff[2 * p + a] = to; w_tlen[2 * p + a] = tl;
@@ -1031,9 +1025,14 @@ __device__ __forceinline__ bool usable_rescue(const nvb_pair_params& pp, const u
     return true;
 }
 
+// one thread per pair that was not concordant as it stood: the best rescue; failing that, with NVB_PE_DISCORDANT, the discordant test
+// (min_score: the MAPQ's table, second_key: the single-end second best of every read, both read only then), and failing that, with
+// NVB_PE_NO_MIXED, both mates unaligned -- their best_key cleared too, so that the traceback reports them unaligned
 __global__ void __launch_bounds__(256)
 pair_finalize_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const uint32_t* __restrict__ want, const uint32_t* __restrict__ job_idx,
                      const uint32_t* __restrict__ w_toff, const int32_t* __restrict__ rs_score, const uint2* __restrict__ rs_sink,
+                     const uint32_t* __restrict__ str_len, const int32_t* __restrict__ min_score,
+                     const unsigned long long* __restrict__ second_key, unsigned long long* __restrict__ best_key,
                      int32_t* __restrict__ pair_score, uint32_t* __restrict__ pair_flags,
                      int32_t* __restrict__ mate_score, uint32_t* __restrict__ mate_pos, uint8_t* __restrict__ mate_strand)
 {
@@ -1047,13 +1046,33 @@ pair_finalize_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const uin
         const int32_t sum = mate_score[a * n_pairs + p] + rs;
         if (sum > best_sum) { best_sum = sum; best_a = a; best_rs = rs; best_pos = end; }
     }
-    if (best_a < 0) return;
-    const int o = 1 - best_a;
-    pair_score[p] = best_sum;
-    pair_flags[p] = o == 0 ? NVB_PAIR_RESCUED_MATE1 : NVB_PAIR_RESCUED_MATE2;
-    mate_score[o * n_pairs + p] = best_rs;
-    mate_pos[o * n_pairs + p] = best_pos;
-    mate_strand[o * n_pairs + p] = (uint8_t)(1u - mate_strand[best_a * n_pairs + p]);
+    const uint32_t r0 = p, r1 = n_pairs + p;
+    if (best_a >= 0) {
+        const int o = 1 - best_a;
+        const uint32_t ra = best_a * n_pairs + p;
+        pair_score[p] = best_sum;
+        pair_flags[p] = o == 0 ? NVB_PAIR_RESCUED_MATE1 : NVB_PAIR_RESCUED_MATE2;
+        mate_score[o * n_pairs + p] = best_rs;
+        mate_pos[o * n_pairs + p] = best_pos;
+        mate_strand[o * n_pairs + p] = (uint8_t)pe_frame(pp.policy, (uint32_t)best_a, mate_strand[ra]).strand;
+        return;
+    }
+    if (pp.flags & NVB_PE_DISCORDANT) {
+        bool unique = true;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const uint32_t r = k ? r1 : r0;
+            unique = unique && mate_pos[r] != 0xFFFFFFFFu && mate_score[r] >= min_score[str_len[2u * r]] && second_key[r] == 0ull;
+        }
+        if (unique) { pair_score[p] = mate_score[r0] + mate_score[r1]; pair_flags[p] = NVB_PAIR_DISCORDANT; return; }
+    }
+    if (pp.flags & NVB_PE_NO_MIXED) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const uint32_t r = k ? r1 : r0;
+            mate_score[r] = INT_MIN; mate_pos[r] = 0xFFFFFFFFu; mate_strand[r] = 0; best_key[r] = 0ull;
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1141,7 +1160,7 @@ pair_second_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const nvb_m
                    const int32_t* __restrict__ pair_score, const uint32_t* __restrict__ pair_flags,
                    const uint32_t* __restrict__ mate_pos, const uint8_t* __restrict__ mate_strand,
                    int32_t* __restrict__ second_pair_score, uint32_t* __restrict__ second_mate_pos, uint8_t* __restrict__ second_mate_strand,
-                   uint8_t* __restrict__ mate_mapq)
+                   int32_t* __restrict__ mate_second_score, uint8_t* __restrict__ mate_mapq)
 {
     const uint32_t p = blockIdx.x * 256 + threadIdx.x;
     if (p >= n_pairs) return;
@@ -1150,21 +1169,28 @@ pair_second_kernel(const uint32_t n_pairs, const nvb_pair_params pp, const nvb_m
     PairSecond ps;
     ps.init(mate_pos[r0], mate_strand[r0], len[0], mate_pos[r1], mate_strand[r1], len[1]);
     const uint32_t flags = pair_flags[p];
+    if (flags == NVB_PAIR_UNPAIRED && (pp.flags & NVB_PE_NO_MIXED)) {       // both mates reported unaligned
+        mate_mapq[r0] = 0; mate_mapq[r1] = 0;
+        if (mate_second_score) { mate_second_score[r0] = INT_MIN; mate_second_score[r1] = INT_MIN; }
+    }
     if (flags != NVB_PAIR_UNPAIRED) {
-        MateCands m[2];
+        if (flags != NVB_PAIR_DISCORDANT) {                                 // a discordant pair has no candidate pair
+            MateCands m[2];
 #pragma unroll
-        for (int k = 0; k < 2; ++k) {
-            const uint32_t r = k ? r1 : r0, b = seg[r];
-            m[k].end = m_end + b; m[k].score = m_score + b; m[k].tie = m_tie + b; m[k].n_fw = n_fw[r]; m[k].n = n_merged[r]; m[k].len = len[k];
-        }
-        pair_combinations(m, pp.min_frag, pp.max_frag, ps);
-        // rescues: the anchor's single-end best with the rescued alignment of the other mate (tie index 0xFFFFFFFF)
-        for (int a = 0; a < 2; ++a) {
-            const uint32_t ra = a ? r1 : r0;
-            int32_t rs; uint32_t end;
-            if (!usable_rescue(pp, want, job_idx, w_toff, rs_score, rs_sink, 2u * p + a, rs, end) || rs < mp.d_min_score[len[1 - a]]) continue;
-            const unsigned long long key = best_key[ra];
-            ps.offer_rescue(a, best_key_score(key) + rs, se_pos[ra], se_strand[ra], best_key_index(key), end);
+            for (int k = 0; k < 2; ++k) {
+                const uint32_t r = k ? r1 : r0, b = seg[r];
+                m[k].end = m_end + b; m[k].score = m_score + b; m[k].tie = m_tie + b; m[k].n_fw = n_fw[r]; m[k].n = n_merged[r]; m[k].len = len[k];
+            }
+            pair_combinations(m, pp.policy, pp.flags, pp.min_frag, pp.max_frag, ps);
+            // rescues: the anchor's single-end best with the rescued alignment of the other mate (tie index 0xFFFFFFFF)
+            for (int a = 0; a < 2; ++a) {
+                const uint32_t ra = a ? r1 : r0;
+                int32_t rs; uint32_t end;
+                if (!usable_rescue(pp, want, job_idx, w_toff, rs_score, rs_sink, 2u * p + a, rs, end) || rs < mp.d_min_score[len[1 - a]]) continue;
+                const unsigned long long key = best_key[ra];
+                ps.offer_rescue(a, best_key_score(key) + rs, se_pos[ra], se_strand[ra], best_key_index(key), end,
+                                pe_frame(pp.policy, (uint32_t)a, se_strand[ra]).strand);
+            }
         }
         const uint8_t q = (uint8_t)bowtie_mapq2(pair_score[p], ps.has, ps.score, (int32_t)(len[0] + len[1]) * mp.match_bonus,
                                                 mp.d_min_score[len[0]] + mp.d_min_score[len[1]], mp.match_bonus == 0);
@@ -1630,7 +1656,7 @@ struct PipeCall : SeedExtendReq {
                                                                   se_pos, rb_strand, best_key, pw_want, pw_idx, pw_toff, rs_score, rs_sink,
                                                                   PO->d_pair_score, PO->d_pair_flags, PO->d_mate_pos, PO->d_mate_strand,
                                                                   PMO->d_second_pair_score, PMO->d_second_mate_pos, PMO->d_second_mate_strand,
-                                                                  PMO->d_mate_mapq);
+                                                                  PMO->d_mate_second_score, PMO->d_mate_mapq);
         return launched();
     }
 
@@ -1654,7 +1680,8 @@ struct PipeCall : SeedExtendReq {
             size_t fb = full_bytes;
             NVB_TRY(nvb_gotoh_score_indirect(P->type, &P->scheme, &v.pats, str_quals, &v.txts, pcounts, cap, rs_score, (nvb_uint2*)rs_sink, full_tmp, &fb, s));
         }
-        pair_finalize_kernel<<<pgrid, 256, 0, s>>>(n_pairs, *PP, pw_want, pw_idx, pw_toff, rs_score, rs_sink, PO->d_pair_score, PO->d_pair_flags,
+        pair_finalize_kernel<<<pgrid, 256, 0, s>>>(n_pairs, *PP, pw_want, pw_idx, pw_toff, rs_score, rs_sink, str_len, MP ? MP->d_min_score : nullptr,
+                                                    second_key, best_key, PO->d_pair_score, PO->d_pair_flags,
                                                     PO->d_mate_score, PO->d_mate_pos, PO->d_mate_strand);
         NVB_LAUNCH_CHECK();
         if (PO->d_n_rescue) NVB_CUDA_TRY(cudaMemcpyAsync(PO->d_n_rescue, pcounts, 2 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
@@ -1815,6 +1842,7 @@ static int seed_extend_impl(const SeedExtendReq& R, void* d_temp, size_t* temp_b
     if (R.PP) {
         if (!R.PO->d_pair_score || !R.PO->d_pair_flags || !R.PO->d_mate_score || !R.PO->d_mate_pos || !R.PO->d_mate_strand) return NVB_E_INVALID;
         if (!P || !P->both_strands || (R.n_reads & 1u) || R.PP->max_frag == 0 || R.PP->min_frag > R.PP->max_frag) return NVB_E_INVALID;
+        if (!valid_pair_policy(R.PP) || ((R.PP->flags & NVB_PE_DISCORDANT) && !R.PMO)) return NVB_E_INVALID;   // discordance needs the MAPQ
     }
     if (!valid_fmindex(R.fmi) || !R.fmi->d_ssa || !R.genome || !valid_strset(R.reads) || !P) return NVB_E_INVALID;
     if (R.reads->bits == 8) return NVB_E_UNSUPPORTED;

@@ -246,11 +246,57 @@ __host__ __device__ inline uint32_t select_distinct(unsigned long long* es, uint
 // begin of an alignment ending at `end` of a read of length len: end - len, clamped at 0 (no traceback: soft clips and indels ignored)
 __host__ __device__ __forceinline__ uint32_t aln_begin(uint32_t end, uint32_t len) { return end > len ? end - len : 0u; }
 
-// FR concordance of a forward mate [fb, fe) and a reverse mate [rb, re): the forward one starts and ends no later than the reverse one and
-// the fragment [fb, re) is non-empty with a length in [min_frag, max_frag] (nvb_seed_extend_paired, PE_POLICY_FR)
-__host__ __device__ __forceinline__ bool fr_concordant(uint32_t fb, uint32_t fe, uint32_t rb, uint32_t re, uint32_t min_frag, uint32_t max_frag)
+// ---------------------------------------------------------------------------------------------
+// Paired-end policy (nvb_pair_params.policy / flags).  nvBowtie numbers its io::PE_POLICY_* FF 0, FR 1, RF 2, RR 3
+// (nvbio/io/sequence/sequence.h:192-195); the C ABI numbers them NVB_PE_FR 0, NVB_PE_RF 1, NVB_PE_FF 2, NVB_PE_RR 3, so that a zeroed
+// nvb_pair_params keeps the FR pairing:  NVB_PE_FR -> PE_POLICY_FR, NVB_PE_RF -> PE_POLICY_RF, NVB_PE_FF -> PE_POLICY_FF,
+// NVB_PE_RR -> PE_POLICY_RR.
+// ---------------------------------------------------------------------------------------------
+struct PeFrame { bool left; uint32_t strand; };     // the other mate lies to the LEFT of the anchor; the strand it aligns on
+
+// where the other mate of anchor mate a (0 = mate 1) aligned on strand t (0 forward) lies: nvBowtie's frame_opposite_mate
+// (nvBowtie/bowtie2/cuda/alignment_utils.h:61-98) with anchor_fw = (t == 0)
+__host__ __device__ __forceinline__ PeFrame pe_frame(uint32_t policy, uint32_t a, uint32_t t)
 {
-    return fb <= rb && fe <= re && re > fb && (re - fb) >= min_frag && (re - fb) <= max_frag;
+    const bool a1 = a == 0u, fw = t == 0u;
+    bool left, ofw;
+    switch (policy) {
+    case NVB_PE_FF: left = a1 != fw; ofw = fw;  break;
+    case NVB_PE_RR: left = a1 == fw; ofw = fw;  break;
+    case NVB_PE_RF: left = fw;       ofw = !fw; break;
+    default:        left = !fw;      ofw = !fw; break;      // NVB_PE_FR
+    }
+    PeFrame f; f.left = left; f.strand = ofw ? 0u : 1u;
+    return f;
+}
+
+// Concordance of mate 1 (strand t1, [b1, e1)) and mate 2 (t2, [b2, e2)) under policy / flags: mate 2 lies on the strand the framing of
+// mate 1 gives it, and with L / R the left / right mate as framed, L starts and ends no later than R, the fragment [L.b, R.e) is
+// non-empty with a length in [min_frag, max_frag], and with NVB_PE_NO_OVERLAP L ends no later than R begins.  Framing from mate 2 gives
+// the same answer.  NVB_PE_FR with flags 0: the forward mate is L (nvb_seed_extend_paired's original FR test).
+__host__ __device__ __forceinline__ bool pe_concordant(uint32_t policy, uint32_t flags, uint32_t t1, uint32_t b1, uint32_t e1,
+                                                       uint32_t t2, uint32_t b2, uint32_t e2, uint32_t min_frag, uint32_t max_frag)
+{
+    const PeFrame f = pe_frame(policy, 0u, t1);
+    if (t2 != f.strand) return false;
+    const uint32_t lb = f.left ? b2 : b1, le = f.left ? e2 : e1, rb = f.left ? b1 : b2, re = f.left ? e1 : e2;
+    return lb <= rb && le <= re && re > lb && (re - lb) >= min_frag && (re - lb) <= max_frag && (!(flags & NVB_PE_NO_OVERLAP) || le <= rb);
+}
+
+// The opposite-mate window of anchor mate a aligned on strand t at [b, e): right of the anchor [b, min(b + max_frag, genome_len)),
+// starting at e with NVB_PE_NO_OVERLAP; left of it [max(e - max_frag, 0), e), ending at b with NVB_PE_NO_OVERLAP
+// (score_opposite_inl.h:177-193 without its min_frag trim).  Writes the window begin and length (0: empty) and returns the other mate's
+// strand.
+__host__ __device__ __forceinline__ uint32_t pe_rescue_window(uint32_t policy, uint32_t flags, uint32_t a, uint32_t t, uint32_t b, uint32_t e,
+                                                              uint32_t max_frag, uint32_t genome_len, uint32_t& wb, uint32_t& wl)
+{
+    const PeFrame f = pe_frame(policy, a, t);
+    const bool no_overlap = (flags & NVB_PE_NO_OVERLAP) != 0u;
+    uint32_t we;
+    if (f.left) { wb = e > max_frag ? e - max_frag : 0u; we = no_overlap ? b : e; }
+    else        { wb = no_overlap ? e : b; we = (genome_len - b) < max_frag ? genome_len : b + max_frag; }
+    wl = we > wb ? we - wb : 0u;
+    return f.strand;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -275,12 +321,17 @@ struct PairSecond {
         if (has && (s < score || (s == score && (i1 > tie[0] || (i1 == tie[0] && i2 >= tie[1]))))) return;
         has = true; score = s; end[0] = e1; strand[0] = t1; tie[0] = i1; end[1] = e2; strand[1] = t2; tie[1] = i2;
     }
-    // a rescue: anchor mate a's single-end best (end ae, strand at, tie index ai) with the other mate placed at end oe on the opposite
-    // strand (tie index 0xFFFFFFFF); s = the anchor's score + the rescue's
+    // a rescue: anchor mate a's single-end best (end ae, strand at, tie index ai) with the other mate placed at end oe on strand ot, the
+    // strand the policy frames it on (tie index 0xFFFFFFFF); s = the anchor's score + the rescue's
+    __host__ __device__ __forceinline__ void offer_rescue(int a, int32_t s, uint32_t ae, uint32_t at, uint32_t ai, uint32_t oe, uint32_t ot)
+    {
+        if (a == 0) offer(s, ae, at, ai, oe, ot, 0xFFFFFFFFu);
+        else        offer(s, oe, ot, 0xFFFFFFFFu, ae, at, ai);
+    }
+    // ... under NVB_PE_FR: the other mate on the anchor's opposite strand
     __host__ __device__ __forceinline__ void offer_rescue(int a, int32_t s, uint32_t ae, uint32_t at, uint32_t ai, uint32_t oe)
     {
-        if (a == 0) offer(s, ae, at, ai, oe, 1u - at, 0xFFFFFFFFu);
-        else        offer(s, oe, 1u - at, 0xFFFFFFFFu, ae, at, ai);
+        offer_rescue(a, s, ae, at, ai, oe, 1u - at);
     }
 };
 
@@ -294,25 +345,40 @@ __host__ __device__ __forceinline__ uint32_t lower_bound_end(const uint32_t* end
     return lo;
 }
 
-// offer every FR-concordant combination of one candidate of each mate: for each forward candidate of either mate, only the other mate's
-// reverse candidates ending in [begin + min_frag, begin + max_frag] are visited (binary search), so the work is bounded by the
-// concordant combinations and not by the product of the two lists
-__host__ __device__ inline void pair_combinations(const MateCands m[2], uint32_t min_frag, uint32_t max_frag, PairSecond& ps)
+// offer every concordant combination (pe_concordant) of one candidate of each mate.  Each candidate c of either mate is framed
+// (pe_frame); when the other mate would lie to its left, c is skipped (that pair is visited from the other member), otherwise only the
+// other mate's candidates on the framed strand ending in [c.begin + min_frag, c.begin + max_frag] are visited (binary search).  So every
+// concordant combination is offered exactly once, and the work is bounded by the concordant combinations, not by the product of the
+// two lists.  NVB_PE_FR: the forward candidates of either mate against the other mate's reverse ones.
+__host__ __device__ inline void pair_combinations(const MateCands m[2], uint32_t policy, uint32_t flags, uint32_t min_frag, uint32_t max_frag,
+                                                  PairSecond& ps)
 {
     for (int a = 0; a < 2; ++a) {
-        const MateCands& F = m[a]; const MateCands& R = m[1 - a];
-        for (uint32_t i = 0; i < F.n_fw; ++i) {
-            const uint32_t fe = F.end[i], fb = aln_begin(fe, F.len);
-            uint32_t k = lower_bound_end(R.end, R.n_fw, R.n, (uint64_t)fb + min_frag);
-            for (; k < R.n && (uint64_t)R.end[k] <= (uint64_t)fb + max_frag; ++k) {
-                const uint32_t re = R.end[k];
-                if (!fr_concordant(fb, fe, aln_begin(re, R.len), re, min_frag, max_frag)) continue;
-                const int32_t s = F.score[i] + R.score[k];
-                if (a == 0) ps.offer(s, fe, 0u, F.tie[i], re, 1u, R.tie[k]);
-                else        ps.offer(s, re, 1u, R.tie[k], fe, 0u, F.tie[i]);
+        const MateCands& A = m[a]; const MateCands& B = m[1 - a];
+        for (uint32_t t = 0; t < 2u; ++t) {
+            const PeFrame f = pe_frame(policy, (uint32_t)a, t);
+            if (f.left) continue;
+            const uint32_t i0 = t ? A.n_fw : 0u, i1 = t ? A.n : A.n_fw, k0 = f.strand ? B.n_fw : 0u, k1 = f.strand ? B.n : B.n_fw;
+            for (uint32_t i = i0; i < i1; ++i) {
+                const uint32_t ae = A.end[i], ab = aln_begin(ae, A.len);
+                uint32_t k = lower_bound_end(B.end, k0, k1, (uint64_t)ab + min_frag);
+                for (; k < k1 && (uint64_t)B.end[k] <= (uint64_t)ab + max_frag; ++k) {
+                    const uint32_t be = B.end[k], bb = aln_begin(be, B.len);
+                    const bool ok = a == 0 ? pe_concordant(policy, flags, t, ab, ae, f.strand, bb, be, min_frag, max_frag)
+                                           : pe_concordant(policy, flags, f.strand, bb, be, t, ab, ae, min_frag, max_frag);
+                    if (!ok) continue;
+                    const int32_t s = A.score[i] + B.score[k];
+                    if (a == 0) ps.offer(s, ae, t, A.tie[i], be, f.strand, B.tie[k]);
+                    else        ps.offer(s, be, f.strand, B.tie[k], ae, t, A.tie[i]);
+                }
             }
         }
     }
+}
+// ... under NVB_PE_FR with flags 0
+__host__ __device__ inline void pair_combinations(const MateCands m[2], uint32_t min_frag, uint32_t max_frag, PairSecond& ps)
+{
+    pair_combinations(m, NVB_PE_FR, 0u, min_frag, max_frag, ps);
 }
 
 // Mapping quality of an unpaired read: nvBowtie's BowtieMapq2 (mapq.h:155-327) for a scheme with perfect_score(len) = perfect,

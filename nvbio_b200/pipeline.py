@@ -400,21 +400,44 @@ def seed_extend_all(fmi: FMIndexDevice, genome: torch.Tensor, reads: PackedStrin
     return workspace.run(fmi, genome, reads, params)
 
 
-PAIR_UNPAIRED, PAIR_CONCORDANT, PAIR_RESCUED_MATE1, PAIR_RESCUED_MATE2 = 0, 1, 2, 4
+PAIR_UNPAIRED, PAIR_CONCORDANT, PAIR_RESCUED_MATE1, PAIR_RESCUED_MATE2, PAIR_DISCORDANT = 0, 1, 2, 4, 8
+# nvb_pair_params.policy (NVB_PE_*) and flags
+PE_POLICIES = ("fr", "rf", "ff", "rr")
+PE_NO_OVERLAP, PE_DISCORDANT, PE_NO_MIXED = 1, 2, 4
 
 
 @dataclass
 class PairParams:
-    """fragment constraints of the paired-end stage (nvBowtie --minins / --maxins, FR orientation)"""
+    """fragment constraints and pairing options of the paired-end stage (nvBowtie --minins / --maxins, --fr / --rf / --ff / --rr,
+    --no-overlap, --no-mixed and discordant pairs; include/nvbio_b200.h nvb_pair_params).  policy: the mates' orientation; overlap=False:
+    a concordant pair's mates may not overlap and the rescue looks only past the anchor; discordant=True (needs mapq): an unpaired pair
+    whose two mates align uniquely is reported as PAIR_DISCORDANT; mixed=False: the mates of a pair that is still unpaired are reported
+    unaligned.  The defaults are the FR pairing with overlap, no discordant pairs and unpaired mates reported."""
     min_frag: int = 0
     max_frag: int = 500
     min_mate_score: int = 60          # a mate's alignment (anchor or rescued) must reach this score to take part in a pair
     rescue_capacity: Optional[int] = None
+    policy: str = "fr"
+    overlap: bool = True
+    discordant: bool = False
+    mixed: bool = True
+
+    @property
+    def policy_code(self) -> int:
+        """NVB_PE_FR 0, NVB_PE_RF 1, NVB_PE_FF 2, NVB_PE_RR 3"""
+        if self.policy not in PE_POLICIES:
+            raise ValueError("PairParams.policy must be one of %s, not %r" % (PE_POLICIES, self.policy))
+        return PE_POLICIES.index(self.policy)
+
+    @property
+    def flags(self) -> int:
+        return (0 if self.overlap else PE_NO_OVERLAP) | (PE_DISCORDANT if self.discordant else 0) | (0 if self.mixed else PE_NO_MIXED)
 
     def struct(self, n_pairs) -> PairParamsStruct:
         p = PairParamsStruct()
         p.min_frag, p.max_frag, p.min_mate_score = self.min_frag, self.max_frag, self.min_mate_score
         p.rescue_capacity = 2 * n_pairs if self.rescue_capacity is None else self.rescue_capacity
+        p.policy, p.flags = self.policy_code, self.flags
         return p
 
 

@@ -98,12 +98,23 @@ def sample_reads(genome_words, n, n_reads, read_len, sub_rate=0.01, indel_rate=0
     return torch.cat(out), torch.cat(poss), torch.cat(strands)
 
 
+# (mate 1, mate 2) of a fragment sequenced in each orientation, from its left (L) and right (R) read_len bases, forward (fw) or reverse
+# complemented (rv): (even pairs, odd pairs); an odd pair reads the fragment off the reverse strand (L <-> R, strands flipped)
+_ORIENT = {"fr": (("fwL", "rvR"), ("rvR", "fwL")), "rf": (("rvL", "fwR"), ("fwR", "rvL")),
+           "ff": (("fwL", "fwR"), ("rvR", "rvL")), "rr": (("fwR", "fwL"), ("rvL", "rvR"))}
+
+
 def sample_pairs(genome_words, n, n_pairs, read_len, frag_mean=350.0, frag_sd=30.0, sub_rate=0.01, hard_frac=0.05, hard_sub_rate=0.2,
-                 device="cuda", seed=SEED_QUERIES ^ 0x7777, mut_seed=SEED_MUT ^ 0x7777, chunk=1 << 18):
-    """C5-shaped pairs, FR orientation: a fragment [p, p + frag) of the genome, one mate = its first read_len bases (forward), the
-    other = the reverse complement of its last read_len bases; odd pairs swap which mate is which.  A fraction `hard_frac` of the
-    second mates carries `hard_sub_rate` substitutions (mostly no exact seed survives: the opposite-mate rescue has to place them).
-    Returns (words [2*n_pairs, ceil(read_len/16)] int32 -- mate 1 of every pair, then mate 2 --, left int64[n_pairs], frag int64[n_pairs])"""
+                 device="cuda", seed=SEED_QUERIES ^ 0x7777, mut_seed=SEED_MUT ^ 0x7777, chunk=1 << 18, orientation="fr"):
+    """C5-shaped pairs of a fragment [p, p + frag) of the genome with L = its first read_len bases and R = its last read_len bases.
+    orientation "fr" (the default): one mate = L forward, the other = the reverse complement of R; "rf": L reverse complemented, R
+    forward; "ff": mate 1 = L, mate 2 = R, both forward; "rr": mate 1 = R, mate 2 = L, both forward.  Odd pairs read the fragment off
+    the reverse strand (FR: which mate is which swaps).  A fraction `hard_frac` of the second mates carries `hard_sub_rate`
+    substitutions (mostly no exact seed survives: the opposite-mate rescue has to place them).  The random draws do not depend on the
+    orientation.  Returns (words [2*n_pairs, ceil(read_len/16)] int32 -- mate 1 of every pair, then mate 2 --, left int64[n_pairs],
+    frag int64[n_pairs])"""
+    if orientation not in _ORIENT:
+        raise ValueError("sample_pairs: orientation must be one of %s, not %r" % (tuple(_ORIENT), orientation))
     g, gm = _gen(seed, device), _gen(mut_seed, device)
     m1, m2, lefts, frags = [], [], [], []
     ar = torch.arange(read_len, device=device, dtype=torch.int64)[None, :]
@@ -111,11 +122,13 @@ def sample_pairs(genome_words, n, n_pairs, read_len, frag_mean=350.0, frag_sd=30
         m = min(chunk, n_pairs - s)
         frag = (frag_mean + frag_sd * torch.randn(m, device=device, generator=g)).round().to(torch.int64).clamp_(read_len, int(frag_mean + 4 * frag_sd))
         left = torch.randint(0, n - int(frag_mean + 4 * frag_sd) - 64, (m,), device=device, generator=g, dtype=torch.int64)
-        fw = gather_symbols(genome_words, left[:, None] + ar)
-        rv = (3 - gather_symbols(genome_words, (left + frag - read_len)[:, None] + ar)).flip(1)
+        fwl = gather_symbols(genome_words, left[:, None] + ar)
+        fwr = gather_symbols(genome_words, (left + frag - read_len)[:, None] + ar)
+        seg = dict(fwL=fwl, rvR=(3 - fwr).flip(1), fwR=fwr, rvL=(3 - fwl).flip(1))
+        (ea, eb), (oa, ob) = _ORIENT[orientation]
         swap = (torch.arange(s, s + m, device=device) & 1).bool()
-        a = torch.where(swap[:, None], rv, fw)
-        b = torch.where(swap[:, None], fw, rv)
+        a = torch.where(swap[:, None], seg[oa], seg[ea])
+        b = torch.where(swap[:, None], seg[ob], seg[eb])
         hard = torch.rand(m, device=device, generator=gm) < hard_frac
         for k, sym in enumerate((a, b)):
             rate = torch.full((m, 1), sub_rate, device=device)
