@@ -70,7 +70,7 @@ def record(inp, k, me, mate, pflag):
     if paired:
         mm = mate[0] == 1
         flag |= 0x1 | (0x80 if k & 1 else 0x40)
-        if pflag != 0 and mapped and mm:
+        if pflag in (1, 2, 4) and mapped and mm:                 # concordant or rescued; a discordant pair (8) is not proper
             flag |= 0x2
         if not mm:
             flag |= 0x8
