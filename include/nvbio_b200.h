@@ -1085,9 +1085,79 @@ int  nvb_pipeline_create(const nvb_fm_index* fmi, const uint32_t* d_genome, cons
                          uint32_t hit_capacity, uint32_t depth, nvb_pipeline** out);
 int  nvb_pipeline_submit(nvb_pipeline* p, const uint32_t* h_read_words, uint32_t* ticket);
 int  nvb_pipeline_wait(nvb_pipeline* p, uint32_t ticket, nvb_pipeline_result* out);
-/* bytes moved per batch: host -> device, device -> host */
+/* bytes moved per batch: host -> device, device -> host (a BAM pipeline: the largest input of a batch, and the fixed part of its results;
+   the payload adds its own byte count) */
 void nvb_pipeline_traffic(const nvb_pipeline* p, size_t* h2d_bytes, size_t* d2h_bytes);
 void nvb_pipeline_destroy(nvb_pipeline* p);
+
+/* BAM mode of the pipeline: host reads, qualities and names in, the batch's BAM payload out (nvBowtie's input thread -> compute thread ->
+ * output writer, compute_thread.cu:213-243, output_bam.cpp:581-601).  Same slots, streams, events, depth and NVB_PIPELINE_COMPUTE_STREAMS
+ * rules as above; one batch runs on its slot's compute stream, each call with its own rules unchanged:
+ *   single end: nvb_seed_extend_mapq with best_alignment -> nvb_finish_alignments -> nvb_bam_records, one name per read;
+ *   paired:     nvb_seed_extend_paired_traceback with mapq (every policy and flag, NVB_PE_DISCORDANT included) -> nvb_finish_alignments
+ *               over the 2n mates with d_strand = d_mate_strand -> nvb_bam_records with d_pair_flags, one name per pair;
+ *   then, with compress, the BGZF members of exactly the d_offsets[n] record bytes (nvb_bgzf_compress's output for them, with the byte
+ *   count read on the device: no host round trip inside a batch).
+ * Genome length for finish: fmi->length.  MAPQ and XS of the records come from the mapping call; qualities go to the mapping call
+ * (params.d_read_quals) and to the records.
+ *
+ * submit: n_reads (1 .. max_reads; even when paired: mate 1 of every pair, then mate 2, so a short last batch is fine) reads of
+ * words_per_read words; h_quals (has_quals): one byte per read symbol, n_reads * words_per_read * (32 / read_bits) bytes in the layout of
+ * the symbols; h_lengths (has_lengths): per-read lengths 1 .. read_len, else every read is read_len long; names: h_names bytes and
+ * h_name_offsets[n_names + 1] (n_names = n_reads, or n_reads / 2 when paired), offsets from 0, each name 1 or more bytes (names longer
+ * than 254 bytes are cut, as nvb_bam_records does), the last offset <= max_name_bytes.  As in nvb_pipeline_submit, host buffers must
+ * stay valid until wait returns for that ticket (pinned memory makes the copies asynchronous).
+ * wait: nvb_pipeline_bam_result, pointers into the slot's pinned host memory, valid until `depth` further submits.  The counts leave the
+ * device with the batch; the payload is then copied with exactly its byte count (by wait, or by the submit that reuses a slot whose
+ * batch was never waited for).  The host payload buffer of a slot grows (cudaHostAlloc) to the largest payload it has held.
+ * payload: with compress, BGZF members that a BAM writer emits verbatim between the header and the EOF block; without, the record stream.
+ *
+ * Slot memory: one device allocation per slot (nvb_pipeline_slot_bytes).  Buffers whose lifetimes do not overlap share bytes: the
+ * mapping call's temp (direction matrices included) is dead once finish starts, the traceback ops once the records are built, the finish
+ * outputs once the records exist, the records once BGZF's first kernel has read them (its members are written over them).  With n =
+ * max_reads, L = read_len: O = n * max_ops (ops), T = the mapping call's temp, F = n * (4 * max_cigar + max_md + 28) (finish outputs),
+ * B = the records' temp, R = n * (36 + 1 + 4 * max_cigar + (L + 1) / 2 + L + 46 + max_md) + max_name_bytes (twice when paired) (the
+ * record bound), Zo = 65,311 * ceil(R / 0xFF00) (members), Zt = the BGZF temp (about R, + 17 MB on an H100): the stage region takes
+ * max(O + T, max(O, R) + F + B, max(R, Zo) + Zt) bytes with compress and max(O + T, max(O, R) + F + B) without, beside O(n) bytes of
+ * inputs and per-read outputs.  From shapes, not measured: 1 M mates of 150 bp, band 31, default sizes: O 0.33 GB, F 2.4 GB, R 2.6 GB.
+ *
+ * NVB_E_INVALID before any CUDA call: the checks of nvb_pipeline_create (bar its refusal of NVB_PE_DISCORDANT); bam, mapq, d_min_score
+ * or d_contig_begin NULL, n_contigs == 0, max_name_bytes == 0; params->d_read_quals != NULL (qualities come per batch); a quality table
+ * without has_quals; mapq->max_read_len < read_len.  In submit: n_reads == 0 or > max_reads, odd when paired; a NULL array the flags
+ * require (words, names, offsets, ticket; quals with has_quals; lengths with has_lengths); name offsets that do not start at 0, do not
+ * increase, or end past max_name_bytes; a length of 0 or above read_len.  submit / wait of the other kind of pipeline.
+ * NVB_E_UNSUPPORTED for read_len > 512 (the traceback calls' limit). */
+typedef struct nvb_pipeline_bam_params {
+    const nvb_mapq_params* mapq;          /* required: d_min_score, max_read_len >= read_len, match_bonus */
+    const uint32_t* d_contig_begin;       /* [n_contigs + 1], as nvb_bam_in */
+    uint32_t        n_contigs;
+    uint32_t        max_name_bytes;       /* bytes of names per batch */
+    uint32_t        has_quals;            /* 1: every submit passes qualities */
+    uint32_t        has_lengths;          /* 1: every submit passes per-read lengths (<= read_len) */
+    uint32_t        compress;             /* 1: BGZF members; 0: the raw record stream */
+    uint32_t        max_ops, max_cigar, max_md;   /* 0 = never truncate: 2 * read_len + band_len, max_ops + 2, 3 * max_ops + 1 */
+} nvb_pipeline_bam_params;
+typedef struct nvb_pipeline_bam_result {
+    const uint8_t*  payload;         /* BGZF members (compress) or BAM records */
+    uint64_t        payload_bytes;
+    uint64_t        record_bytes;    /* bytes of the records (= payload_bytes without compress) */
+    uint32_t        n_records;       /* 2 per pair when paired */
+    uint32_t        n_blocks;        /* BGZF members (0 without compress) */
+    const uint32_t* counts;          /* [4] nvb_bam_records' tallies: records, mapped, unmapped by the contig rule, unfinished */
+    const uint32_t* n_hits;          /* [3] hits kept, found, distinct alignment jobs */
+    const uint32_t* n_rescue;        /* [2] paired (NULL when single end): full-DP jobs run, wanted */
+    float           device_ms;       /* device time of this batch's kernels (its compute stream) */
+} nvb_pipeline_bam_result;
+
+int  nvb_pipeline_create_bam(const nvb_fm_index* fmi, const uint32_t* d_genome, const nvb_seed_extend_params* params,
+                             const nvb_pair_params* pair_params /* NULL = single end */, const nvb_pipeline_bam_params* bam,
+                             uint32_t max_reads, uint32_t read_len, uint32_t words_per_read, uint32_t read_bits,
+                             uint32_t hit_capacity, uint32_t depth, nvb_pipeline** out);
+int  nvb_pipeline_submit_bam(nvb_pipeline* p, uint32_t n_reads, const uint32_t* h_read_words, const uint8_t* h_quals,
+                             const uint32_t* h_lengths, const char* h_names, const uint32_t* h_name_offsets, uint32_t* ticket);
+int  nvb_pipeline_wait_bam(nvb_pipeline* p, uint32_t ticket, nvb_pipeline_bam_result* out);
+/* bytes of device memory one slot of a BAM pipeline holds (its single allocation) */
+size_t nvb_pipeline_slot_bytes(const nvb_pipeline* p);
 
 /* Profiling aid (the reference wraps every stage in cuda::Timer, nvBowtie/bowtie2/cuda/aligner_best_approx.h:
  * 219-241): device time in ms of the seven stages of the most recent nvb_seed_extend call -- [fw,rc] strings,

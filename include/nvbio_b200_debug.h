@@ -4,6 +4,7 @@
 #ifndef NVBIO_B200_DEBUG_H
 #define NVBIO_B200_DEBUG_H
 #include <stdint.h>
+#include "nvbio_b200.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -63,6 +64,20 @@ int nvb_debug_mapq_eval(const int32_t* d_best, const uint8_t* d_has_second, cons
 
 /* nvb_bgzf_compress: CTAs of the resident compression grid, 0 (default) = one per SM.  Same output at every grid size; for tests */
 void nvb_debug_bgzf_grid(uint32_t ctas);
+/* nvb_bgzf_compress with its byte count in device memory, as the BAM mode of nvb_pipeline runs it: *d_n_bytes bytes at d_in (at most
+   max_bytes; a larger value is taken as max_bytes).  max_bytes sizes the grids, the temp (the NVB_E_TEMP_SIZE answer) and the offsets:
+   out->d_block_offsets has ceil(max_bytes / 0xFF00) + 1 entries, [0, n_blocks] as nvb_bgzf_compress writes them for the real count and
+   the total repeated in every entry after n_blocks.  Members, offsets and capacity rules are otherwise those of nvb_bgzf_compress, byte
+   for byte.  NVB_E_INVALID for a NULL d_n_bytes and nvb_bgzf_compress's checks on max_bytes.  For tests */
+int nvb_debug_bgzf_compress_device_count(const uint8_t* d_in, const uint64_t* d_n_bytes, uint64_t max_bytes, const nvb_bgzf_out* out,
+                                         void* d_temp, size_t* temp_bytes, void* stream);
+
+/* the host-side checks nvb_pipeline_submit_bam makes before any CUDA call, for a pipeline made with `bam`, pair_params != NULL when
+   paired != 0, max_reads and read_len: NVB_OK when a submit with these arguments passes them, else NVB_E_INVALID.  Needs no device;
+   for tests of the rules without a pipeline */
+int nvb_debug_pipeline_bam_submit_check(const nvb_pipeline_bam_params* bam, uint32_t paired, uint32_t max_reads, uint32_t read_len,
+                                        uint32_t n_reads, const uint32_t* h_read_words, const uint8_t* h_quals, const uint32_t* h_lengths,
+                                        const char* h_names, const uint32_t* h_name_offsets);
 
 #ifdef __cplusplus
 }

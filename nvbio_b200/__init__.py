@@ -8,10 +8,10 @@ from .fmindex import (FMIndexDevice, FMIndexFilterDevice, rank, rank4, match, ma
                       MAP_EXACT, MAP_APPROX, dict_rank, dict_build_occ,
                       MATCH_FORWARD_ORDER, MATCH_COMPLEMENT)
 from . import aln                                                                # noqa: F401
-from .pipeline import SeedExtendParams, seed_extend, StreamingSeedExtend, PairParams, seed_extend_paired, MapqParams, seed_extend_all, AllAlignments, ReseedParams, seed_extend_reseed, seed_extend_paired_reseed     # noqa: F401
+from .pipeline import SeedExtendParams, seed_extend, StreamingSeedExtend, StreamingBam, PairParams, seed_extend_paired, MapqParams, seed_extend_all, AllAlignments, ReseedParams, seed_extend_reseed, seed_extend_paired_reseed     # noqa: F401
 from .pipeline import PAIR_UNPAIRED, PAIR_CONCORDANT, PAIR_RESCUED_MATE1, PAIR_RESCUED_MATE2, PAIR_DISCORDANT    # noqa: F401
 from .finish import finish_alignments, FinishedAlignments                        # noqa: F401
-from .bam import ContigTable, BamRecords, bam_records, bam_records_all, bam_header, write_bam, numbered_names    # noqa: F401
+from .bam import ContigTable, BamRecords, bam_records, bam_records_all, bam_header, write_bam, numbered_names, BamBatch, pack_names    # noqa: F401
 from .bgzf import BgzfBlocks, BgzfCall, bgzf_compress                           # noqa: F401
 from .bam_sort import SortedBamRecords, sort_bam_records, bam_index, write_sorted_bam    # noqa: F401
 from .sam import SamText, SamCall, sam_header, sam_text, write_sam                  # noqa: F401

@@ -15,6 +15,7 @@ EXPORTS = [
     "nvb_dict_rank", "nvb_dict_rank4", "nvb_dict_build_occ",
     "nvb_map_seeds", "nvb_fm_locate_init", "nvb_fm_locate_lookup", "nvb_fm_locate_sorted",
     "nvb_pipeline_create", "nvb_pipeline_submit", "nvb_pipeline_wait", "nvb_pipeline_traffic", "nvb_pipeline_destroy",
+    "nvb_pipeline_create_bam", "nvb_pipeline_submit_bam", "nvb_pipeline_wait_bam", "nvb_pipeline_slot_bytes",
     "nvb_finish_alignments", "nvb_bam_records", "nvb_bam_records_all", "nvb_bgzf_compress", "nvb_bam_sort", "nvb_bam_index", "nvb_sam_format",
 ]
 # test / tuning hooks of include/nvbio_b200_debug.h (not part of the drop-in ABI)
@@ -22,7 +23,7 @@ DEBUG_EXPORTS = [
     "nvb_debug_gotoh_last_route", "nvb_debug_force_gotoh_path", "nvb_debug_full_minb", "nvb_debug_full_warp", "nvb_debug_full_traceback_warp",
     "nvb_debug_pair_format", "nvb_debug_pair_rows2", "nvb_debug_traceback_fast", "nvb_debug_pair_extra_smem",
     "nvb_debug_pipeline_path", "nvb_debug_seed_split", "nvb_debug_seed_todo", "nvb_debug_perfect_shortcut", "nvb_debug_dp_jobs", "nvb_debug_mapq_eval",
-    "nvb_debug_bgzf_grid",
+    "nvb_debug_bgzf_grid", "nvb_debug_bgzf_compress_device_count", "nvb_debug_pipeline_bam_submit_check",
 ]
 
 
@@ -141,6 +142,17 @@ class PipelineResultStruct(C.Structure):    # nvb_pipeline_result
                 ("n_rescue", C.c_void_p), ("device_ms", C.c_float)]
 
 
+class PipelineBamParamsStruct(C.Structure):  # nvb_pipeline_bam_params
+    _fields_ = [("mapq", C.c_void_p), ("d_contig_begin", C.c_void_p), ("n_contigs", C.c_uint32), ("max_name_bytes", C.c_uint32),
+                ("has_quals", C.c_uint32), ("has_lengths", C.c_uint32), ("compress", C.c_uint32), ("max_ops", C.c_uint32),
+                ("max_cigar", C.c_uint32), ("max_md", C.c_uint32)]
+
+
+class PipelineBamResultStruct(C.Structure):  # nvb_pipeline_bam_result
+    _fields_ = [("payload", C.c_void_p), ("payload_bytes", C.c_uint64), ("record_bytes", C.c_uint64), ("n_records", C.c_uint32),
+                ("n_blocks", C.c_uint32), ("counts", C.c_void_p), ("n_hits", C.c_void_p), ("n_rescue", C.c_void_p), ("device_ms", C.c_float)]
+
+
 _lib = None
 
 
@@ -154,6 +166,7 @@ def lib():
         _lib.nvb_error_string.restype = C.c_char_p
         _lib.nvb_pipeline_destroy.restype = None
         _lib.nvb_pipeline_traffic.restype = None
+        _lib.nvb_pipeline_slot_bytes.restype = C.c_size_t
         for name in EXPORTS + DEBUG_EXPORTS:
             getattr(_lib, name)            # raises AttributeError if a symbol is not exported
     return _lib

@@ -242,6 +242,35 @@ def bam_records_all(al, finished: FinishedAlignments, reads: PackedStringSet, co
     return BamRecords(data=data[:int(capacity)], offsets=offsets[:n_rec + 1], counts=counts)
 
 
+def pack_names(names: Sequence):
+    """(bytes, offsets) of read names on the host, as nvb_pipeline_submit_bam takes them: a uint8 numpy array and uint32 offsets [n + 1]
+    (name j = bytes[offsets[j]:offsets[j + 1]]).  Names are str or bytes of 1 or more bytes; nvb_bam_records cuts them at 254."""
+    raw = [nm.encode() if isinstance(nm, str) else bytes(nm) for nm in names]
+    off = np.zeros(len(raw) + 1, np.uint32)
+    off[1:] = np.cumsum([len(nm) for nm in raw])
+    return np.frombuffer(b"".join(raw) + b"\0", np.uint8), off
+
+
+@dataclass
+class BamBatch:
+    """One batch of StreamingBam (nvb_pipeline_wait_bam): payload, a uint8 view of the pipeline's pinned host memory (valid until `depth`
+    further submits) holding BGZF members when compressed, else the BAM records; n_records; counts = nvb_bam_records' tallies (records,
+    mapped, unmapped by the contig rule, unfinished); n_hits = (kept, found, distinct jobs); n_rescue = (run, wanted) when paired, else None;
+    record_bytes and n_blocks (BGZF members, 0 when not compressed); device_ms of the batch's kernels."""
+    payload: torch.Tensor
+    compressed: bool
+    n_records: int
+    counts: tuple
+    n_hits: tuple
+    n_rescue: Optional[tuple]
+    record_bytes: int
+    n_blocks: int
+    device_ms: float
+
+    def to_bytes(self) -> bytes:
+        return self.payload.numpy().tobytes()
+
+
 def bam_header(contigs: ContigTable, program: str = "nvbio_b200", sort_order: str = "unsorted") -> bytes:
     """BAM header bytes: magic, the SAM header text (@HD with SO:sort_order, one @SQ per contig, @PG) and the reference list"""
     from .sam import sam_header
@@ -273,8 +302,9 @@ def _bgzf_block(data: bytes) -> bytes:
 
 def write_bam(path: str, header: bytes, batches: Iterable) -> int:
     """write a .bam file: header (bam_header) then the records of every batch (BamRecords, or bytes), BGZF-framed on the host with zlib
-    (blocks of at most 64 KiB, then the 28-byte EOF block).  A BgzfBlocks batch (bgzf_compress on the device) is written verbatim.  Raises
-    if a batch did not store all its records or members.  Returns the bytes written."""
+    (blocks of at most 64 KiB, then the 28-byte EOF block).  A BgzfBlocks batch (bgzf_compress on the device) is written verbatim, and so
+    is a compressed BamBatch (StreamingBam); an uncompressed BamBatch is framed like BamRecords.  Raises if a batch did not store all its
+    records or members.  Returns the bytes written."""
     from .bgzf import BgzfBlocks
     total = 0
     with open(path, "wb") as f:
@@ -291,6 +321,12 @@ def write_bam(path: str, header: bytes, batches: Iterable) -> int:
                 z = b.to_bytes()
                 f.write(z); total += len(z)
                 continue
+            if isinstance(b, BamBatch):
+                if b.compressed:
+                    z = b.to_bytes()
+                    f.write(z); total += len(z)
+                    continue
+                b = b.to_bytes()
             if isinstance(b, BamRecords):
                 if b.stored() != b.offsets.numel() - 1:
                     raise ValueError("write_bam: a batch stored %d of %d records (capacity too small)" % (b.stored(), b.offsets.numel() - 1))

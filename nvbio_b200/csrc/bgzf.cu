@@ -11,6 +11,10 @@
 //                         temp of its own, so the size query needs no device);
 //   bgzf_copy_kernel      each member from its slot to d_out through a shared-memory span laid out like the output modulo 16, stored
 //                         with aligned 16-byte stores (bytes only at the head and tail), as bam_write_kernel does.
+// The byte count is a host value (nvb_bgzf_compress) or lives in device memory beside a host upper bound (bgzf_compress_device_count,
+// which the BAM pipeline runs on nvb_bam_records' total so that no batch waits for it on the host).  The bound sizes the grids and the
+// temp; each kernel reads the real count itself (bgzf_count): the resident grid strides over the blocks that exist, the scan repeats the
+// total past them, the copy stops at them.  With a host count both are the same number, so there is one code path.
 #include <cub/cub.cuh>
 #include "bgzf_core.cuh"
 
@@ -44,6 +48,13 @@ struct BgzfSmem {
 };
 static_assert(sizeof(BgzfSmem) <= 227u * 1024u, "one CTA per SM: an H100 CTA gets at most 227 KB of shared memory");
 
+// the byte count: the device value when there is one (never above the host bound), else the host value
+__device__ __forceinline__ uint64_t bgzf_count(const uint64_t n_bytes, const uint64_t* __restrict__ d_n_bytes)
+{
+    return d_n_bytes ? min(*d_n_bytes, n_bytes) : n_bytes;
+}
+__device__ __forceinline__ uint32_t bgzf_blocks(const uint64_t n) { return (uint32_t)(n / BGZF_BLOCK + (n % BGZF_BLOCK != 0u)); }
+
 // the parse walk of segment [s0, s1) from entry g: marks its token starts and returns the first position at or past s1
 __device__ __forceinline__ uint32_t bgzf_walk(BgzfSmem& S, const BgzfParse& v, uint32_t s0, uint32_t s1, uint32_t g)
 {
@@ -56,9 +67,11 @@ __device__ __forceinline__ uint32_t bgzf_walk(BgzfSmem& S, const BgzfParse& v, u
 }
 
 __global__ void __launch_bounds__(BGZF_THREADS, 1)
-bgzf_compress_kernel(const uint8_t* __restrict__ d_in, const uint64_t n_bytes, const uint32_t n_blocks, uint8_t* __restrict__ slots,
+bgzf_compress_kernel(const uint8_t* __restrict__ d_in, const uint64_t n_bound, const uint64_t* __restrict__ d_n_bytes, uint8_t* __restrict__ slots,
                      uint16_t* __restrict__ dist_scratch, uint64_t* __restrict__ sizes)
 {
+    const uint64_t n_bytes = bgzf_count(n_bound, d_n_bytes);
+    const uint32_t n_blocks = bgzf_blocks(n_bytes);
     extern __shared__ __align__(16) uint8_t smem_raw[];
     BgzfSmem& S = *reinterpret_cast<BgzfSmem*>(smem_raw);
     const uint32_t t = threadIdx.x, lane = t & 31u;
@@ -190,16 +203,17 @@ bgzf_compress_kernel(const uint8_t* __restrict__ d_in, const uint64_t n_bytes, c
 }
 
 __global__ void __launch_bounds__(BGZF_SCAN_THREADS)
-bgzf_scan_kernel(const uint64_t* __restrict__ sizes, const uint32_t n_blocks, uint64_t* __restrict__ offsets)
+bgzf_scan_kernel(const uint64_t* __restrict__ sizes, const uint64_t n_bound, const uint64_t* __restrict__ d_n_bytes, uint64_t* __restrict__ offsets)
 {
     typedef cub::BlockScan<uint64_t, BGZF_SCAN_THREADS> Scan;
     __shared__ typename Scan::TempStorage ts;
+    const uint32_t n_blocks = bgzf_blocks(bgzf_count(n_bound, d_n_bytes)), n_out = bgzf_blocks(n_bound);
     uint64_t carry = 0u;
-    for (uint64_t b = 0; b <= n_blocks; b += BGZF_SCAN_THREADS) {                  // n_blocks + 1 outputs: [n_blocks] is the total
+    for (uint64_t b = 0; b <= n_out; b += BGZF_SCAN_THREADS) {     // n_out + 1 outputs: [n_blocks] is the total, repeated after it
         const uint64_t i = b + threadIdx.x;
         uint64_t y, sum;
         Scan(ts).ExclusiveSum(i < n_blocks ? sizes[i] : 0u, y, sum);
-        if (i <= n_blocks) offsets[i] = carry + y;
+        if (i <= n_out) offsets[i] = carry + y;
         carry += sum;
         __syncthreads();
     }
@@ -207,11 +221,12 @@ bgzf_scan_kernel(const uint64_t* __restrict__ sizes, const uint32_t n_blocks, ui
 
 // members whose end fits the capacity, from their slots to d_out
 __global__ void __launch_bounds__(BGZF_COPY_THREADS)
-bgzf_copy_kernel(const uint8_t* __restrict__ slots, const uint64_t* __restrict__ offsets, const uint32_t n_blocks, uint8_t* __restrict__ out,
-                 const uint64_t capacity)
+bgzf_copy_kernel(const uint8_t* __restrict__ slots, const uint64_t* __restrict__ offsets, const uint64_t n_bound, const uint64_t* __restrict__ d_n_bytes,
+                 uint8_t* __restrict__ out, const uint64_t capacity)
 {
     extern __shared__ __align__(16) uint8_t stage[];                   // BGZF_SLOT + 16 bytes
     const uint32_t t = threadIdx.x;
+    const uint32_t n_blocks = bgzf_blocks(bgzf_count(n_bound, d_n_bytes));
     for (uint32_t blk = blockIdx.x; blk < n_blocks; blk += gridDim.x) {
         const uint64_t lo = offsets[blk], hi = offsets[blk + 1u];
         if (hi > capacity) return;                                     // so are all later members
@@ -237,13 +252,8 @@ bgzf_copy_kernel(const uint8_t* __restrict__ slots, const uint64_t* __restrict__
 
 static uint32_t g_bgzf_grid = 0u;                                      // nvb_debug_bgzf_grid: 0 = one CTA per SM
 
-} // namespace nvb
-
-using namespace nvb;
-
-extern "C" void nvb_debug_bgzf_grid(uint32_t ctas) { g_bgzf_grid = ctas; }
-
-extern "C" int nvb_bgzf_compress(const uint8_t* d_in, uint64_t n_bytes, const nvb_bgzf_out* out, void* d_temp, size_t* temp_bytes, void* stream)
+int bgzf_compress_device_count(const uint8_t* d_in, uint64_t n_bytes, const uint64_t* d_n_bytes, const nvb_bgzf_out* out, void* d_temp,
+                               size_t* temp_bytes, void* stream)
 {
     if (!out || !temp_bytes || (!d_in && n_bytes) || !out->d_block_offsets || (!out->d_out && out->capacity)) return NVB_E_INVALID;
     const uint64_t nb = n_bytes / BGZF_BLOCK + (n_bytes % BGZF_BLOCK != 0u);
@@ -254,7 +264,6 @@ extern "C" int nvb_bgzf_compress(const uint8_t* d_in, uint64_t n_bytes, const nv
         NVB_CUDA_TRY(cudaMemsetAsync(out->d_block_offsets, 0, sizeof(uint64_t), s));
         return NVB_OK;
     }
-    const uint32_t n_blocks = (uint32_t)nb;
     const uint32_t grid = (uint32_t)std::min<uint64_t>(nb, g_bgzf_grid ? g_bgzf_grid : sm_count());
     TempCarver tc(nullptr);
     tc.take<uint8_t>(nb * BGZF_SLOT); tc.take<uint64_t>(nb); tc.take<uint16_t>((size_t)grid * BGZF_BLOCK);
@@ -268,12 +277,30 @@ extern "C" int nvb_bgzf_compress(const uint8_t* d_in, uint64_t n_bytes, const nv
     const int smem = (int)sizeof(BgzfSmem), copy_smem = (int)(BGZF_SLOT + 16u);
     NVB_CUDA_TRY(cudaFuncSetAttribute(bgzf_compress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     NVB_CUDA_TRY(cudaFuncSetAttribute(bgzf_copy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, copy_smem));
-    bgzf_compress_kernel<<<grid, BGZF_THREADS, smem, s>>>(d_in, n_bytes, n_blocks, slots, dist, sizes);
+    bgzf_compress_kernel<<<grid, BGZF_THREADS, smem, s>>>(d_in, n_bytes, d_n_bytes, slots, dist, sizes);
     NVB_LAUNCH_CHECK();
-    bgzf_scan_kernel<<<1, BGZF_SCAN_THREADS, 0, s>>>(sizes, n_blocks, out->d_block_offsets);
+    bgzf_scan_kernel<<<1, BGZF_SCAN_THREADS, 0, s>>>(sizes, n_bytes, d_n_bytes, out->d_block_offsets);
     NVB_LAUNCH_CHECK();
     if (out->capacity == 0u) return NVB_OK;
     const uint32_t copy_grid = (uint32_t)std::min<uint64_t>(nb, 4u * (uint64_t)sm_count());
-    bgzf_copy_kernel<<<copy_grid, BGZF_COPY_THREADS, copy_smem, s>>>(slots, out->d_block_offsets, n_blocks, out->d_out, out->capacity);
+    bgzf_copy_kernel<<<copy_grid, BGZF_COPY_THREADS, copy_smem, s>>>(slots, out->d_block_offsets, n_bytes, d_n_bytes, out->d_out, out->capacity);
     return (int)cudaGetLastError();
+}
+
+} // namespace nvb
+
+using namespace nvb;
+
+extern "C" void nvb_debug_bgzf_grid(uint32_t ctas) { g_bgzf_grid = ctas; }
+
+extern "C" int nvb_bgzf_compress(const uint8_t* d_in, uint64_t n_bytes, const nvb_bgzf_out* out, void* d_temp, size_t* temp_bytes, void* stream)
+{
+    return bgzf_compress_device_count(d_in, n_bytes, nullptr, out, d_temp, temp_bytes, stream);
+}
+
+extern "C" int nvb_debug_bgzf_compress_device_count(const uint8_t* d_in, const uint64_t* d_n_bytes, uint64_t max_bytes, const nvb_bgzf_out* out,
+                                                    void* d_temp, size_t* temp_bytes, void* stream)
+{
+    if (!d_n_bytes) return NVB_E_INVALID;
+    return bgzf_compress_device_count(d_in, max_bytes, d_n_bytes, out, d_temp, temp_bytes, stream);
 }

@@ -111,6 +111,13 @@ struct SymReader {
     }
 };
 
+// nvb_bgzf_compress with the byte count in device memory (bgzf.cu): d_n_bytes (NULL = n_bytes) holds the count, n_bytes is a host upper
+// bound that sizes the grids, the temp and d_block_offsets ([ceil(n_bytes / 0xFF00) + 1] entries; those past the real members repeat the
+// total).  nvb_bgzf_compress is this call with d_n_bytes = NULL.  Only its first kernel reads d_in, and only its last one writes d_out, so
+// d_out may overlap d_in (never the temp): the BAM pipeline writes the members over the records they compress
+int bgzf_compress_device_count(const uint8_t* d_in, uint64_t n_bytes, const uint64_t* d_n_bytes, const nvb_bgzf_out* out, void* d_temp,
+                               size_t* temp_bytes, void* stream);
+
 // dispatch a callable templated on <BITS,BE> from runtime (bits, big_endian)
 #define NVB_DISPATCH_STREAM(bits, be, CALL)                         \
     do {                                                            \

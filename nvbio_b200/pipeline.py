@@ -673,3 +673,125 @@ class StreamingSeedExtend:
             self.close()
         except Exception:
             pass
+
+
+class StreamingBam:
+    """Host reads in, BAM out: the BAM mode of nvb_pipeline (nvb_pipeline_create_bam, include/nvbio_b200.h).  Every batch runs mapping with
+    MAPQ and traceback (seed_extend(traceback=True, mapq=...) or seed_extend_paired(traceback=True, mapq=...)), finish_alignments,
+    bam_records and, with compress=True, bgzf_compress on the device, `depth` batches in flight; only the batch's counts and its payload
+    (exactly its byte count) come back.  The payload equals what that chain gives for the batch: the record stream, or its BGZF members,
+    which write_bam writes verbatim.
+
+    max_reads: reads per batch at most (paired: mates, mate 1 of every pair then mate 2); contigs: a ContigTable of the genome; mapq: the
+    MapqParams of the mapping call (max_read_len >= read_len); pair: PairParams for paired batches (every policy and flag, discordant pairs
+    included); quals / lengths: every submit passes base qualities / per-read lengths; max_name_bytes: bytes of names per batch (default 64
+    per name); max_ops / max_cigar / max_md: 0 = never truncate (2 * read_len + band_len, max_ops + 2, 3 * max_ops + 1, the defaults of
+    seed_extend / finish_alignments).  .slot_bytes is the device memory one slot holds."""
+
+    def __init__(self, fmi: FMIndexDevice, genome: torch.Tensor, params: SeedExtendParams, max_reads: int, read_len: int, words_per_read: int,
+                 contigs, mapq: MapqParams, pair: Optional[PairParams] = None, quals: bool = False, lengths: bool = False, compress: bool = True,
+                 depth: int = 2, bits: int = 2, hit_capacity: Optional[int] = None, max_name_bytes: Optional[int] = None,
+                 max_ops: int = 0, max_cigar: int = 0, max_md: int = 0):
+        from ._lib import PipelineBamParamsStruct
+        if params.read_quals is not None:
+            raise ValueError("StreamingBam: qualities come with every batch (quals=True), not in params.read_quals")
+        self.fmi, self.genome, self.params, self.pair, self.contigs, self.mapq = fmi, genome, params, pair, contigs, mapq   # keep alive
+        self.max_reads, self.read_len, self.wpr, self.bits, self.depth = int(max_reads), int(read_len), int(words_per_read), int(bits), int(depth)
+        self.quals, self.lengths, self.compress = bool(quals), bool(lengths), bool(compress)
+        self.n_names = self.max_reads // 2 if pair is not None else self.max_reads
+        self.max_name_bytes = int(max_name_bytes) if max_name_bytes is not None else 64 * max(self.n_names, 1)
+        if hit_capacity is None:
+            hit_capacity = 32 * self.max_reads + 1024
+        self._params_struct = params.struct()
+        self._mapq_struct = mapq.struct()
+        self._contig_dev = contigs.device(fmi.device)
+        bp = self._bam_struct = PipelineBamParamsStruct()
+        bp.mapq = C.addressof(self._mapq_struct)
+        bp.d_contig_begin, bp.n_contigs = self._contig_dev.data_ptr(), len(contigs.names)
+        bp.max_name_bytes, bp.has_quals, bp.has_lengths, bp.compress = self.max_name_bytes, int(self.quals), int(self.lengths), int(self.compress)
+        bp.max_ops, bp.max_cigar, bp.max_md = int(max_ops), int(max_cigar), int(max_md)
+        s = fmi.struct()
+        pp = pair.struct(self.max_reads // 2) if pair is not None else None
+        self._h = C.c_void_p()
+        with torch.cuda.device(fmi.device):
+            check(lib().nvb_pipeline_create_bam(C.byref(s), C.c_void_p(genome.data_ptr()), C.byref(self._params_struct),
+                                                C.byref(pp) if pp is not None else None, C.byref(bp),
+                                                C.c_uint32(self.max_reads), C.c_uint32(self.read_len), C.c_uint32(self.wpr), C.c_uint32(self.bits),
+                                                C.c_uint32(hit_capacity), C.c_uint32(self.depth), C.byref(self._h)), "nvb_pipeline_create_bam")
+        self.slot_bytes = int(lib().nvb_pipeline_slot_bytes(self._h))
+        self._keep = {}
+        self.last_device_ms = None
+
+    @staticmethod
+    def _host(a, dtype, what):
+        t = torch.as_tensor(a)
+        if t.is_cuda:
+            raise ValueError("StreamingBam.submit: %s must be in host memory" % what)
+        t = t.contiguous()
+        if t.dtype == dtype:
+            return t
+        if t.element_size() == torch.tensor([], dtype=dtype).element_size():
+            return t.view(dtype)                                  # (uint32 words / lengths: the same bits)
+        return t.to(dtype)
+
+    def submit(self, words, names, quals=None, lengths=None, n: Optional[int] = None) -> int:
+        """enqueue one batch and return its ticket.  words: int32 [n, words_per_read] in host memory (pinned = asynchronous copy); names:
+        one per read (per pair when paired), str or bytes, or the (bytes, offsets) pair of bam.pack_names; quals: uint8 [n, symbols per
+        read] (words_per_read * 32 / bits) when the stream was made with quals=True; lengths: [n] per-read lengths with lengths=True;
+        n: reads of the batch (default: all rows of words).  The host arrays stay referenced until result(ticket)."""
+        from .bam import pack_names
+        w = self._host(words, torch.int32, "words")
+        n = w.numel() // self.wpr if n is None else int(n)
+        if w.numel() < n * self.wpr:
+            raise ValueError("StreamingBam.submit: %d words for %d reads" % (w.numel(), n))
+        if isinstance(names, tuple):
+            nbytes, noff = names
+        else:
+            nbytes, noff = pack_names(names)
+        nbytes = np.ascontiguousarray(nbytes, dtype=np.uint8)
+        noff = np.ascontiguousarray(noff, dtype=np.uint32)
+        want = n // 2 if self.pair is not None else n
+        if noff.size != want + 1:
+            raise ValueError("StreamingBam.submit: %d names for %d %s" % (noff.size - 1, want, "pairs" if self.pair is not None else "reads"))
+        q = ln = None
+        if quals is not None:
+            q = self._host(quals, torch.uint8, "quals")
+            if q.numel() < n * self.wpr * (32 // self.bits):
+                raise ValueError("StreamingBam.submit: quals hold %d bytes for %d reads" % (q.numel(), n))
+        if lengths is not None:
+            ln = self._host(lengths, torch.int32, "lengths")
+            if ln.numel() < n:
+                raise ValueError("StreamingBam.submit: %d lengths for %d reads" % (ln.numel(), n))
+        t = C.c_uint32(0)
+        check(lib().nvb_pipeline_submit_bam(self._h, C.c_uint32(n), C.c_void_p(w.data_ptr()), C.c_void_p(q.data_ptr()) if q is not None else None,
+                                            C.c_void_p(ln.data_ptr()) if ln is not None else None, C.c_void_p(nbytes.ctypes.data),
+                                            C.c_void_p(noff.ctypes.data), C.byref(t)), "nvb_pipeline_submit_bam")
+        self._keep[int(t.value)] = (w, q, ln, nbytes, noff)       # asynchronous copies: keep the sources alive until result()
+        return int(t.value)
+
+    def result(self, ticket: int):
+        """wait for batch `ticket` and return its BamBatch (views of the pipeline's pinned host memory, valid until `depth` further
+        submits)"""
+        from ._lib import PipelineBamResultStruct
+        from .bam import BamBatch
+        r = PipelineBamResultStruct()
+        check(lib().nvb_pipeline_wait_bam(self._h, C.c_uint32(ticket), C.byref(r)), "nvb_pipeline_wait_bam")
+        self._keep.pop(ticket, None)
+        self.last_device_ms = float(r.device_ms)
+        nb = int(r.payload_bytes)
+        payload = _host_view(r.payload, nb, torch.uint8) if nb else torch.empty(0, dtype=torch.uint8)
+        ints = lambda ptr, k: tuple(int(v) for v in (C.c_uint32 * k).from_address(ptr))      # noqa: E731
+        return BamBatch(payload=payload, compressed=self.compress, n_records=int(r.n_records), counts=ints(r.counts, 4),
+                        n_hits=ints(r.n_hits, 3), n_rescue=ints(r.n_rescue, 2) if r.n_rescue else None, record_bytes=int(r.record_bytes),
+                        n_blocks=int(r.n_blocks), device_ms=float(r.device_ms))
+
+    def close(self):
+        if self._h:
+            lib().nvb_pipeline_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
