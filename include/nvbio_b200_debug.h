@@ -78,6 +78,11 @@ int nvb_debug_bgzf_compress_device_count(const uint8_t* d_in, const uint64_t* d_
 int nvb_debug_pipeline_bam_submit_check(const nvb_pipeline_bam_params* bam, uint32_t paired, uint32_t max_reads, uint32_t read_len,
                                         uint32_t n_reads, const uint32_t* h_read_words, const uint8_t* h_quals, const uint32_t* h_lengths,
                                         const char* h_names, const uint32_t* h_name_offsets);
+/* the slot layout of a BAM-mode pipeline, in bytes (see nvb_pipeline_create_bam): out[0] = O (the traceback ops), out[1] = R (the record
+   bound), out[2] = the finish outputs' offset in the stage region (max(O, R)), out[3] = the records' temp offset, out[4] = BGZF blocks of
+   R, out[5] = the BGZF members' capacity, out[6] = the stage region's offset in the slot, out[7] = slot bytes.  Writes min(n_out, 8)
+   entries; NVB_E_INVALID for a NULL argument or a pipeline not in BAM mode.  For tests */
+int nvb_debug_pipeline_bam_layout(const nvb_pipeline* p, uint64_t* out, uint32_t n_out);
 
 #ifdef __cplusplus
 }

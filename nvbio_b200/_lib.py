@@ -24,6 +24,7 @@ DEBUG_EXPORTS = [
     "nvb_debug_pair_format", "nvb_debug_pair_rows2", "nvb_debug_traceback_fast", "nvb_debug_pair_extra_smem",
     "nvb_debug_pipeline_path", "nvb_debug_seed_split", "nvb_debug_seed_todo", "nvb_debug_perfect_shortcut", "nvb_debug_dp_jobs", "nvb_debug_mapq_eval",
     "nvb_debug_bgzf_grid", "nvb_debug_bgzf_compress_device_count", "nvb_debug_pipeline_bam_submit_check",
+    "nvb_debug_pipeline_bam_layout",
 ]
 
 

@@ -620,6 +620,15 @@ extern "C" int nvb_pipeline_wait_bam(nvb_pipeline* p, uint32_t ticket, nvb_pipel
     return NVB_OK;
 }
 
+extern "C" int nvb_debug_pipeline_bam_layout(const nvb_pipeline* p, uint64_t* out, uint32_t n_out)
+{
+    if (!p || !p->bam || !out) return NVB_E_INVALID;
+    const uint64_t v[8] = {align_up((size_t)p->n_reads * p->max_ops, 256), p->rec_cap, p->x_fin, p->x_btemp, p->z_blocks, p->z_cap, p->o_x,
+                           p->slot_bytes};
+    for (uint32_t i = 0; i < n_out && i < 8; ++i) out[i] = v[i];
+    return NVB_OK;
+}
+
 extern "C" size_t nvb_pipeline_slot_bytes(const nvb_pipeline* p)
 {
     return p && p->bam ? p->slot_bytes : 0;
