@@ -54,7 +54,7 @@ map_seeds_kernel(const FmIndex f, const StrSet reads, const uint32_t* __restrict
     const uint32_t id = blockIdx.x * 128 + threadIdx.x;
     if (id >= n_queue) return;
     const uint32_t read_id = queue ? queue[id] : id;
-    const uint32_t begin = str_off(reads, read_id), read_len = str_len(reads, read_id), end = begin + read_len;
+    const uint32_t begin = str_off(reads, read_id), read_len = str_len(reads, read_id);
     if (read_len < g.min_read_len) { counts[read_id] = 0u; return; }           // (the reference leaves reseed[id] untouched here too)
 
     const uint32_t seed_len  = g.seed_len < read_len ? g.seed_len : read_len;
@@ -64,14 +64,16 @@ map_seeds_kernel(const FmIndex f, const StrSet reads, const uint32_t* __restrict
     uint32_t range_sum = 0u, range_count = 0u;
     SymReader<BITS, true> rd(reads.words);
 
-    for (uint32_t pos = begin + g.retry * stride; pos + seed_len <= end; pos += (seed_freq ? seed_freq : 1u)) {
+    // seed positions relative to the read: begin + read_len is 2^32 for a read ending on the stream's last symbol
+    for (uint32_t rel = g.retry * stride; rel + seed_len <= read_len; rel += (seed_freq ? seed_freq : 1u)) {
+        const uint32_t pos = begin + rel;
         // seeds with N's: BOTH mappers skip a seed with any N.  The approximate one asks util::count_occurrences(seed, len, 4, 2) -- which
         // returns the COUNT (capped at 2), not "count >= 2" -- inside an if(): one N already makes it true (mapping_inl.h:258, 343-346;
         // nvbio/basic/numbers.h:108-122), so map()'s own single-N handling is never reached from here
         uint32_t n_cnt = 0u;
         for (uint32_t i = 0; i < seed_len; ++i) n_cnt += (rd.get(pos + i) > 3u) ? 1u : 0u;
         if (n_cnt >= 1u) continue;
-        const uint32_t pos_fw = end - pos - seed_len, pos_rc = pos - begin;     // SeedHit::m_pos of the two strands (:267, :301)
+        const uint32_t pos_fw = read_len - rel - seed_len, pos_rc = rel;        // SeedHit::m_pos of the two strands (:267, :301)
         if (g.algorithm == NVB_MAP_EXACT) {
             uint32_t x, y;
             if (g.fw) {

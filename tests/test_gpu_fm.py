@@ -98,18 +98,28 @@ def _queries(rng, text, nq, lo=1, hi=30, n_frac=0.0):
     return q, offs, lens
 
 
-@pytest.mark.parametrize("bits,be", [(2, True), (2, False), (4, True), (4, False), (8, False)])
-def test_match_all_stream_formats(O, bits, be):
+@pytest.mark.parametrize("bits,be,layout", [pytest.param(b, e, "concat", id="%d-%s" % (b, e)) for b, e in
+                                             ((2, True), (2, False), (4, True), (4, False), (8, False))] +
+                                            [pytest.param(b, e, "sparse", id="%d-%s-sparse" % (b, e)) for b, e in
+                                             ((2, True), (2, False), (4, True), (4, False))])
+def test_match_all_stream_formats(O, bits, be, layout):
+    """every stream format, concatenated and as a sparse set (permuted storage order, gaps of random symbols, tests/read_layouts.py)"""
+    from tests import read_layouts as rl
     rng = np.random.default_rng(bits * 2 + be)
     text = rng.integers(0, 4, 70001).astype(np.uint8)
     idx = O.build_index(text)
     fmi = upload(idx)
     q, offs, lens = _queries(rng, text, 20000, n_frac=0.02 if bits > 2 else 0.0)
     want, _ = O.match(idx, q, offs, lens)
-    got = host_u32(nb.match(fmi, PackedStringSet.from_symbols(q, offs, lens, bits=bits, big_endian=be)))
+    if layout == "sparse":
+        reads = [q[o:o + l] for o, l in zip(offs, lens)]
+        qs = rl.build(reads, None, bits, be, "sparse", seed=bits).reads
+    else:
+        qs = PackedStringSet.from_symbols(q, offs, lens, bits=bits, big_endian=be)
+    got = host_u32(nb.match(fmi, qs))
     assert np.array_equal(got, want)
     # nvBowtie's reverse-complement seed search: forward order + complement on the forward index
-    if bits == 2:
+    if bits == 2 and layout == "concat":
         rc = np.concatenate([(3 - q[o:o + l])[::-1] for o, l in zip(offs, lens)]).astype(np.uint8)
         want_rc, _ = O.match(idx, rc, offs, lens)
         got_rc = host_u32(nb.match(fmi, PackedStringSet.from_symbols(q, offs, lens, bits=2, big_endian=be),
